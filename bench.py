@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- IMU windows/sec of the batched closed-form preintegration hot path (BASELINE.json metric).
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload v1_10k_200|v2_100k_400]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload v1_10k_200|v2_100k_400] [--dump-outputs DIR]
 
 One "step" = one pass of the hot path over one batch of synthetic IMU windows (cpi_b200/synth.py, seed 20260924).
 Default workload = BASELINE.json configs[1]: 10 000 windows x 200 samples, CPI model 1 (mean + Jacobians + covariance),
@@ -10,16 +10,21 @@ the step ends with ONE NCCL all-gather of the result records, the kernel having 
 slice of the gather buffer -- both through the product's C ABI (cpi_preintegrate_batch_sharded, cpi_b200.shard.Communicator):
 the all-gather runs on the communicator's own stream, so step i's collective overlaps step i+1's kernel (two gather buffers).  Timing: W untimed warm-up steps, then K steps between barrier + synchronize, CUDA events on
 the launching stream, max over ranks.  Inputs rotate over several distinct resident batches whose total size exceeds
-the 126 MB L2, so no step finds its samples in cache.
+the 50 MB L2 of an H100, so no step finds its samples in cache.
 
 The default run appends a "configs" array to the same JSON line: short measurements of the other BASELINE configs
 (configs[2] v2 100k x 400, configs[3] fp32 125k per GPU, configs[4] the 5k factor chain, configs[0] single window).
 
-Extra keys: roofline (dominant kernel vs the measured fp64 DFMA peak and vs measured HBM bandwidth), cpu_baseline (the
+Extra keys: roofline (dominant kernel vs the H100 SXM data-sheet fp64 / fp32 and HBM3 peaks), cpu_baseline (the
 reference's own CPU implementation timed on this box's host cores, rank 0, N = 1), e2e (same metric through the C-ABI
 host entry point with pinned HOST buffers: H2D + kernel + D2H inside the timed region), clocks, gpu_launches.
 `--impl reference` times the reference's CPU path (oracle/_ref when it was compiled, else the oracle port) on all host
 threads on a bounded sample of the same workload.
+
+`--dump-outputs DIR` writes, after the timed steps, what the last timed step computed (the records of the preintegration
+workloads, e / H1 / H2 of the factor workloads) as DIR/<name>.npy, at most 64 MB in all: larger outputs are reduced to a fixed,
+seeded sample of rows, whose indices are written as DIR/rows.npy.  Inputs depend only on the arguments, so two builds can
+be compared output for output.
 """
 import argparse
 import json
@@ -56,31 +61,37 @@ WORKLOADS = {
     "factor_1m": dict(model=1, n=1_000_000, ns=20, rate=200.0, factor=True, distinct=20_000,
                       desc="1M-factor chain, batched ImuFactorCPIv1 residual + H1 + H2 (bandwidth regime of the configs[4] kernel)"),
 }
-FFMA_PEAK_TFLOPS = 72.51   # same microbenchmark, fp32 FFMA
-DFMA_PEAK_TFLOPS = 34.17   # measured on this pool's B200 by tools/microbench.cu (profiles/microbench_r01.jsonl), burst == sustained
-# dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed `ncu --set full` captures of the CURRENT kernels
-# (profiles/r02_*.txt); None where no capture exists
-NCU_TRAFFIC = {   # dram__bytes_read.sum + dram__bytes_write.sum per launch of the committed `ncu --set full` captures (algorithmic bytes in brackets)
-    "v1_10k_200": (113.96e6 + 4.29e6, "profiles/r02_k1_tri_10k_final.txt"),                # [136.2 MB incl. 23.2 MB of records; the record writes mostly stay in L2]
-    "v2_100k_400": (2.2553e9 + 246.57e6, "profiles/r02_k2_tri_100k_final.txt"),            # [2.497 GB]
-    "v1_125k_200": (1.4247e9 + 273.82e6, "profiles/r02_k1_tri_125k.txt"),                  # [1.703 GB]
-    "v1_1m_200_fp32": (709.55e6 + 129.51e6, "profiles/r02_k1_tri_fp32_125k.txt"),          # [851.5 MB]
-}
-# sm__pipe_fp64_cycles_active.avg.pct_of_peak_sustained_elapsed of the same captures: the hardware-utilisation figure next to the contract fraction
-# (model 2 executes ~55 % of the survey's 15 kflop/sample contract -- RK4 applied directly to the consumed Discrete_J_b columns -- so its
-# contract fraction overstates the pipe utilisation; DESIGN.md section 4)
-NCU_FP64_PIPE_PCT = {"v1_10k_200": 43.8, "v2_100k_400": 49.7, "v1_125k_200": 50.6, "v1_1m_200_fp32": 21.6}
+# Roofline denominators: NVIDIA's H100 SXM data sheet (cards allowed 700 W; a card with a lower power limit clocks lower, and the
+# "clocks" key of the result line shows what the run got).  Non-tensor fp64 and fp32, since no kernel of this path uses tensor cores.
+DFMA_PEAK_TFLOPS = 34.0
+FFMA_PEAK_TFLOPS = 67.0
+HBM_PEAK_GBS = 3350.0
+PEAK_SOURCE = "H100 SXM data sheet (700 W), not measured"
+DUMP_LIMIT_BYTES = 64 << 20
 
 
-def measured_peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        return json.load(open(p)), "measured"
-    return {"hbm_gbs": 6650.0}, "fallback"
+def dump_outputs(dirname, tensors):
+    """Write {name: tensor} as dirname/<name>.npy (float32 / float64), at most DUMP_LIMIT_BYTES in all.  Tensors share their leading
+    dimension; if they do not fit, the same fixed, seeded sample of rows is selected on the device from each (only those rows are
+    copied to the host) and its indices are written as rows.npy."""
+    import torch
+    os.makedirs(dirname, exist_ok=True)
+    tensors = {k: v.detach().to(torch.float32 if v.dtype == torch.float32 else torch.float64) for k, v in tensors.items()}
+    rows = next(iter(tensors.values())).shape[0]
+    row_bytes = sum(v.numel() // max(v.shape[0], 1) * v.element_size() for v in tensors.values())
+    out = {}
+    if rows * row_bytes > DUMP_LIMIT_BYTES:
+        keep = DUMP_LIMIT_BYTES // (row_bytes + 8)
+        idx = np.sort(np.random.default_rng(20260924).choice(rows, size=keep, replace=False))
+        tensors = {k: v.index_select(0, torch.from_numpy(idx).to(v.device)) for k, v in tensors.items()}
+        out["rows"] = idx.astype(np.float64)
+    out.update({k: v.cpu().numpy() for k, v in tensors.items()})
+    for k, v in out.items():
+        np.save(os.path.join(dirname, f"{k}.npy"), np.ascontiguousarray(v))
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -147,12 +158,12 @@ def config_dict(wl, world, note=None):
     es = 4 if f32 else 8
     if wl.get("factor"):
         return {"workload": wl["desc"], "factors_per_step": n, "model": f"ImuFactorCPIv{model}", "parallelism": "rank 0 only (the solver lives there)",
-                "l2": "192 MB buffer written between timed launches (outside the event pair)"}
+                "l2": "192 MB buffer written between timed launches (outside the event pair) > 50 MB L2"}
     bytes_in = n * ns * 7 * es + n * 13 * es
     nb = 2 if bytes_in > 300e6 else min(8, max(2, int(np.ceil(300e6 / bytes_in))))
     return {"workload": wl["desc"], "windows_per_gpu": n, "samples_per_window": ns, "model": f"CpiV{model}",
             "parallelism": f"window-sharded x{world}" + (", one NCCL all-gather of records per step (overlapped with the next step's kernel)" if world > 1 else ""),
-            "l2": f"{nb} rotating resident input batches = {nb * bytes_in / 1e6:.0f} MB > 126 MB L2"}
+            "l2": f"{nb} rotating resident input batches = {nb * bytes_in / 1e6:.0f} MB > 50 MB L2"}
 
 
 def run_reference(args, wl):
@@ -197,7 +208,7 @@ def run_reference(args, wl):
     print(json.dumps(line), flush=True)
 
 
-def run_factor(args, wl, emit=True, cpu=True):
+def run_factor(args, wl, emit=True, cpu=True, dump=None):
     """configs[4]: K3 (ImuFactorCPIv1::evaluateError batched) over a 5k-keyframe chain.  HBM-write bound: 4 496 algorithmic
     bytes per factor (776 in, 3 720 out); at 5k factors the launch is ~10 us, i.e. launch-latency sized."""
     from cpi_b200 import synth
@@ -232,7 +243,7 @@ def run_factor(args, wl, emit=True, cpu=True):
     dX, dR, dL = (torch.from_numpy(a).cuda() for a in (X, rec, L))
     outs = (torch.empty((n, 15), dtype=torch.float64, device="cuda"), torch.empty((n, 225), dtype=torch.float64, device="cuda"),
             torch.empty((n, 225), dtype=torch.float64, device="cuda"))
-    flush = torch.empty(192 << 20, dtype=torch.uint8, device="cuda")      # > 126 MB L2: written between timed launches
+    flush = torch.empty(192 << 20, dtype=torch.uint8, device="cuda")      # > 50 MB L2: written between timed launches
     big = n > 100_000
     stream = torch.cuda.current_stream()
     t_settle = time.perf_counter()
@@ -249,7 +260,8 @@ def run_factor(args, wl, emit=True, cpu=True):
     torch.cuda.synchronize()
     launches = capi.launch_count() - launches0
     ms = float(np.mean([a.elapsed_time(b) for a, b in evs]))
-    peaks, how = measured_peaks()
+    if dump:
+        dump_outputs(dump, dict(zip(("e", "H1", "H2"), outs)))
     ach = 4496.0 * n / (ms * 1e-3) * 1e-9
     hX, hR, hL = (torch.from_numpy(a).pin_memory() for a in (X, rec, L))
     hE, hH1, hH2 = (torch.empty(sh, dtype=torch.float64).pin_memory() for sh in ((n, 15), (n, 225), (n, 225)))
@@ -268,9 +280,8 @@ def run_factor(args, wl, emit=True, cpu=True):
     out = {"metric": "imu_factors_per_sec", "value": n / (ms * 1e-3), "unit": "factors/s", "n_gpus": 1, "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms,
            "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f64", "data": "synthetic",
            "config": config_dict(wl, 1), "gpu_launches": int(launches), "kernel_ms": ms,
-           "roofline": {"bound": "hbm", "achieved": ach, "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": ach / peaks["hbm_gbs"],
-                        "traffic": (872.34e6 + 3662.35e6) if big else None, "traffic_source": "profiles/r02_k3_factor_1m.txt (4.496 GB algorithmic)" if big else None,
-                        "note": "4 496 algorithmic B/factor; at 5k factors (22 MB) the launch is latency-sized: 22 MB at peak would take 3.4 us; the 1M-factor workload shows the bandwidth regime"},
+           "roofline": {"bound": "hbm", "achieved": ach, "peak": HBM_PEAK_GBS, "unit": "GB/s", "frac": ach / HBM_PEAK_GBS, "peak_source": PEAK_SOURCE,
+                        "note": "4 496 algorithmic B/factor; at 5k factors (22 MB) the launch is latency-sized: 22 MB at peak would take 6.7 us; the 1M-factor workload shows the bandwidth regime"},
            "e2e": {"value": n / (e2e_ms * 1e-3), "unit": "factors/s", "ms_per_step": e2e_ms, "h2d_bytes_per_step": int((hX.numel() + hR.numel() + hL.numel()) * 8),
                    "d2h_bytes_per_step": int((hE.numel() + hH1.numel() + hH2.numel()) * 8), "api": "cpi_imu_factor_eval_batch_host",
                    "ms_per_call": [round(t, 3) for t in per_call]}}
@@ -356,7 +367,7 @@ def _pin_to_gpu_numa_node(self, torch):
 Ctx.pin_to_gpu_numa_node = _pin_to_gpu_numa_node
 
 
-def measure_preint(ctx, name, args, steps, warmup, distinct=None, e2e=True, cpu=False, clocks=True):
+def measure_preint(ctx, name, args, steps, warmup, distinct=None, e2e=True, cpu=False, clocks=True, dump=None):
     """One workload of the preintegration path on this process' GPU (all ranks call it together).  `distinct`: generate only
     that many distinct windows on the host and tile them on the device (host generation is ~0.5 ms per window; the kernel does not
     care, and the resident set still exceeds L2) -- the headline workload always uses all-distinct windows."""
@@ -447,6 +458,9 @@ def measure_preint(ctx, name, args, steps, warmup, distinct=None, e2e=True, cpu=
         dist.barrier()
     launches = capi.launch_count() - launches0
     gc.enable()
+    if dump and rank == 0:
+        last = gathers[(warmup + steps - 1) % NG]
+        dump_outputs(dump, {"records": last.reshape(world * n, rd) if world > 1 else last[0]})
     clk = sampler.stop(t0, t1) if sampler else None
     total_ms = ev0.elapsed_time(ev1)
     kern_ms = float(np.mean([a.elapsed_time(b) for a, b in kev]))
@@ -459,7 +473,6 @@ def measure_preint(ctx, name, args, steps, warmup, distinct=None, e2e=True, cpu=
     ms_per_step = total_ms / steps
     value = world * n / (ms_per_step * 1e-3)
 
-    peaks, how = measured_peaks()
     flops = wl["flops_per_sample"] * ns * n          # algorithmic flops per launch (SURVEY 8d contract)
     ach_tf = flops / (kern_ms * 1e-3) * 1e-12
     ach_gbs = wl["bytes_per_window"] * n / (kern_ms * 1e-3) * 1e-9
@@ -472,16 +485,13 @@ def measure_preint(ctx, name, args, steps, warmup, distinct=None, e2e=True, cpu=
            "config": cfg, "gpu_launches": int(launches), "kernel_ms": kern_ms, **({"exchange": exchange} if exchange else {}),
            "roofline": {"bound": "fp32+fp64 CUDA cores" if f32 else "fp64", "achieved": ach_tf, "peak": FFMA_PEAK_TFLOPS if f32 else DFMA_PEAK_TFLOPS, "unit": "TFLOP/s",
                         "frac": ach_tf / (FFMA_PEAK_TFLOPS if f32 else DFMA_PEAK_TFLOPS),
-                        "fp64_pipe_active_pct_ncu": NCU_FP64_PIPE_PCT.get(name),
-                        **({"contract_vs_executed": "model 2 executes ~8 k fp64 flop-equivalents per window-sample (ncu pipe counters; RK4 applied directly to the consumed "
-                                                    "Discrete_J_b columns, Phi never formed) against the survey's 15 k contract, so this contract fraction can exceed 1 and says "
-                                                    "nothing about the pipe: fp64_pipe_active_pct_ncu is the utilisation figure"} if model == 2 else {}),
-                        "traffic": NCU_TRAFFIC.get(name, (None, None))[0], "traffic_source": NCU_TRAFFIC.get(name, (None, None))[1],
-                        "note": "CUDA-core FMA bound, not HBM/tensor (85 flop/B); peak = DFMA / FFMA microbenchmark measured on this pool (tools/microbench.cu, "
-                                "profiles/microbench_r02.jsonl); achieved = algorithmic flops (5.8 kflop/sample v1, 15 v2; SURVEY 8d) / CUDA-event kernel time "
-                                "(the executed fp64 instruction count is below that contract for v2 -- see DESIGN.md); traffic = DRAM bytes per launch of the "
-                                "committed ncu capture of this kernel, where one exists",
-                        "hbm": {"achieved": ach_gbs, "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": ach_gbs / peaks["hbm_gbs"], "peak_source": how}},
+                        "peak_source": PEAK_SOURCE,
+                        **({"contract_vs_executed": "model 2 applies RK4 directly to the consumed Discrete_J_b columns (Phi never formed) and executes fewer "
+                                                    "fp64 operations than the survey's 15 k flop/sample contract, so this contract fraction can exceed what the pipe does"}
+                           if model == 2 else {}),
+                        "note": "CUDA-core FMA bound, not HBM/tensor (85 flop/B); achieved = algorithmic flops (5.8 kflop/sample v1, 15 v2; SURVEY 8d) / "
+                                "CUDA-event kernel time (the executed fp64 instruction count is below that contract for v2 -- see DESIGN.md)",
+                        "hbm": {"achieved": ach_gbs, "peak": HBM_PEAK_GBS, "unit": "GB/s", "frac": ach_gbs / HBM_PEAK_GBS, "peak_source": PEAK_SOURCE}},
            "clocks": clk}
 
     # ---- e2e through the C-ABI host entry point, pinned host buffers, H2D + kernel + D2H inside the timed region
@@ -564,7 +574,7 @@ def measure_preint(ctx, name, args, steps, warmup, distinct=None, e2e=True, cpu=
     return out
 
 
-def measure_single(ctx, args, wl):
+def measure_single(ctx, args, wl, steps=50, dump=None):
     """configs[0]: ONE 100-sample window -- for the GPU arm this is launch latency (one CTA, three lanes)."""
     import torch
     from cpi_b200 import preint, synth
@@ -575,11 +585,13 @@ def measure_single(ctx, args, wl):
     for _ in range(20):
         preint.preintegrate(1, dS, dL, synth.SIGMAS, 0, ns=wl["ns"], out=out, stream=stream)
     torch.cuda.synchronize()
-    evs = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(50)]
+    evs = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(steps)]
     for a, b in evs:
         a.record(stream); preint.preintegrate(1, dS, dL, synth.SIGMAS, 0, ns=wl["ns"], out=out, stream=stream); b.record(stream)
     torch.cuda.synchronize()
     ms = float(np.median([a.elapsed_time(b) for a, b in evs]))
+    if dump:
+        dump_outputs(dump, {"records": out})
     hS, hL = S.copy(), L.copy()
     for _ in range(5):
         preint.preintegrate_host(1, hS, hL, synth.SIGMAS, 0, ns=wl["ns"])
@@ -620,7 +632,13 @@ def main():
     ap.add_argument("--no-configs", action="store_true", help="skip the short runs of the other BASELINE configs appended to the default line")
     ap.add_argument("--distinct", type=int, default=0, help="generate only this many distinct windows on the host and tile them on the device (0 = all distinct)")
     ap.add_argument("--no-clocks", action="store_true", help="debug: do not poll nvidia-smi during the timed region")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy (at most 64 MB in all)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
+    if args.dump_outputs and args.impl != "ours":
+        ap.error("--dump-outputs records the GPU path (--impl ours)")
     wl = WORKLOADS[args.workload]
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     if args.impl == "reference":
@@ -629,16 +647,16 @@ def main():
     ctx = Ctx()
     if wl.get("factor"):
         if ctx.rank == 0:
-            run_factor(args, wl)
+            run_factor(args, wl, dump=args.dump_outputs)
         return
     if wl.get("single"):
         if ctx.rank == 0:
-            r = measure_single(ctx, args, wl)
-            r.update({"n_gpus": 1, "steps": 50, "warmup": 20, "ms_per_step": r["kernel_ms"], "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-                      "dtype": "f64", "data": "synthetic", "gpu_launches": 50})
+            r = measure_single(ctx, args, wl, steps=args.steps, dump=args.dump_outputs)
+            r.update({"n_gpus": 1, "steps": args.steps, "warmup": 20, "ms_per_step": r["kernel_ms"], "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
+                      "dtype": "f64", "data": "synthetic", "gpu_launches": args.steps})
             print(json.dumps(r), flush=True)
         return
-    out = measure_preint(ctx, args.workload, args, args.steps, args.warmup, distinct=args.distinct or None, e2e=True, cpu=True)
+    out = measure_preint(ctx, args.workload, args, args.steps, args.warmup, distinct=args.distinct or None, e2e=True, cpu=True, dump=args.dump_outputs)
 
     # ---- the other BASELINE configs, short runs, appended to the default line so that the driver's record carries them
     if args.workload == "v1_10k_200" and not args.no_configs:

@@ -1,6 +1,6 @@
-"""cpi_b200 -- batched closed-form IMU preintegration (rpng/cpi hot path) on B200.
+"""cpi_b200 -- batched closed-form IMU preintegration (rpng/cpi hot path) on H100.
 
-Everything computes in ``libcpi_b200.so`` (CUDA, sm_100a; C ABI in ``include/cpi_b200.h``); there is no CPU fallback.
+Everything computes in ``libcpi_b200.so`` (CUDA, sm_90a; C ABI in ``include/cpi_b200.h``); there is no CPU fallback.
 Submodules are imported lazily so that ``import cpi_b200`` works on a box without the built extension:
 
     cpi_b200.capi      ctypes binding of the C ABI (``load()`` raises if the library is missing)

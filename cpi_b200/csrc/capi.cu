@@ -44,9 +44,10 @@ int device_info(DevInfo& d) {
     static DevInfo cache[64];
     std::lock_guard<std::mutex> lk(mu);
     if (dev < 64 && cache[dev].ok) { d = cache[dev]; return CPI_OK; }
-    int major = 0;
+    int major = 0, minor = 0;
     CU(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
-    if (major != 10) return fail(CPI_ENODEVICE, "device %d is sm_%d*, this library is built for sm_100a (B200) only", dev, major * 10);
+    CU(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev));
+    if (major != 9 || minor != 0) return fail(CPI_ENODEVICE, "device %d is sm_%d%d, this library is built for sm_90a (H100) only", dev, major, minor);
     CU(cudaDeviceGetAttribute(&d.sms, cudaDevAttrMultiProcessorCount, dev));
     CU(cudaDeviceGetAttribute(&d.max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
     d.ok = true;
@@ -133,7 +134,7 @@ int preintegrate_dev(int model, int dtype, int64_t n_windows, const int64_t* sam
 extern "C" {
 
 const char* cpi_last_error(void) { return g_err.c_str(); }
-const char* cpi_version(void) { return "cpi_b200 0.2 (sm_100a)"; }
+const char* cpi_version(void) { return "cpi_b200 0.2 (sm_90a)"; }
 int cpi_record_doubles(int model) { return model == 1 ? CPI_REC_V1_DOUBLES : (model == 2 ? CPI_REC_V2_DOUBLES : CPI_EINVAL); }
 int64_t cpi_launch_count(void) { return g_launches.load(); }
 
@@ -143,8 +144,9 @@ int cpi_device_count(void) {
     if (e != cudaSuccess) return fail(CPI_ENODEVICE, "cudaGetDeviceCount: %s", cudaGetErrorString(e));
     int ok = 0;
     for (int i = 0; i < n; i++) {
-        int major = 0;
-        if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, i) == cudaSuccess && major == 10) ok++;
+        int major = 0, minor = 0;
+        if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, i) == cudaSuccess &&
+            cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, i) == cudaSuccess && major == 9 && minor == 0) ok++;
     }
     return ok;
 }
@@ -194,9 +196,9 @@ int cpi_preintegrate_batch_host(int model, int dtype, int64_t n_windows, const i
     // many small chunks.  The lane-per-window kernels (imu_avg / analytic modes) are launched with the windows-per-block the WHOLE
     // batch would use, so that a chunk occupies only its share of the SMs.
     //
-    // Wavefront schedule (uniform layout, fp64, default modes).  A window is a chain of ns DEPENDENT samples (~3.7 us each on B200,
-    // whatever the occupancy), so a chunk that travels whole finishes ~ns x 3.7 us after it arrived, however small it is: 0.74 ms
-    // behind the last byte of H2D for 200-sample windows, a quarter of the PCIe time of the whole 10k-window batch.  Instead the batch
+    // Wavefront schedule (uniform layout, fp64, default modes).  A window is a chain of ns DEPENDENT samples (a few microseconds each,
+    // whatever the occupancy), so a chunk that travels whole finishes ~ns sample latencies after it arrived, however small it is: for
+    // 200-sample windows a sizeable fraction of the PCIe time of the whole 10k-window batch.  Instead the batch
     // is cut into G window groups x S sample segments, and the (group, segment) tiles are sent along ANTI-DIAGONALS: tile (g, s) is a
     // strided copy (cudaMemcpy2DAsync: rows = windows of the group, row = samples [s ns/S, (s+1) ns/S)) followed, on the group's stream,
     // by a CONTINUATION kernel over the group (cpi_preintegrate_batch_continue).  Every group's chain then runs WHILE its samples
@@ -218,7 +220,7 @@ int cpi_preintegrate_batch_host(int model, int dtype, int64_t n_windows, const i
     const int wpb = (int)(need < cap ? (need < 1 ? 1 : need) : cap);
     const int64_t blocks = (n_windows + wpb - 1) / wpb;
     // wavefront geometry: the first wave_H % of the windows travel as whole-window chunks, the rest as G groups x S segments.
-    // Defaults (measured on B200, tools/host_pipeline_probe.py, profiles/r02_host_pipeline_probe.json): every copy costs ~3.5 us of dead
+    // Defaults (tools/host_pipeline_probe.py compares geometries): every copy costs a few microseconds of dead
     // time on the copy engine, so few large tiles beat a fine wavefront -- ONE group of 4 segments, sized so that its transfer lasts
     // about as long as its sample chain (ns x ~4.6 us incl. the per-segment record reload, x ~50 GB/s of PCIe; model 2 chains are
     // ~1.5x longer), behind whole-window chunks for everything before it.

@@ -1,4 +1,4 @@
-// Shared device helpers for the CPI kernels (sm_100a).  All small-matrix code works on register arrays with
+// Shared device helpers for the CPI kernels (sm_90a).  All small-matrix code works on register arrays with
 // compile-time indices so that nothing is spilled to local memory by dynamic indexing.
 #pragma once
 #include <cuda_runtime.h>

@@ -1,10 +1,9 @@
 // K1 / K2: batched closed-form IMU preintegration, CpiV1::feed_IMU (cpi/CpiV1.h:62-361) and CpiV2::feed_IMU
-// (cpi/CpiV2.h:84-467) of rpng/cpi, re-designed for B200 (sm_100a).  See DESIGN.md for the derivation.
+// (cpi/CpiV2.h:84-467) of rpng/cpi, for H100 (sm_90a).  See DESIGN.md for the derivation.
 //
-// Mapping: ONE LANE PER WINDOW, a warp advances 32 independent windows in lock-step.  Measured on B200
-// (profiles/microbench_r01.jsonl): DFMA peak 34.2 TFLOP/s and a single warp per SMSP already reaches 90 % of it at
-// ILP >= 4, whereas every cross-lane double costs as much as 4 DFMA (SHFL / LDS bandwidth is 16 doubles/clk/SM vs 64
-// DFMA/clk/SM).  So the window recurrence is kept free of cross-lane traffic; the per-window state that does not fit
+// Mapping: ONE LANE PER WINDOW, a warp advances 32 independent windows in lock-step.  A single warp per SMSP keeps the
+// DFMA pipe busy at ILP >= 4, whereas every cross-lane double costs as much as 4 DFMA (SHFL / LDS bandwidth is 16
+// doubles/clk/SM vs 64 DFMA/clk/SM; tools/microbench.cu measures both).  So the window recurrence is kept free of cross-lane traffic; the per-window state that does not fit
 // the register file -- the 90 unique non-trivial entries of the 15x15 covariance (ping-pong copy), the RK4 stage values
 // other blocks depend on and the Jacobian state -- lives in shared memory in [entry][window] order (conflict-free:
 // lane == window; base + immediate addressing because the window stride is a compile-time constant).
@@ -1063,8 +1062,8 @@ __global__ void __launch_bounds__(128, 1) k_preintegrate(const PreintParams p) {
 //     FRONT warp: sample fetch (TMA), rotation chain, closed-form means, analytic bias Jacobians      (~2.1 k instr/sample)
 //     BACK  warp: the covariance RK4 cascade                                                          (~3.4 k instr/sample)
 // FRONT hands (R_mid, R_new, w_hat, a_hat, dt) to BACK through a double-buffered shared-memory mailbox guarded by
-// full/empty mbarriers per warp pair.  Small batches are single-warp-latency bound (148 windows take 85 % of the time of
-// 10 000), so shortening the per-warp chain by ~1.6x is the lever there; large batches gain from twice as many resident
+// full/empty mbarriers per warp pair.  Small batches are single-warp-latency bound (one window per SM takes most of the time
+// of 10 000), so shortening the per-warp chain by ~1.6x is the lever there; large batches gain from twice as many resident
 // warps for the same tile footprint.
 enum : int { H_RM = 0, H_R1 = 9, H_W = 18, H_A_ = 21, H_DT = 24, NHAND = 26 };
 template <class T> struct TileWS {
@@ -1308,7 +1307,7 @@ cudaError_t preint_launch(int model, int dtype, int flags, const PreintParams& p
     }
     if (p.init) return cudaErrorNotSupported;      // continuation exists for the default (tri-lane) modes only
     // fp32 tiles are small enough that the fused kernel holds 128 windows (4 full warps) per SM: for batches beyond one wave
-    // of the warp-specialised kernel it is the faster one (measured: 14.2 vs 13.1 M windows/s on 125k x 200)
+    // of the warp-specialised kernel it is the faster one
     const bool ws_pays = dtype != 32 || p.n_windows <= (int64_t)num_sms * TileWS<float>::S;
     if (model == 1 && !(flags & CPI_FLAG_IMU_AVG) && !force_fused && ws_pays && p.n_windows < (int64_t)2147483647) {
         if (launches) *launches = 1;

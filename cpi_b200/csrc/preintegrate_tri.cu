@@ -20,8 +20,8 @@
 // operations per sample of the lane-per-window layout, and the covariance tile no longer lives in shared memory at
 // all (residency is register-bound, not smem-bound).  The four RK4 stages are the reference's (CpiV1.h:272-353).
 //
-// Measured on B200 (profiles/microbench_r02.jsonl): SHFL.b32 = 1 warp-instr/clk/SM, LDS.64 = 1 warp-instr/clk/SM on the
-// same MIO pipe, DFMA = 2 warp-instr/clk/SM, and SHFL overlaps fully with DFMA.
+// Issue rates the mapping rests on (tools/microbench.cu): SHFL.b32 = 1 warp-instr/clk/SM, LDS.64 = 1 warp-instr/clk/SM on the
+// same MIO pipe, DFMA = 2 warp-instr/clk/SM, and SHFL overlaps with DFMA.
 #include <cstdlib>
 #include "cpi_common.cuh"
 #include "cpi_kernels.h"
@@ -31,7 +31,7 @@ namespace cpi {
 
 constexpr int TRI_WPW = 10;                 // windows per warp (lanes 30, 31 idle)
 // CTA = ONE warp = ten windows.  Nothing in the kernel is shared between warps, so one-warp CTAs cost nothing and buy (a) even
-// distribution by the hardware block scheduler (10 000 windows = 1 000 CTAs over 148 SMs: 6 or 7 per SM, one wave), (b) kernels of
+// distribution by the hardware block scheduler (10 000 windows = 1 000 CTAs over 132 SMs: 7 or 8 per SM, one wave), (b) kernels of
 // different streams co-residing on an SM, which is what lets the host entry point pipeline a batch in many small chunks, and (c) a
 // finer tail on multi-wave batches.  Up to 8 CTAs per SM: 255 registers x 32 lanes x 8 = the register file; shared memory per CTA is
 // kept under 220 KB / 8 for every instantiation (model 1 fp64: 21 KB, model 2 fp64: 24 KB).

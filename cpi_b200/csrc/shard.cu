@@ -10,9 +10,8 @@
 //        NVLink with the COPY ENGINES (cudaMemcpyAsync into CUDA-IPC mappings of the peers' buffers), bracketed by two one-element
 //        NCCL all-reduces that act as barriers ("every rank has released this buffer" before, "every slice has landed" after).
 //        No SM is involved in moving the records.  This matters because the preintegration kernel of configs[1] is a ONE-WAVE
-//        kernel (1 000 one-warp CTAs on 1 184 slots): an NCCL all-gather kernel running beside it takes whole SMs (one NCCL CTA
-//        ~ 7 of an SM's 8 slots), pushes part of the grid into a second wave and costs more than it hides (measured at N = 4:
-//        0.75 -> 0.89 ms per step).
+//        kernel (1 000 one-warp CTAs on the 1 056 slots of 132 SMs): an NCCL all-gather kernel running beside it takes whole SMs
+//        (one NCCL CTA ~ 7 of an SM's 8 slots) and pushes part of the grid into a second wave.
 //   NCCL (unregistered buffers, or CUDA IPC unavailable for them): ncclAllGather on the communicator's stream, with the
 //        communicator limited to CPI_B200_NCCL_MAX_CTAS (default 16) CTAs so that the kernel beside it still fits one wave.
 //

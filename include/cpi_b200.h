@@ -1,5 +1,5 @@
 /*
- * cpi_b200.h -- C ABI of libcpi_b200.so: batched closed-form IMU preintegration (CPI) on B200 (sm_100a).
+ * cpi_b200.h -- C ABI of libcpi_b200.so: batched closed-form IMU preintegration (CPI) on H100 (sm_90a).
  *
  * This is the drop-in boundary for the ONE hot path of rpng/cpi (reference tree paths are relative to
  * /root/reference/cpi_compare/src):
@@ -79,7 +79,7 @@ extern "C" {
 #define CPI_OK          0
 #define CPI_EINVAL     -1   /* bad argument (NULL pointer, unknown model/dtype, negative count) */
 #define CPI_ECUDA      -2   /* a CUDA runtime call failed; see cpi_last_error() */
-#define CPI_ENODEVICE  -3   /* no CUDA device / not an sm_100 device */
+#define CPI_ENODEVICE  -3   /* no CUDA device / not an sm_90 device */
 #define CPI_ENOMEM     -4
 
 /* ---- preintegration ---------------------------------------------------------------------------------------------- */
@@ -291,7 +291,7 @@ int cpi_comm_wait(cpi_comm* comm, void* stream);
 const char* cpi_last_error(void);
 const char* cpi_version(void);
 int cpi_record_doubles(int model);          /* 290 or 308; CPI_EINVAL otherwise */
-int cpi_device_count(void);                 /* number of usable sm_100 devices, or negative error */
+int cpi_device_count(void);                 /* number of usable sm_90 devices, or negative error */
 /* number of kernel launches issued by this library on the calling process since load (for bench.py's gpu_launches) */
 int64_t cpi_launch_count(void);
 

@@ -2,7 +2,7 @@
 
   * ``Oracle()``    -> oracle/liboracle.so       (plain-C restatement, oracle/cpi_oracle.c)
   * ``Reference()`` -> oracle/_ref/libcpi_ref.so (the UNMODIFIED reference compiled in place by oracle/ref_shim.cpp;
-                       built only where /root/reference exists, travels prebuilt to the GPU box)
+                       built only where an rpng/cpi checkout is given: make -C oracle ref REF=...)
 
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / ``--impl reference`` leg may import this module.
 The product package ``cpi_b200`` never does.  Both classes expose the same numpy-level methods.

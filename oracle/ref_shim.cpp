@@ -1,9 +1,9 @@
 // TEST INFRASTRUCTURE ONLY -- never linked into or called by the product path (cpi_b200/).
 //
-// C-ABI wrapper around the UNMODIFIED reference, compiled in place from /root/reference (no source is copied):
+// C-ABI wrapper around the UNMODIFIED reference, compiled in place from an rpng/cpi checkout (make ref REF=...; no source is copied):
 //   cpi_compare/src/cpi/{CpiBase,CpiV1,CpiV2}.h, utils/quat_ops.h        (header-only, Eigen 3.2.10 vendored in the reference)
 //   cpi_compare/src/gtsam/{ImuFactorCPIv1,ImuFactorCPIv2,JPLNavState}.cpp (against oracle/gtsam_stub/, see stub_core.h)
-// Output: oracle/_ref/libcpi_ref.so (git-ignored; travels to the GPU box with the snapshot).
+// Output: oracle/_ref/libcpi_ref.so (git-ignored).
 // Uses the batch layouts of include/cpi_b200.h so that tests can compare buffers directly.
 //
 // The driving loop mirrors GraphSolver::createimufactor_cpi_v1/_v2 (solvers/GraphSolver_IMU.cpp:43-75, 97-130):

@@ -10,7 +10,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (B200); run with -m gpu")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (H100); run with -m gpu")
 
 
 @pytest.fixture(scope="session")
@@ -27,7 +27,7 @@ def reference():
     """The unmodified reference compiled in place (oracle/_ref/libcpi_ref.so); prebuilt, may be absent."""
     from oracle import oracle as om
     if not om.Reference.available():
-        pytest.skip("oracle/_ref/libcpi_ref.so not built (needs /root/reference at build time)")
+        pytest.skip("oracle/_ref/libcpi_ref.so not built (needs the rpng/cpi checkout at CPI_REFERENCE, by default /root/reference)")
     return om.Reference()
 
 

@@ -1,6 +1,6 @@
 // Test driver for include/cpi_b200/CpiGpu.h: runs the SAME feed loop (solvers/GraphSolver_IMU.cpp:43-75 shape) through the
-// reference's CpiV1/CpiV2 (compiled in place from /root/reference) and through CpiV1Gpu/CpiV2Gpu, and compares the public
-// fields.  Built by __graft_entry__.build() only where the reference tree exists; the binary travels to the GPU box.
+// reference's CpiV1/CpiV2 (compiled in place from an rpng/cpi checkout) and through CpiV1Gpu/CpiV2Gpu, and compares the public
+// fields.  Built only where an rpng/cpi checkout is given (make -C tests/cpp REF=...).
 #include <cmath>
 #include <cstdio>
 #include <random>

@@ -1,9 +1,9 @@
 // Test driver for include/cpi_b200/ImuFactorGpu.h: the reference's own ImuFactorCPIv1 / ImuFactorCPIv2 (gtsam/ImuFactorCPIv1.cpp,
-// ImuFactorCPIv2.cpp, JPLNavState.cpp compiled UNMODIFIED, in place from /root/reference, against oracle/gtsam_stub) and the drop-in
+// ImuFactorCPIv2.cpp, JPLNavState.cpp compiled UNMODIFIED, in place from an rpng/cpi checkout, against oracle/gtsam_stub) and the drop-in
 // ImuFactorCPIv1Gpu / ImuFactorCPIv2Gpu live in ONE binary, are constructed from the same arguments (the public fields of a
 // reference CpiV1 / CpiV2 after its feed loop, exactly as GraphSolver_IMU.cpp:74-75 / :129-130 does) and evaluated on the same
 // states; e, H1, H2 are compared per factor, once through the per-factor path and once through the graph-level batch.
-// Built by __graft_entry__.build() only where the reference tree exists; the binary travels to the GPU box.
+// Built only where an rpng/cpi checkout is given (make -C tests/cpp REF=...).
 #include <cmath>
 #include <cstdio>
 #include <map>

@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """Generate the committed golden fixtures from the UNMODIFIED reference (oracle/_ref/libcpi_ref.so).
 
-Run in the build container (needs /root/reference for the datasets and for building oracle/_ref):
-    python tests/golden/make_golden.py
+Needs the rpng/cpi checkout (CPI_REFERENCE, by default /root/reference) for the datasets and for building oracle/_ref:
+    make -C oracle ref && python tests/golden/make_golden.py
 Writes
     tests/golden/imu_200hz_run00_head.dat   first 700 lines of GAZEBO_FREQ_200/rawdata_00/imu_data_meas.dat (input fixture)
     tests/golden/preint_golden.npz          inputs + reference CpiV1/CpiV2 records for every case below
@@ -19,7 +19,7 @@ sys.path.insert(0, ROOT)
 from oracle.oracle import Reference, FLAG_IMU_AVG, FLAG_ANALYTIC_JACOBIANS  # noqa: E402
 from cpi_b200 import synth  # noqa: E402
 
-REF = "/root/reference/cpi_simulation"
+REF = os.path.join(os.environ.get("CPI_REFERENCE", "/root/reference"), "cpi_simulation")
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 
@@ -114,11 +114,10 @@ def main():
                 S, off = c["samples"], c["offsets"]
                 if flags & FLAG_IMU_AVG:
                     # imu_avg consumes one trailing entry per window: re-cut so that every window keeps >= 0 steps
+                    # (not stored: tests/parity.py:imu_avg_inputs rebuilds this layout)
                     wins = [S[off[i]:off[i + 1]] for i in range(n)]
                     wins = [np.concatenate([w_, w_[-1:]]) if len(w_) else w_ for w_ in wins]
                     S, off = csr(wins)
-                    out[f"{name}/samples_avg"] = S
-                    out[f"{name}/offsets_avg"] = off
                 out[f"{name}/records_m{model}_f{flags}"] = R.preintegrate(model, S, c["lin"], synth.SIGMAS, flags, offsets=off)
     out["sigmas"] = synth.SIGMAS
     out["cam200_init300/samples"] = extra_init["samples"]; out["cam200_init300/offsets"] = extra_init["offsets"]

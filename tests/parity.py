@@ -22,6 +22,17 @@ def window_band(samples, offsets, lin):
     return out
 
 
+def imu_avg_inputs(samples, offsets):
+    """The imu_avg form of a CSR batch: imu_avg consumes one trailing entry per window, so every non-empty window repeats its last
+    entry (tests/golden/make_golden.py ran the reference on exactly this layout)."""
+    n = len(offsets) - 1
+    wins = [samples[offsets[i]:offsets[i + 1]] for i in range(n)]
+    wins = [np.concatenate([w, w[-1:]]) if len(w) else w for w in wins]
+    off = np.zeros(n + 1, dtype=np.int64)
+    off[1:] = np.cumsum([len(w) for w in wins])
+    return np.ascontiguousarray(np.concatenate(wins).reshape(-1, 7)), off
+
+
 def rel(a, b, floor=1e-300):
     return float(np.linalg.norm(a - b) / max(np.linalg.norm(b), floor))
 

@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on a B200): the CUDA path, called through the C ABI, against
+"""GPU parity tests (run with -m gpu on an H100): the CUDA path, called through the C ABI, against
  (1) the committed golden vectors produced by the unmodified reference,
  (2) the plain-C oracle on seeded inputs,
  (3) the compiled reference itself when oracle/_ref/libcpi_ref.so travelled with the snapshot,
@@ -7,23 +7,22 @@ import numpy as np
 import pytest
 
 from cpi_b200 import synth
-from parity import compare_records, window_band
+from parity import compare_records, imu_avg_inputs, window_band
 
 pytestmark = pytest.mark.gpu
 CASES = ("cam200", "real200", "real100", "real400", "synth200", "edge")
 MODES = [(1, 0), (1, 1), (2, 0), (2, 1), (2, 2), (2, 3)]
-# fp32-storage variant (dtype 32): no fp32 reference exists; gates = 2x the worst error observed on B200 against the fp64 oracle on the
+# fp32-storage variant (dtype 32): no fp32 reference exists; gates = 2x the worst error observed against the fp64 oracle on the
 # same float-rounded inputs (DESIGN.md section 3a).  R/alpha/beta/J/H: fp64 arithmetic, float output rounding; P: fp32 RK4.
 FP32_GATES = {1: dict(R=1.5e-7, alpha=1.5e-7, beta=1.5e-7, J_q=1.5e-7, J_a=1.5e-7, J_b=1.5e-7, H_a=1.5e-7, H_b=1.5e-7, P=6e-7, P_block=6e-7),
               2: dict(R=1.5e-7, alpha=1.5e-7, beta=1.5e-7, J_q=1.5e-7, J_a=1.5e-7, J_b=1.5e-7, H_a=1.5e-7, H_b=1.5e-7, O_a=1.5e-7, O_b=1.5e-7, P=1e-6, P_block=1e-6)}
-# observed on B200 (profiles/r02_parity_vs_reference.json), model 1: R 6.4e-8, alpha/beta 5.1e-8, J/H 5.5e-8, P 2.3e-7, worst 3x3 block of P 2.9e-7:
 # with the state accumulated in fp64 even the fp32 variant meets the north_star's 1e-6 on P, block-wise.
 
 
 def _inputs(G, name, flags):
-    avg = bool(flags & 1)
-    S = G[f"{name}/samples_avg"] if avg else G[f"{name}/samples"]
-    off = G[f"{name}/offsets_avg"] if avg else G[f"{name}/offsets"]
+    S, off = G[f"{name}/samples"], G[f"{name}/offsets"]
+    if flags & 1:
+        S, off = imu_avg_inputs(S, off)
     return S, off, G[f"{name}/lin"]
 
 
@@ -45,7 +44,7 @@ def test_cuda_matches_oracle_seeded(cuda, oracle, model, flags):
     """Device-pointer entry point on the bench distribution (incl. forced small_w / zero-w / dt=0 windows)."""
     from cpi_b200 import preint
     torch = cuda
-    n, ns = 2100, 60                       # > 148 windows per SM-wave boundary effects: ragged last block
+    n, ns = 2100, 60                       # > 132 windows per SM-wave boundary effects: ragged last block
     S, L = synth.make_windows(n, ns, rate=200.0, first_window=0, imu_avg=bool(flags & 1))
     got = preint.preintegrate(model, torch.from_numpy(S).cuda(), torch.from_numpy(L).cuda(), synth.SIGMAS, flags, ns=ns)
     torch.cuda.synchronize()
@@ -291,7 +290,7 @@ def test_chunk_pipelined_host_path_is_bitwise_the_single_launch(cuda, model, dty
 @pytest.mark.parametrize("model", [1, 2])
 def test_factor_hessian_against_dense_cpu_solve(cuda, model):
     """Information-form linearisation (SURVEY 8f rank 1).  GTSAM is not in the reference tree: PARITY UNPINNED, validated against a
-    dense numpy solve (Jacobi-scaled: cond(P_meas) ~ 1e7 but cond(D P D) ~ 25).  Observed on B200: 2e-15; gate 1e-10 per block."""
+    dense numpy solve (Jacobi-scaled: cond(P_meas) ~ 1e7 but cond(D P D) ~ 25).  Gate 1e-10 per block."""
     from cpi_b200 import preint, factor
     n = 300
     S, L = synth.make_windows(n, 60, rate=200.0, first_window=31337, special=False)

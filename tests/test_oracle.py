@@ -4,16 +4,16 @@ import numpy as np
 import pytest
 
 from cpi_b200 import synth
-from parity import compare_records, window_band
+from parity import compare_records, imu_avg_inputs, window_band
 
 CASES = ("cam200", "real200", "real100", "real400", "synth200", "edge")
 TIGHT = dict(tol_mean=1e-12, tol_P=1e-12, tol_J=1e-11, tol_Ja_band=1e-9)
 
 
 def _inputs(G, name, flags):
-    avg = bool(flags & 1)
-    S = G[f"{name}/samples_avg"] if avg else G[f"{name}/samples"]
-    off = G[f"{name}/offsets_avg"] if avg else G[f"{name}/offsets"]
+    S, off = G[f"{name}/samples"], G[f"{name}/offsets"]
+    if flags & 1:
+        S, off = imu_avg_inputs(S, off)
     return S, off, G[f"{name}/lin"]
 
 

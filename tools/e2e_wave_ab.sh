@@ -1,5 +1,5 @@
 #!/bin/bash
-# e2e A/B of the host entry's tail handling (run on the GPU box from the repo root)
+# e2e A/B of the host entry's tail handling (run from the repo root)
 B="python bench.py --no-cpu-baseline --no-configs --no-clocks --steps 50 --warmup 3"
 for spec in "0,0" "14,8" "8,8" "24,8" "14,4" "14,16" "32,8" "0,0" "14,8"; do
   echo "== wave G,S $spec"

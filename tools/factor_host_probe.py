@@ -1,5 +1,5 @@
 import sys, os, time, ctypes
-sys.path.insert(0, "/root/repo")
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
 from cpi_b200 import capi, synth, preint, factor
 lib = capi.load()

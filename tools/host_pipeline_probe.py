@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """In-process A/B of the host entry point's schedules (CPI_B200_HOST_WAVE = "G,S[,H]") on BASELINE configs[1], next to the raw PCIe
-numbers of the box: one plain pinned H2D of the same bytes, and the same bytes as strided 2-D tile copies.  Run on the GPU box:
-    python tools/host_pipeline_probe.py > gpurun_out/host_probe.json"""
+numbers of the box: one plain pinned H2D of the same bytes, and the same bytes as strided 2-D tile copies:
+    python tools/host_pipeline_probe.py > host_probe.json"""
 import ctypes, json, os, statistics, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np

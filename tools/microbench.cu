@@ -1,5 +1,5 @@
-// Micro-benchmarks that size the design of the preintegration kernels on B200 (sm_100a).
-// Not part of the product path.  Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o microbench microbench.cu
+// Micro-benchmarks that size the design of the preintegration kernels on H100 (sm_90a).
+// Not part of the product path.  Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o microbench microbench.cu
 //
 // Measures (all on the current device, CUDA-event timed, after warm-up):
 //   1. fp64 DFMA peak (all SMs saturated)           -> roofline denominator for K1/K2 ("of measured")
@@ -154,7 +154,7 @@ int main() {
     printf("{\"device\": \"%s\", \"sms\": %d, \"clock_khz_attr\": %d}\n", p.name, sms, clk_khz);
     double* out; CK(cudaMalloc(&out, sizeof(double) * 1024 * 1024 * 4));
 
-    // 1. DFMA peak: 148*8 blocks x 256 threads, ILP 8
+    // 1. DFMA peak: 8 blocks per SM x 256 threads, ILP 8
     {
         const int iters = 20000, blocks = sms * 8, thr = 256;
         float ms = time_ms([&] { k_dfma<8><<<blocks, thr>>>(out, iters, 1.0000001, 1e-9); });

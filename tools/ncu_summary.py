@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Summarise an .ncu-rep (captured on the GPU box with `ncu --set full`) into a small text file for profiles/.
-usage: python tools/ncu_summary.py gpurun_out/prof.ncu-rep profiles/out.txt ["note"]"""
+"""Summarise an .ncu-rep (captured with `ncu --set full`) into a small text file.
+usage: python tools/ncu_summary.py prof.ncu-rep out.txt ["note"]"""
 import csv, io, subprocess, sys
 
 KEYS = ["gpu__time_duration.sum", "launch__grid_size", "launch__block_size", "launch__registers_per_thread",

@@ -1,12 +1,11 @@
 #!/usr/bin/env python
 """Pack the reference's shipped Monte-Carlo runs into compact .npz files for the dataset replay (tools/replay_datasets.py).
 
-    python tools/pack_datasets.py            (needs /root/reference; writes tests/golden/_datasets/replay_<rate>.npz)
+    python tools/pack_datasets.py            (needs the rpng/cpi checkout, CPI_REFERENCE, by default /root/reference; writes tests/golden/_datasets/replay_<rate>.npz)
 
 Only what the preintegration path consumes is kept: per run the IMU stream of imu_data_meas.dat ("wx wy wz ax ay az <unused> t_ms",
 sim/SimParser.h:148-175) and the camera stamps of camera_data_meas.dat (last column, ms).  The output directory is git-ignored
-(it is ~100 MB of the reference's data, not source of this repository) but NOT gpurun-ignored, so it travels to the GPU box for the
-one replay call and can be deleted afterwards."""
+(it is ~100 MB of the reference's data, not source of this repository)."""
 import os
 import sys
 

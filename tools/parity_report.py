@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Parity report at scale: the CUDA path (through the C ABI) against the UNMODIFIED reference compiled in place
 (oracle/_ref/libcpi_ref.so, all host threads) on the bench distribution.  Writes one JSON object to stdout.
-Run on the GPU box:  python tools/parity_report.py > gpurun_out/parity_r02.json"""
+Run:  python tools/parity_report.py > parity.json"""
 import json, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))

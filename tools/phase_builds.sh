@@ -8,7 +8,7 @@ cd "$(dirname "$0")/../cpi_b200/csrc"
 make -s
 for v in LOAD COV; do
   lv=$(echo $v | tr A-Z a-z)
-  nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -lineinfo -Xcompiler -fPIC --expt-relaxed-constexpr -DCPI_TRI_PHASE_$v -c -o /tmp/tri_phase_$lv.o preintegrate_tri.cu
-  nvcc -gencode arch=compute_100a,code=sm_100a -shared -o ../libcpi_b200_phase_$lv.so capi.o preintegrate.o /tmp/tri_phase_$lv.o factor.o shard.o windows.o solve.o -lcudart -ldl
+  nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -Xcompiler -fPIC --expt-relaxed-constexpr -DCPI_TRI_PHASE_$v -c -o /tmp/tri_phase_$lv.o preintegrate_tri.cu
+  nvcc -gencode arch=compute_90a,code=sm_90a -shared -o ../libcpi_b200_phase_$lv.so capi.o preintegrate.o /tmp/tri_phase_$lv.o factor.o shard.o windows.o solve.o -lcudart -ldl
 done
 ls -la ../libcpi_b200_phase_*.so

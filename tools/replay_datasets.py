@@ -3,10 +3,10 @@
 cpi_cut_windows (host window builder) + K1 / K2 on the GPU -- and compare EVERY window with the unmodified reference driven by its own
 driver loop (oracle/ref_shim.cpp:ref_replay_run).  SURVEY.md 8f rank 3.
 
-    python tools/pack_datasets.py                       (here, where /root/reference exists)
-    gpurun -- python tools/replay_datasets.py           (GPU box: needs tests/golden/_datasets/*.npz and oracle/_ref/libcpi_ref.so)
+    python tools/pack_datasets.py                       (where an rpng/cpi checkout exists)
+    python tools/replay_datasets.py                     (GPU: needs tests/golden/_datasets/*.npz and oracle/_ref/libcpi_ref.so)
 
-Writes gpurun_out/dataset_replay.json: per rate and model the number of windows, whether the cut is bit-identical to the
+Prints a JSON report on its last line: per rate and model the number of windows, whether the cut is bit-identical to the
 reference's, the worst error per record field, and the windows/s of the real-data batch.  The linearisation points (biases, q_k,
 gravity) come from a seeded generator: the reference takes them from its state estimate, which needs the vision factors (GTSAM)."""
 import json
@@ -33,7 +33,7 @@ def main():
     for rate in (100, 200, 400):
         path = os.path.join(ROOT, "tests", "golden", "_datasets", f"replay_{rate}.npz")
         if not os.path.exists(path):
-            print("missing", path); continue
+            print("missing", path, file=sys.stderr); continue
         D = np.load(path)
         runs = sorted({k.split("/")[0] for k in D.files})
         Ss, offs, lins, refs = [], [0], [], {1: [], 2: []}
@@ -77,11 +77,9 @@ def main():
             host = preint.preintegrate_host(model, S, L, synth.SIGMAS, 0, offsets=off)
             entry[f"model{model}"] = {"worst": {k: float(f"{v:.3e}") for k, v in worst.items()}, "kernel_ms": ms, "windows_per_s": n / (ms * 1e-3),
                                       "host_entry_bitwise_equal": bool(np.array_equal(host, got.cpu().numpy())), "windows_in_ill_conditioned_band": int(band.sum())}
-            print(rate, model, n, entry[f"model{model}"])
+            print(rate, model, n, entry[f"model{model}"], file=sys.stderr)
         report["rates"][str(rate)] = entry
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    json.dump(report, open(os.path.join(ROOT, "gpurun_out", "dataset_replay.json"), "w"), indent=1)
-    print(json.dumps(report)[:600])
+    print(json.dumps(report))
 
 
 if __name__ == "__main__":

@@ -1,14 +1,14 @@
 #!/usr/bin/env python
-"""SASS evidence for profiles/: per kernel of libcpi_b200.so the counts of the instructions the design rests on
+"""SASS evidence: per kernel of libcpi_b200.so the counts of the instructions the design rests on
 (UBLKCP = 1-D TMA bulk copy, SYNCS = mbarrier, DFMA/DMUL/DADD = fp64 pipe, FFMA = fp32 variant, SHFL = trio gathers, LDS/STS = slots,
-tensor-core opcodes = must be zero).    python tools/sass_counts.py > profiles/r02_sass_counts.txt"""
+tensor-core opcodes = must be zero).    python tools/sass_counts.py"""
 import collections
 import os
 import re
 import subprocess
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-OPS = ["UBLKCP", "SYNCS", "DFMA", "DMUL", "DADD", "FFMA", "SHFL", "LDS", "STS", "LDL", "STL", "MUFU", "HMMA", "UTCMMA", "TCGEN", "BAR"]
+OPS = ["UBLKCP", "SYNCS", "DFMA", "DMUL", "DADD", "FFMA", "SHFL", "LDS", "STS", "LDL", "STL", "MUFU", "HMMA", "HGMMA", "BAR"]
 
 
 def main():
@@ -28,7 +28,7 @@ def main():
             for o in OPS:
                 if op.startswith(o):
                     counts[kern][o] += 1
-    print("# cuobjdump -sass cpi_b200/libcpi_b200.so (sm_100a): static instruction counts per kernel")
+    print("# cuobjdump -sass cpi_b200/libcpi_b200.so (sm_90a): static instruction counts per kernel")
     print(f"{'kernel':86s} {'instr':>6s} " + " ".join(f"{o:>6s}" for o in OPS))
     for k, c in counts.items():
         print(f"{k[:86]:86s} {size[k]:6d} " + " ".join(f"{c[o]:6d}" for o in OPS))
