@@ -470,6 +470,94 @@ int cpi_predict_state_batch(int model, int64_t n, const double* states_k, const 
     return CPI_OK;
 }
 
+}  // extern "C"
+
+namespace {
+// argument checks shared by both merge entry points (no CUDA call)
+int merge_check(int model, int dtype, int64_t n_groups, const int64_t* group_offsets, int64_t group_uniform) {
+    if (model == 2)
+        return fail(CPI_EINVAL, "model 2 records cannot be merged: their gravity removal depends on q_k_lin, which a merge would have to "
+                                "re-linearise (only model 1 is supported)");
+    if (model != 1) return fail(CPI_EINVAL, "model must be 1 (got %d)", model);
+    if (dtype != 64 && dtype != 32) return fail(CPI_EINVAL, "dtype must be 64 or 32 (got %d)", dtype);
+    if (n_groups < 0 || (!group_offsets && group_uniform < 0)) return fail(CPI_EINVAL, "negative count");
+    if (n_groups > 2147483647) return fail(CPI_EINVAL, "too many groups (%lld; at most 2^31 - 1 per call)", (long long)n_groups);
+    return CPI_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int cpi_merge_records(int model, int dtype, int64_t n_groups, const int64_t* group_offsets, int64_t group_uniform,
+                      const void* records, const void* lin, void* out_records, void* stream) {
+    int rc = merge_check(model, dtype, n_groups, group_offsets, group_uniform);
+    if (rc || n_groups == 0) return rc;
+    if (!out_records) return fail(CPI_EINVAL, "null pointer argument (out_records)");
+    if ((!records || !lin) && (group_offsets || group_uniform > 0)) return fail(CPI_EINVAL, "null pointer argument (records / lin)");
+    if (out_records == records) return fail(CPI_EINVAL, "out_records must not overlap records");
+    if (!group_offsets && records) {           // the uniform layout's extent is known: check the whole range
+        const size_t es = dtype == 32 ? 4 : 8, rb = (size_t)CPI_REC_V1_DOUBLES * es;
+        const char *r0 = (const char*)records, *r1 = r0 + (size_t)n_groups * group_uniform * rb;
+        const char *o0 = (const char*)out_records, *o1 = o0 + (size_t)n_groups * rb;
+        if (o0 < r1 && r0 < o1) return fail(CPI_EINVAL, "out_records must not overlap records");
+    }
+    DevInfo d;
+    if ((rc = device_info(d))) return rc;
+    CU(cpi::merge_launch(dtype, n_groups, group_offsets, group_uniform, records, lin, out_records, (cudaStream_t)stream));
+    g_launches += 1;
+    return CPI_OK;
+}
+
+int cpi_merge_records_host(int model, int dtype, int64_t n_groups, const int64_t* group_offsets, int64_t group_uniform,
+                           const void* records, const void* lin, void* out_records) {
+    int rc = merge_check(model, dtype, n_groups, group_offsets, group_uniform);
+    if (rc || n_groups == 0) return rc;
+    if (!out_records) return fail(CPI_EINVAL, "null pointer argument (out_records)");
+    const size_t es = dtype == 32 ? 4 : 8;
+    const int64_t max_records = (int64_t)(((uint64_t)1 << 62) / ((uint64_t)CPI_REC_V1_DOUBLES * es));
+    if (group_offsets) {                        // the host copy of the CSR layout is validated before anything reaches the device
+        if (group_offsets[0] < 0) return fail(CPI_EINVAL, "group_offsets out of range: group_offsets[0] = %lld is negative", (long long)group_offsets[0]);
+        for (int64_t g = 0; g < n_groups; g++)
+            if (group_offsets[g + 1] < group_offsets[g])
+                return fail(CPI_EINVAL, "group_offsets must be non-decreasing (group %lld)", (long long)g);
+        if (group_offsets[n_groups] > max_records)
+            return fail(CPI_EINVAL, "group_offsets out of range: %lld records", (long long)group_offsets[n_groups]);
+    } else if (group_uniform > max_records / n_groups) {
+        return fail(CPI_EINVAL, "group_uniform out of range: %lld x %lld records", (long long)n_groups, (long long)group_uniform);
+    }
+    const int64_t n_rec = group_offsets ? group_offsets[n_groups] : n_groups * group_uniform;
+    if (n_rec > 0 && (!records || !lin)) return fail(CPI_EINVAL, "null pointer argument (records / lin)");
+    if (n_rec > 0 && out_records == records) return fail(CPI_EINVAL, "out_records must not overlap records");
+    DevInfo d;
+    if ((rc = device_info(d))) return rc;
+    std::lock_guard<std::mutex> lk(g_scratch_mu);
+    if ((rc = scratch_prepare())) return rc;
+    const size_t rb = (size_t)CPI_REC_V1_DOUBLES * es;
+    void *d_r, *d_l, *d_o, *d_off = nullptr;
+    if ((rc = dev_buf(0, (size_t)n_rec * rb, &d_r))) return rc;
+    if ((rc = dev_buf(1, (size_t)n_rec * CPI_LIN_DOUBLES * es, &d_l))) return rc;
+    if ((rc = dev_buf(2, (size_t)n_groups * rb, &d_o))) return rc;
+    if (group_offsets && (rc = dev_buf(3, (size_t)(n_groups + 1) * 8, &d_off))) return rc;
+    cudaStream_t st = g_scratch.stream;
+    // every error path drains the stream before returning: async copies from / into the caller's buffers must not outlive the call
+#define CUX(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { rc = fail(CPI_ECUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); goto drain; } } while (0)
+    if (group_offsets) CUX(cudaMemcpyAsync(d_off, group_offsets, (size_t)(n_groups + 1) * 8, cudaMemcpyHostToDevice, st));
+    if (n_rec > 0) {
+        CUX(cudaMemcpyAsync(d_r, records, (size_t)n_rec * rb, cudaMemcpyHostToDevice, st));
+        CUX(cudaMemcpyAsync(d_l, lin, (size_t)n_rec * CPI_LIN_DOUBLES * es, cudaMemcpyHostToDevice, st));
+    }
+    rc = cpi_merge_records(model, dtype, n_groups, (const int64_t*)d_off, group_uniform, d_r, d_l, d_o, st);
+    if (rc) goto drain;
+    CUX(cudaMemcpyAsync(out_records, d_o, (size_t)n_groups * rb, cudaMemcpyDeviceToHost, st));
+drain:
+#undef CUX
+    {
+        cudaError_t e_ = cudaStreamSynchronize(st);
+        if (e_ != cudaSuccess && rc == CPI_OK) rc = fail(CPI_ECUDA, "cudaStreamSynchronize failed: %s", cudaGetErrorString(e_));
+    }
+    return rc;
+}
+
 int cpi_retract_batch(int64_t n, const double* states, const double* xi, double* states_out, void* stream) {
     if (n < 0) return fail(CPI_EINVAL, "negative count");
     if (n == 0) return CPI_OK;

@@ -46,6 +46,9 @@ cudaError_t chain_assemble_launch(int64_t nf, const double* G11, const double* G
                                   int diagonal_damping, const double* prior_info, const double* prior_rhs, double* D, double* E, double* rhs, cudaStream_t st);
 int64_t chain_solve_workspace_bytes(int64_t n_states);
 cudaError_t chain_solve_launch(int64_t n_states, const double* D, const double* E, const double* b, double* x, double* ws, cudaStream_t st, int* launches);
+// merge.cu: one merged model-1 record per group (dtype 64 or 32)
+cudaError_t merge_launch(int dtype, int64_t n_groups, const int64_t* offsets, int64_t uniform, const void* records, const void* lin,
+                         void* out, cudaStream_t st);
 cudaError_t retract_launch(int64_t n, const double* states, const double* xi, double* out, cudaStream_t st);
 
 }  // namespace cpi

@@ -122,6 +122,77 @@ def preintegrate(model, samples, lin, sigmas, flags=0, offsets=None, ns=None, ou
     return out
 
 
+def _merge_layout(n_rec, group_offsets, group, n_offsets):
+    """(n_groups, uniform) of a merge call; group_offsets has n_offsets entries (or is None)."""
+    if (group_offsets is None) == (group is None):
+        raise ValueError("give exactly one of group_offsets (CSR, n_groups + 1 entries) and group (uniform group length)")
+    if group_offsets is not None:
+        return n_offsets - 1, 0
+    group = int(group)
+    if group < 1:
+        raise ValueError("group must be >= 1 (use group_offsets for empty groups)")
+    if n_rec % group:
+        raise ValueError(f"{n_rec} records do not split into groups of {group}")
+    return n_rec // group, group
+
+
+def merge_host(model, records, lin, group_offsets=None, group=None):
+    """Merge consecutive records (``cpi_merge_records_host``): HOST numpy in and out.  records (n, 290) float64 or float32, lin (n, 13)
+    in the same dtype, one linearisation point per record; either ``group_offsets`` (int64, n_groups + 1: group g is records
+    offsets[g] .. offsets[g+1]-1, in time order) or ``group`` (groups of that many consecutive records).  Returns one record per group,
+    at the linearisation point of the group's first record."""
+    lib = capi.load()
+    records = np.asarray(records)
+    dtype = np.dtype(np.float32) if records.dtype == np.float32 else np.dtype(np.float64)
+    records = np.ascontiguousarray(records, dtype=dtype).reshape(-1, REC_DOUBLES.get(model, REC_DOUBLES[1]))   # the library rejects model 2
+    lin = np.ascontiguousarray(lin, dtype=dtype).reshape(-1, 13)
+    if lin.shape[0] != records.shape[0]:
+        raise ValueError("lin must hold one linearisation point per record")
+    offs = None if group_offsets is None else np.ascontiguousarray(group_offsets, dtype=np.int64)
+    n, uniform = _merge_layout(records.shape[0], offs, group, 0 if offs is None else offs.shape[0])
+    if offs is not None and offs.shape[0] and offs[-1] > records.shape[0]:
+        raise ValueError("group_offsets run past the record array")
+    out = np.empty((max(n, 0), records.shape[1]), dtype=dtype)
+    capi.check(lib.cpi_merge_records_host(model, 8 * dtype.itemsize, n, _ptr(offs), uniform, _ptr(records), _ptr(lin), _ptr(out)))
+    return out
+
+
+def merge(model, records, lin, group_offsets=None, group=None, out=None, stream=None):
+    """Merge consecutive records on the device (``cpi_merge_records``): CUDA tensors (float64, or float32 records and lin), contiguous,
+    on one device; enqueues on ``stream`` (default: torch's current stream) and does not synchronise.  Layout as ``merge_host``;
+    ``group_offsets`` is an int64 CUDA tensor.  Returns ``out`` (n_groups, 290), which must not overlap ``records``."""
+    import torch
+
+    lib = capi.load()
+    if not (records.is_cuda and lin.is_cuda):
+        raise ValueError("merge() takes CUDA tensors; use merge_host() for host arrays")
+    if records.dtype not in (torch.float64, torch.float32) or lin.dtype != records.dtype:
+        raise ValueError("records and lin must both be float64 or both float32")
+    dev = records.device
+    for name, t in (("lin", lin), ("group_offsets", group_offsets), ("out", out)):
+        if t is not None and t.device != dev:
+            raise ValueError(f"{name} lives on {t.device}, records on {dev}: all tensors of one call must be on the same CUDA device")
+    rd = REC_DOUBLES[1]
+    records = records.contiguous(); lin = lin.contiguous()
+    n_rec = records.numel() // rd
+    if lin.numel() != 13 * n_rec:
+        raise ValueError("lin must hold one linearisation point per record")
+    if group_offsets is not None:
+        group_offsets = group_offsets.contiguous()
+        if group_offsets.dtype != torch.int64:
+            raise ValueError("group_offsets must be int64")
+    n, uniform = _merge_layout(n_rec, group_offsets, group, 0 if group_offsets is None else group_offsets.numel())
+    if out is None:
+        out = torch.empty((max(n, 0), rd), dtype=records.dtype, device=dev)
+    elif out.numel() < n * rd or not out.is_contiguous() or out.dtype != records.dtype:
+        raise ValueError("out must be a contiguous tensor of n_groups * 290 elements in the records' dtype")
+    with torch.cuda.device(dev):
+        st = stream if stream is not None else torch.cuda.current_stream(dev)
+        capi.check(lib.cpi_merge_records(model, 64 if records.dtype == torch.float64 else 32, n, _tptr(group_offsets), uniform,
+                                         _tptr(records), _tptr(lin), _tptr(out), ctypes.c_void_p(st.cuda_stream)))
+    return out
+
+
 # ------------------------------------------------------------------------------------------------------------------
 # reference-shaped objects
 # ------------------------------------------------------------------------------------------------------------------
@@ -216,6 +287,17 @@ class CpiBase:
 class CpiV1(CpiBase):
     """Model 1, piecewise-constant measurement (cpi/CpiV1.h:41)."""
     model = 1
+
+    def mergeWith(self, later):
+        """Extend this finalised window by the finalised window that follows it (GTSAM's mergeWith), in place: the fields become those
+        of the combined interval, at this object's linearisation point (``later`` is moved to it to first order).  The staged steps
+        are concatenated too, so a later ``finalize()`` re-preintegrates the combined window from its samples."""
+        if not isinstance(later, CpiV1):
+            raise TypeError("mergeWith takes a CpiV1")
+        rec = merge_host(1, np.stack([self.record(), later.record()]), np.stack([self._lin(), later._lin()]), group=2)
+        self._steps = self._steps + later._steps
+        self._adopt(rec[0])
+        return self
 
 
 class CpiV2(CpiBase):

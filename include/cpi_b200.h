@@ -146,6 +146,37 @@ int cpi_host_last_timing(double* submit_ms, double* total_ms);
 int cpi_host_register(void* ptr, size_t bytes);
 int cpi_host_unregister(void* ptr);
 
+/* ---- merging records ------------------------------------------------------------------------------------------- */
+
+/*
+ * Merge consecutive model-1 records: the record of the interval k -> j from the records of k -> m and m -> j, what GTSAM's
+ * PreintegratedImuMeasurements::mergeWith does.  Used to combine two IMU factors into one when the keyframe between them is dropped,
+ * and to preintegrate ONE long window in parallel: cut it into S segments, preintegrate them as S windows of one CSR
+ * cpi_preintegrate_batch call, merge each group of S records here (DESIGN.md "Merging records").
+ *   model          1.  Model 2 returns CPI_EINVAL (its gravity removal depends on q_k_lin, which a merge would have to re-linearise).
+ *   dtype          64, or 32 for float records and lin (the arithmetic is fp64 either way)
+ *   group_offsets  device int64[n_groups+1] (the _host variant: HOST): group g is records group_offsets[g] .. group_offsets[g+1]-1,
+ *                  in time order; or NULL for groups of `group_uniform` consecutive records.  Device-resident offsets cannot be
+ *                  validated by this entry point: a decreasing pair yields an empty group (the _host variant returns CPI_EINVAL).
+ *   records        device, CPI_REC_V1_DOUBLES per record
+ *   lin            device, CPI_LIN_DOUBLES per RECORD: the linearisation point each record was preintegrated at
+ *   out_records    device, one record per group; must not overlap `records`
+ * The merged record is expressed at the linearisation point of the group's first record: every later record is first moved there
+ * to first order (R <- Exp(J_q db_w) R, alpha/beta += J db_w + H db_a; its Jacobians and P are used as they are, as mergeWith does).
+ * At equal linearisation points the means and the bias Jacobians are exact compositions (~1e-15 of the one-shot record) and P
+ * agrees with the one-shot RK4 to its truncation error (~1e-10 relative).  An empty group yields the zero-step record (R = I,
+ * q = [0 0 0 1], everything else 0); a group of one yields a bitwise copy of its record.  Long groups are merged as a pairwise tree
+ * (logarithmic depth); one kernel launch per call.
+ */
+int cpi_merge_records(int model, int dtype, int64_t n_groups, const int64_t* group_offsets, int64_t group_uniform,
+                      const void* records, const void* lin, void* out_records, void* stream);
+
+/* Same with HOST buffers (H2D + kernel + D2H through device buffers owned by the library, synchronous).  group_offsets is a HOST
+ * array, checked before anything reaches the device: non-decreasing, group_offsets[0] >= 0, group_offsets[n_groups] records in
+ * `records` and `lin`. */
+int cpi_merge_records_host(int model, int dtype, int64_t n_groups, const int64_t* group_offsets, int64_t group_uniform,
+                           const void* records, const void* lin, void* out_records);
+
 /* ---- factor evaluation ------------------------------------------------------------------------------------------- */
 
 /*

@@ -63,6 +63,37 @@ protected:
     virtual int flags() const { return imu_avg ? CPI_FLAG_IMU_AVG : 0; }
     virtual void adopt_extra(const double*) {}
 
+    // the public result fields in the record layout (include/cpi_b200.h), and the linearisation point
+    void pack_v1(double* r) const {
+        Eigen::Map<Eigen::Matrix<double, 4, 1> >(r + CPI_REC_Q) = q_k2tau;
+        Eigen::Map<Eigen::Matrix<double, 3, 3> >(r + CPI_REC_R) = R_k2tau;
+        Eigen::Map<Eigen::Matrix<double, 3, 1> >(r + CPI_REC_ALPHA) = alpha_tau;
+        Eigen::Map<Eigen::Matrix<double, 3, 1> >(r + CPI_REC_BETA) = beta_tau;
+        r[CPI_REC_DT] = DT;
+        Eigen::Map<Eigen::Matrix<double, 3, 3> >(r + CPI_REC_JQ) = J_q;
+        Eigen::Map<Eigen::Matrix<double, 3, 3> >(r + CPI_REC_JA) = J_a;
+        Eigen::Map<Eigen::Matrix<double, 3, 3> >(r + CPI_REC_JB) = J_b;
+        Eigen::Map<Eigen::Matrix<double, 3, 3> >(r + CPI_REC_HA) = H_a;
+        Eigen::Map<Eigen::Matrix<double, 3, 3> >(r + CPI_REC_HB) = H_b;
+        Eigen::Map<Eigen::Matrix<double, 15, 15> >(r + CPI_REC_P) = P_meas;
+    }
+    void pack_lin(double* l) const {
+        const double v[13] = {b_w_lin(0), b_w_lin(1), b_w_lin(2), b_a_lin(0), b_a_lin(1), b_a_lin(2),
+                              q_k_lin(0), q_k_lin(1), q_k_lin(2), q_k_lin(3), grav(0), grav(1), grav(2)};
+        std::memcpy(l, v, sizeof v);
+    }
+    // k -> m (this) (+) m -> j (later): merged on the device, the fields re-adopted; the staged steps are concatenated
+    void merge_v1(const CpiGpuBase& later) {
+        std::vector<double> rec(2 * (size_t)CPI_REC_V1_DOUBLES), lin(2 * (size_t)CPI_LIN_DOUBLES), out(CPI_REC_V1_DOUBLES);
+        pack_v1(rec.data()); later.pack_v1(rec.data() + CPI_REC_V1_DOUBLES);
+        pack_lin(lin.data()); later.pack_lin(lin.data() + CPI_LIN_DOUBLES);
+        const int rc = cpi_merge_records_host(1, 64, 1, nullptr, 2, rec.data(), lin.data(), out.data());
+        if (rc != CPI_OK) throw std::runtime_error(std::string("cpi_b200: ") + cpi_last_error());
+        steps_.insert(steps_.end(), later.steps_.begin(), later.steps_.end());
+        next_.insert(next_.end(), later.next_.begin(), later.next_.end());
+        adopt(out.data());
+    }
+
 private:
     int model_;
     double sig_[4];
@@ -121,6 +152,10 @@ class CpiV1Gpu : public CpiGpuBase {
 public:
     CpiV1Gpu(double sigma_w, double sigma_wb, double sigma_a, double sigma_ab, bool imu_avg_ = false)
         : CpiGpuBase(1, sigma_w, sigma_wb, sigma_a, sigma_ab, imu_avg_) {}
+
+    /// Extend this finalised window by the finalised window that follows it (GTSAM's mergeWith), in place, at this object's
+    /// linearisation point (`later` is moved to it to first order).  Throws std::runtime_error if the library reports an error.
+    void mergeWith(const CpiV1Gpu& later) { merge_v1(later); }
 };
 
 /// Drop-in for CpiV2 (cpi/CpiV2.h:41)
