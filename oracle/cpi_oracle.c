@@ -11,67 +11,81 @@
  * golden vectors under tests/golden/ that were generated from that library by tests/golden/make_golden.py.
  *
  * Build: oracle/Makefile (gcc -O2 -ffp-contract=off: no FMA contraction, to stay close to the reference's SSE2 code).
+ *
+ * Precision-generic: all arithmetic is in `real`.  liboracle.so builds it as double (the restatement above);
+ * liboracle_ld.so builds the same source with -DCPI_ORACLE_LONG_DOUBLE (x86-64 x87 extended precision, 64-bit mantissa) as
+ * the high-precision truth the precision tests measure the kernels and the fp64 build against.  Inputs and outputs are
+ * double in both builds.  The two branch decisions of the reference (small_w and dt == 0) are taken on the values the fp64
+ * code sees, so the extended build evaluates the same piecewise function, only more accurately.
  */
 #include "cpi_oracle.h"
 #include "../include/cpi_b200.h"
-#include <math.h>
 #include <pthread.h>
 #include <stdlib.h>
 #include <string.h>
+#include <tgmath.h>
+
+#ifdef CPI_ORACLE_LONG_DOUBLE
+typedef long double real;
+#else
+typedef double real;
+#endif
 
 /* ------------------------------------------------------------------ small dense helpers (column-major) ---------- */
 #define E(M, ld, i, j) ((M)[(i) + (j) * (ld)])
 
-static void mat_zero(double* A, int n) { memset(A, 0, sizeof(double) * (size_t)n); }
-static void mat_eye(double* A, int n) { mat_zero(A, n * n); for (int i = 0; i < n; i++) E(A, n, i, i) = 1.0; }
+static void load(real* dst, const double* src, int n) { for (int i = 0; i < n; i++) dst[i] = src[i]; }
+static void store(double* dst, const real* src, int n) { for (int i = 0; i < n; i++) dst[i] = (double)src[i]; }
+static void mat_zero(real* A, int n) { memset(A, 0, sizeof *A * (size_t)n); }
+static void mat_eye(real* A, int n) { mat_zero(A, n * n); for (int i = 0; i < n; i++) E(A, n, i, i) = 1.0; }
 /* C(m x n) = A(m x k) * B(k x n) */
-static void gemm(int m, int n, int k, const double* A, const double* B, double* C) {
+static void gemm(int m, int n, int k, const real* A, const real* B, real* C) {
     for (int j = 0; j < n; j++) for (int i = 0; i < m; i++) {
-        double s = 0.0;
+        real s = 0.0;
         for (int l = 0; l < k; l++) s += E(A, m, i, l) * E(B, k, l, j);
         E(C, m, i, j) = s;
     }
 }
 /* C(m x n) = A(m x k) * B(n x k)^T */
-static void gemm_nt(int m, int n, int k, const double* A, const double* B, double* C) {
+static void gemm_nt(int m, int n, int k, const real* A, const real* B, real* C) {
     for (int j = 0; j < n; j++) for (int i = 0; i < m; i++) {
-        double s = 0.0;
+        real s = 0.0;
         for (int l = 0; l < k; l++) s += E(A, m, i, l) * E(B, n, j, l);
         E(C, m, i, j) = s;
     }
 }
-static void transpose(int m, int n, const double* A, double* At) {
+static void transpose(int m, int n, const real* A, real* At) {
     for (int i = 0; i < m; i++) for (int j = 0; j < n; j++) E(At, n, j, i) = E(A, m, i, j);
 }
 /* dst block (r0,c0) of size br x bc in a matrix with leading dim ld  <-  s * B */
-static void set_block(double* M, int ld, int r0, int c0, int br, int bc, const double* B, double s) {
+static void set_block(real* M, int ld, int r0, int c0, int br, int bc, const real* B, real s) {
     for (int j = 0; j < bc; j++) for (int i = 0; i < br; i++) E(M, ld, r0 + i, c0 + j) = s * E(B, br, i, j);
 }
-static void get_block(const double* M, int ld, int r0, int c0, int br, int bc, double* B) {
+static void get_block(const real* M, int ld, int r0, int c0, int br, int bc, real* B) {
     for (int j = 0; j < bc; j++) for (int i = 0; i < br; i++) E(B, br, i, j) = E(M, ld, r0 + i, c0 + j);
 }
-static void m3_mul(const double* A, const double* B, double* C) { double T[9]; gemm(3, 3, 3, A, B, T); memcpy(C, T, sizeof T); }
-static void m3_vec(const double* A, const double* v, double* o) {
-    double t[3];
+static void m3_mul(const real* A, const real* B, real* C) { real T[9]; gemm(3, 3, 3, A, B, T); memcpy(C, T, sizeof T); }
+static void m3_vec(const real* A, const real* v, real* o) {
+    real t[3];
     for (int i = 0; i < 3; i++) t[i] = E(A, 3, i, 0) * v[0] + E(A, 3, i, 1) * v[1] + E(A, 3, i, 2) * v[2];
     o[0] = t[0]; o[1] = t[1]; o[2] = t[2];
 }
-static double norm3(const double* v) { return sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]); }
-static double norm4(const double* v) { return sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2] + v[3] * v[3]); }
+static real norm3(const real* v) { return sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]); }
+static real norm4(const real* v) { return sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2] + v[3] * v[3]); }
 
 /* ------------------------------------------------------------------ utils/quat_ops.h ----------------------------- */
 
 /* skew_x, quat_ops.h:92-98 */
-static void skew_x(const double* w, double* M) {
+static void skew_x(const real* w, real* M) {
     E(M, 3, 0, 0) = 0;     E(M, 3, 0, 1) = -w[2]; E(M, 3, 0, 2) = w[1];
     E(M, 3, 1, 0) = w[2];  E(M, 3, 1, 1) = 0;     E(M, 3, 1, 2) = -w[0];
     E(M, 3, 2, 0) = -w[1]; E(M, 3, 2, 1) = w[0];  E(M, 3, 2, 2) = 0;
 }
 
 /* rot_2_quat, quat_ops.h:45-86 : four-case largest-diagonal extraction, force w >= 0, normalise */
-void oracle_rot_2_quat(const double* rot, double* q) {
-    double r00 = E(rot, 3, 0, 0), r11 = E(rot, 3, 1, 1), r22 = E(rot, 3, 2, 2);
-    double T = r00 + r11 + r22;
+static void rot_2_quat(const real* rot, real* q) {
+    real r00 = E(rot, 3, 0, 0), r11 = E(rot, 3, 1, 1), r22 = E(rot, 3, 2, 2);
+    real T = r00 + r11 + r22;
     if (r00 >= T && r00 >= r11 && r00 >= r22) {
         q[0] = sqrt((1 + (2 * r00) - T) / 4);
         q[1] = (1 / (4 * q[0])) * (E(rot, 3, 0, 1) + E(rot, 3, 1, 0));
@@ -94,72 +108,91 @@ void oracle_rot_2_quat(const double* rot, double* q) {
         q[2] = (1 / (4 * q[3])) * (E(rot, 3, 0, 1) - E(rot, 3, 1, 0));
     }
     if (q[3] < 0) { for (int i = 0; i < 4; i++) q[i] = -q[i]; }
-    double n = norm4(q);
+    real n = norm4(q);
     for (int i = 0; i < 4; i++) q[i] = q[i] / n;
 }
 
 /* quat_2_Rot, quat_ops.h:104-109 : (2 q4^2 - 1) I - 2 q4 [q_v x] + 2 q_v q_v^T */
-void oracle_quat_2_Rot(const double* q, double* R) {
-    double qx[9]; skew_x(q, qx);
-    double s = 2 * pow(q[3], 2) - 1;
+static void quat_2_Rot(const real* q, real* R) {
+    real qx[9]; skew_x(q, qx);
+    real s = 2 * pow(q[3], 2) - 1;
     for (int j = 0; j < 3; j++) for (int i = 0; i < 3; i++)
         E(R, 3, i, j) = s * (i == j ? 1.0 : 0.0) - 2 * q[3] * E(qx, 3, i, j) + 2 * q[i] * q[j];
 }
 
 /* quat_multiply, quat_ops.h:115-128 : JPL product q (x) p, force w >= 0, normalise */
-void oracle_quat_multiply(const double* q, const double* p, double* out) {
-    double Qm[16], qx[9], t[4];
+static void quat_multiply(const real* q, const real* p, real* out) {
+    real Qm[16], qx[9], t[4];
     skew_x(q, qx);
     for (int j = 0; j < 3; j++) for (int i = 0; i < 3; i++) E(Qm, 4, i, j) = q[3] * (i == j ? 1.0 : 0.0) - E(qx, 3, i, j);
     for (int i = 0; i < 3; i++) { E(Qm, 4, i, 3) = q[i]; E(Qm, 4, 3, i) = -q[i]; }
     E(Qm, 4, 3, 3) = q[3];
     gemm(4, 1, 4, Qm, p, t);
     if (t[3] < 0) { for (int i = 0; i < 4; i++) t[i] *= -1; }
-    double n = norm4(t);
+    real n = norm4(t);
     for (int i = 0; i < 4; i++) out[i] = t[i] / n;
 }
 
 /* Exp, quat_ops.h:145-162 : I + sin(th)/th [w x] + (1-cos th)/th^2 [w x]^2 ; identity iff th == 0 */
-void oracle_Exp(const double* w, double* R) {
-    double wx[9], wx2[9];
+static void Exp(const real* w, real* R) {
+    real wx[9], wx2[9];
     skew_x(w, wx);
-    double th = norm3(w);
+    real th = norm3(w);
     if (th == 0) { mat_eye(R, 3); return; }
     gemm(3, 3, 3, wx, wx, wx2);
-    double a = sin(th) / th, b = (1 - cos(th)) / pow(th, 2);
+    real a = sin(th) / th, b = (1 - cos(th)) / pow(th, 2);
     for (int k = 0; k < 9; k++) R[k] = (k % 4 == 0 ? 1.0 : 0.0) + a * wx[k] + b * wx2[k];
 }
 
+void oracle_rot_2_quat(const double* R, double* q) { real r[9], o[4]; load(r, R, 9); rot_2_quat(r, o); store(q, o, 4); }
+void oracle_quat_2_Rot(const double* q, double* R) { real a[4], o[9]; load(a, q, 4); quat_2_Rot(a, o); store(R, o, 9); }
+void oracle_quat_multiply(const double* q, const double* p, double* out) {
+    real a[4], b[4], o[4]; load(a, q, 4); load(b, p, 4); quat_multiply(a, b, o); store(out, o, 4);
+}
+void oracle_Exp(const double* w, double* R) { real a[3], o[9]; load(a, w, 3); Exp(a, o); store(R, o, 9); }
+
 /* Inv, quat_ops.h:190-197 */
-static void quat_inv(const double* q, double* o) { o[0] = -q[0]; o[1] = -q[1]; o[2] = -q[2]; o[3] = q[3]; }
+static void quat_inv(const real* q, real* o) { o[0] = -q[0]; o[1] = -q[1]; o[2] = -q[2]; o[3] = q[3]; }
 
 /* ------------------------------------------------------------------ cpi/CpiBase.h -------------------------------- */
 
 typedef struct {
-    int imu_avg, stj;                          /* CpiBase.h:95, CpiV2.h:58 */
-    double DT, alpha[3], beta[3], q[4], R[9];  /* CpiBase.h:99-103 */
-    double J_q[9], J_a[9], J_b[9], H_a[9], H_b[9];  /* :106-110 */
-    double O_a[9], O_b[9];                     /* CpiV2.h:62-63 */
-    double b_w[3], b_a[3], q_lin[4], grav[3];  /* CpiBase.h:113-118 */
-    double Qc[144];                            /* :121 */
-    double P[225];                             /* :124 */
-    double Pbig[441], D[441];                  /* CpiV2.h:46-49 */
+    int imu_avg, stj;                        /* CpiBase.h:95, CpiV2.h:58 */
+    real DT, alpha[3], beta[3], q[4], R[9];  /* CpiBase.h:99-103 */
+    real J_q[9], J_a[9], J_b[9], H_a[9], H_b[9];  /* :106-110 */
+    real O_a[9], O_b[9];                     /* CpiV2.h:62-63 */
+    real b_w[3], b_a[3], q_lin[4], grav[3];  /* CpiBase.h:113-118 */
+    real Qc[144];                            /* :121 */
+    real P[225];                             /* :124 */
+    real Pbig[441], D[441];                  /* CpiV2.h:46-49 */
 } cpi_t;
 
 /* ctor CpiBase.h:52-66 + setLinearizationPoints :73-80 + member initialisers :99-124 */
 static void cpi_init(cpi_t* c, const double* sig, const double* lin, int imu_avg, int stj) {
     memset(c, 0, sizeof *c);
     c->imu_avg = imu_avg; c->stj = stj;
-    for (int b = 0; b < 4; b++) for (int i = 0; i < 3; i++) E(c->Qc, 12, 3 * b + i, 3 * b + i) = pow(sig[b], 2);
+    for (int b = 0; b < 4; b++) for (int i = 0; i < 3; i++) E(c->Qc, 12, 3 * b + i, 3 * b + i) = pow((real)sig[b], 2);
     mat_eye(c->R, 3);
     c->q[3] = 1.0;                 /* uninitialised in the reference; see include/cpi_b200.h */
     mat_eye(c->D, 21);             /* CpiV2.h:49 */
-    memcpy(c->b_w, lin, 24); memcpy(c->b_a, lin + 3, 24); memcpy(c->q_lin, lin + 6, 32); memcpy(c->grav, lin + 10, 24);
+    load(c->b_w, lin, 3); load(c->b_a, lin + 3, 3); load(c->q_lin, lin + 6, 4); load(c->grav, lin + 10, 3);
+}
+
+/* The reference's branch test |w_hat| < small_w (CpiV1.h:101), always evaluated in double exactly as the fp64 code does
+ * (w_hat = w_m_0 - b_w, averaged with w_m_1 - b_w under imu_avg; the same in both models). */
+static int small_w_branch(const double* w_m_0, const double* w_m_1, const real* b_w, int imu_avg) {
+    double w[3];
+    for (int i = 0; i < 3; i++) {
+        w[i] = w_m_0[i] - (double)b_w[i];
+        if (imu_avg) { w[i] += w_m_1[i] - (double)b_w[i]; w[i] = 0.5 * w[i]; }
+    }
+    double mag_w = sqrt(w[0] * w[0] + w[1] * w[1] + w[2] * w[2]);
+    return mag_w < 0.008726646;
 }
 
 /* Closed-form scalars shared by both models.  CpiV1.h:132-142 & 196-238  ==  CpiV2.h:158-168 & 231-274 */
-typedef struct { double f1, f2, f3, f4, df1, df2, df3, df4; } coef_t;
-static void coefficients(int small_w, double dt, double mag_w, double w_dt, double s, double c, coef_t* k) {
+typedef struct { real f1, f2, f3, f4, df1, df2, df3, df4; } coef_t;
+static void coefficients(int small_w, real dt, real mag_w, real w_dt, real s, real c, coef_t* k) {
     if (small_w) {
         k->f1 = -(pow(dt, 3) / 3); k->f2 = (pow(dt, 4) / 8); k->f3 = -(pow(dt, 2) / 2); k->f4 = (pow(dt, 3) / 6);
         k->df1 = -(pow(dt, 5) / 15); k->df2 = (pow(dt, 6) / 72); k->df3 = -(pow(dt, 4) / 12); k->df4 = (pow(dt, 5) / 60);
@@ -176,13 +209,13 @@ static void coefficients(int small_w, double dt, double mag_w, double w_dt, doub
 }
 
 /* I - a*W + b*W2  (the three rotation expressions CpiV1.h:119-120, 267-268; CpiV2.h:138-139, 321-322) */
-static void rot_from(double a, double b, const double* W, const double* W2, double* R) {
+static void rot_from(real a, real b, const real* W, const real* W2, real* R) {
     for (int k = 0; k < 9; k++) R[k] = (k % 4 == 0 ? 1.0 : 0.0) - a * W[k] + b * W2[k];
 }
 
 /* Dense Lyapunov right-hand side  F P + P F^T + G Qc G^T  for n = 15 or 21  (CpiV1.h:291, CpiV2.h:348) */
-static void lyap_rhs(int n, const double* F, const double* G, const double* Qc, const double* P, double* out) {
-    double FP[441], PFt[441], GQ[21 * 12], GQGt[441];
+static void lyap_rhs(int n, const real* F, const real* G, const real* Qc, const real* P, real* out) {
+    real FP[441], PFt[441], GQ[21 * 12], GQGt[441];
     gemm(n, n, n, F, P, FP);
     gemm_nt(n, n, n, P, F, PFt);
     gemm(n, 12, 12, G, Qc, GQ);
@@ -191,9 +224,9 @@ static void lyap_rhs(int n, const double* F, const double* G, const double* Qc, 
 }
 
 /* F and G for one RK4 stage.  CpiV1.h:276-288 (n=15); CpiV2.h:330-344 (n=21, with the two gravity blocks) */
-static void build_FG(int n, const double* w_x, const double* a_x, const double* Rstar, const double* R_old,
-                     const double* RGk, const double* grav, double* F, double* G) {
-    double RsT[9], t[9], eye[9];
+static void build_FG(int n, const real* w_x, const real* a_x, const real* Rstar, const real* R_old,
+                     const real* RGk, const real* grav, real* F, real* G) {
+    real RsT[9], t[9], eye[9];
     mat_zero(F, n * n); mat_zero(G, n * 12); mat_eye(eye, 3);
     transpose(3, 3, Rstar, RsT);
     set_block(F, n, 0, 0, 3, 3, w_x, -1.0);
@@ -202,7 +235,7 @@ static void build_FG(int n, const double* w_x, const double* a_x, const double* 
     set_block(F, n, 6, 9, 3, 3, RsT, -1.0);
     set_block(F, n, 12, 6, 3, 3, eye, 1.0);
     if (n == 21) {
-        double g_k[3], g_tau[3], sk[9], t2[9];
+        real g_k[3], g_tau[3], sk[9], t2[9];
         m3_vec(RGk, grav, g_k);                       /* R_G_to_k * grav */
         m3_vec(R_old, g_k, g_tau);                    /* R_k2tau * R_G_to_k * grav  (always the OLD R_k2tau) */
         skew_x(g_tau, sk); gemm(3, 3, 3, RsT, sk, t); set_block(F, n, 6, 15, 3, 3, t, -1.0);        /* CpiV2.h:335 */
@@ -217,22 +250,22 @@ static void build_FG(int n, const double* w_x, const double* a_x, const double* 
 /* The analytic mean / bias-Jacobian part that the two models share textually.
  * model 1: CpiV1.h:119-259.  model 2: CpiV2.h:138-305 (adds O_a/O_b and the gravity terms, incl. the sign slip at :296-297).
  * Outputs R1 (= R_k2tau1) and leaves c->R untouched (the caller commits it after the covariance, CpiV1.h:357). */
-static void means_and_jacobians(cpi_t* c, int model, double dt, const double* w_hat, double* a_hat,
-                                const double* a_m_1, double mag_w, double w_dt, int small_w, double sin_wt, double cos_wt,
-                                const double* w_x, const double* w_tx, const double* w_x_2, double* R1) {
-    double eye[9], Rstep[9], R1T[9];
+static void means_and_jacobians(cpi_t* c, int model, real dt, const real* w_hat, real* a_hat,
+                                const double* a_m_1, real mag_w, real w_dt, int small_w, real sin_wt, real cos_wt,
+                                const real* w_x, const real* w_tx, const real* w_x_2, real* R1) {
+    real eye[9], Rstep[9], R1T[9];
     mat_eye(eye, 3);
-    double dt_2 = pow(dt, 2);
+    real dt_2 = pow(dt, 2);
     if (small_w) rot_from(dt, pow(dt, 2) / 2, w_x, w_x_2, Rstep);
     else rot_from(sin_wt / mag_w, (1.0 - cos_wt) / (pow(mag_w, 2.0)), w_x, w_x_2, Rstep);
     gemm(3, 3, 3, Rstep, c->R, R1);
     transpose(3, 3, R1, R1T);
 
-    double RGk[9], g_k[3] = {0, 0, 0}, g_tau[3] = {0, 0, 0};
+    real RGk[9], g_k[3] = {0, 0, 0}, g_tau[3] = {0, 0, 0};
     if (model == 2) {
-        oracle_quat_2_Rot(c->q_lin, RGk);
+        quat_2_Rot(c->q_lin, RGk);
         if (c->imu_avg) {            /* CpiV2.h:146-149 : average the LOCAL acceleration using the NEW rotation */
-            double t[3], u[3];
+            real t[3], u[3];
             m3_vec(RGk, c->grav, t); m3_vec(R1, t, u);
             for (int i = 0; i < 3; i++) { a_hat[i] += a_m_1[i] - c->b_a[i] - u[i]; a_hat[i] = 0.5 * a_hat[i]; }
         }
@@ -241,7 +274,7 @@ static void means_and_jacobians(cpi_t* c, int model, double dt, const double* w_
     }
 
     coef_t k; coefficients(small_w, dt, mag_w, w_dt, sin_wt, cos_wt, &k);
-    double alpha_arg[9], Beta_arg[9], H_al[9], H_be[9], t3[3];
+    real alpha_arg[9], Beta_arg[9], H_al[9], H_be[9], t3[3];
     for (int i = 0; i < 9; i++) {
         alpha_arg[i] = ((dt_2 / 2.0) * eye[i] + k.f1 * w_x[i] + k.f2 * w_x_2[i]);
         Beta_arg[i] = (dt * eye[i] + k.f3 * w_x[i] + k.f4 * w_x_2[i]);
@@ -254,9 +287,9 @@ static void means_and_jacobians(cpi_t* c, int model, double dt, const double* w_
     for (int i = 0; i < 3; i++) c->beta[i] += t3[i];
 
     /* right Jacobian and J_q */
-    double J_r[9], wtx2[9], J_save[9], t9[9];
+    real J_r[9], wtx2[9], J_save[9], t9[9];
     gemm(3, 3, 3, w_tx, w_tx, wtx2);
-    if (small_w) for (int i = 0; i < 9; i++) J_r[i] = eye[i] - .5 * w_tx[i] + (1.0 / 6.0) * wtx2[i];
+    if (small_w) for (int i = 0; i < 9; i++) J_r[i] = eye[i] - .5 * w_tx[i] + ((real)1 / 6) * wtx2[i];
     else for (int i = 0; i < 9; i++)
         J_r[i] = eye[i] - ((1 - cos_wt) / (pow((w_dt), 2.0))) * w_tx[i] + ((w_dt - sin_wt) / (pow(w_dt, 3.0))) * wtx2[i];
     memcpy(J_save, c->J_q, sizeof J_save);
@@ -268,7 +301,7 @@ static void means_and_jacobians(cpi_t* c, int model, double dt, const double* w_
     for (int i = 0; i < 9; i++) c->H_b[i] -= H_be[i];
 
     if (model == 2) {                /* CpiV2.h:203-205 */
-        double sk[9], t1[9], t2[9];
+        real sk[9], t1[9], t2[9];
         skew_x(g_k, sk);
         for (int i = 0; i < 9; i++) c->O_a[i] += dt * c->O_b[i];
         gemm(3, 3, 3, H_al, c->R, t1); gemm(3, 3, 3, t1, sk, t2);
@@ -279,20 +312,20 @@ static void means_and_jacobians(cpi_t* c, int model, double dt, const double* w_
 
     for (int i = 0; i < 9; i++) c->J_a[i] += c->J_b[i] * dt;      /* old J_b */
     for (int col = 0; col < 3; col++) {
-        double e[3] = {0, 0, 0}, ex[9], Jq_e[3], sk[9], dR[9], inner[9], exw[9], wex[9], M[9], v[3];
+        real e[3] = {0, 0, 0}, ex[9], Jq_e[3], sk[9], dR[9], inner[9], exw[9], wex[9], M[9], v[3];
         e[col] = 1.0; skew_x(e, ex);
         m3_vec(c->J_q, e, Jq_e);                /* NEW J_q */
         skew_x(Jq_e, sk); gemm(3, 3, 3, R1T, sk, dR);
         for (int i = 0; i < 9; i++) dR[i] = -dR[i];
         gemm(3, 3, 3, ex, w_x, exw); gemm(3, 3, 3, w_x, ex, wex);
-        double wi = w_hat[col];
+        real wi = w_hat[col];
         /* J_a column */
         for (int i = 0; i < 9; i++) inner[i] = (wi * k.df1) * w_x[i] - k.f1 * ex[i] + (wi * k.df2) * w_x_2[i] - k.f2 * (exw[i] + wex[i]);
         gemm(3, 3, 3, dR, alpha_arg, M); gemm(3, 3, 3, R1T, inner, t9);
         for (int i = 0; i < 9; i++) M[i] += t9[i];
         m3_vec(M, a_hat, v);
         if (model == 2) {
-            double Js_e[3], sk2[9], t1[9], u[3];
+            real Js_e[3], sk2[9], t1[9], u[3];
             m3_vec(J_save, e, Js_e); skew_x(Js_e, sk2); gemm(3, 3, 3, H_al, sk2, t1); m3_vec(t1, g_tau, u);
             for (int i = 0; i < 3; i++) v[i] = v[i] - u[i];                          /* CpiV2.h:285, 289, 293 */
         }
@@ -303,7 +336,7 @@ static void means_and_jacobians(cpi_t* c, int model, double dt, const double* w_
         for (int i = 0; i < 9; i++) M[i] += t9[i];
         m3_vec(M, a_hat, v);
         if (model == 2) {
-            double Js_e[3], sk2[9], t1[9], u[3];
+            real Js_e[3], sk2[9], t1[9], u[3];
             m3_vec(J_save, e, Js_e); skew_x(Js_e, sk2); gemm(3, 3, 3, H_be, sk2, t1); m3_vec(t1, g_tau, u);
             /* CpiV2.h:296-297 reads "a_hat-\n-H_be*..." : a double minus, i.e. PLUS, for column 0 only */
             for (int i = 0; i < 3; i++) v[i] = (col == 0) ? v[i] + u[i] : v[i] - u[i];
@@ -313,31 +346,31 @@ static void means_and_jacobians(cpi_t* c, int model, double dt, const double* w_
 }
 
 /* CpiV1::feed_IMU, CpiV1.h:62-361 */
-static void feed_imu_v1(cpi_t* c, double dt, const double* w_m_0, const double* a_m_0, const double* w_m_1, const double* a_m_1) {
+static void feed_imu_v1(cpi_t* c, real dt, const double* w_m_0, const double* a_m_0, const double* w_m_1, const double* a_m_1) {
     c->DT += dt;                                             /* :69 */
     if (dt == 0) return;                                     /* :72-74 */
-    double w_hat[3], a_hat[3], w_hatdt[3];
+    real w_hat[3], a_hat[3], w_hatdt[3];
     for (int i = 0; i < 3; i++) { w_hat[i] = w_m_0[i] - c->b_w[i]; a_hat[i] = a_m_0[i] - c->b_a[i]; }
     if (c->imu_avg) for (int i = 0; i < 3; i++) {            /* :81-86 */
         w_hat[i] += w_m_1[i] - c->b_w[i]; w_hat[i] = 0.5 * w_hat[i];
         a_hat[i] += a_m_1[i] - c->b_a[i]; a_hat[i] = .5 * a_hat[i];
     }
     for (int i = 0; i < 3; i++) w_hatdt[i] = w_hat[i] * dt;
-    double mag_w = norm3(w_hat), w_dt = mag_w * dt;
-    int small_w = (mag_w < 0.008726646);                     /* :101 */
-    double cos_wt = cos(w_dt), sin_wt = sin(w_dt);
-    double w_x[9], a_x[9], w_tx[9], w_x_2[9], R1[9];
+    real mag_w = norm3(w_hat), w_dt = mag_w * dt;
+    int small_w = small_w_branch(w_m_0, w_m_1, c->b_w, c->imu_avg);   /* :101 */
+    real cos_wt = cos(w_dt), sin_wt = sin(w_dt);
+    real w_x[9], a_x[9], w_tx[9], w_x_2[9], R1[9];
     skew_x(w_hat, w_x); skew_x(a_hat, a_x); skew_x(w_hatdt, w_tx); gemm(3, 3, 3, w_x, w_x, w_x_2);
 
     means_and_jacobians(c, 1, dt, w_hat, a_hat, a_m_1, mag_w, w_dt, small_w, sin_wt, cos_wt, w_x, w_tx, w_x_2, R1);
 
     /* covariance, RK4 on the Lyapunov ODE, :267-353 */
-    double R_mid[9], t9[9];
+    real R_mid[9], t9[9];
     if (small_w) rot_from(.5 * dt, pow(.5 * dt, 2) / 2, w_x, w_x_2, t9);
     else rot_from(sin(mag_w * .5 * dt) / mag_w, (1.0 - cos(mag_w * .5 * dt)) / (pow(mag_w, 2.0)), w_x, w_x_2, t9);
     gemm(3, 3, 3, t9, c->R, R_mid);
 
-    double F[225], G[180], k1[225], k2[225], k3[225], k4[225], Ps[225];
+    real F[225], G[180], k1[225], k2[225], k3[225], k4[225], Ps[225];
     build_FG(15, w_x, a_x, c->R, 0, 0, 0, F, G);  lyap_rhs(15, F, G, c->Qc, c->P, k1);
     build_FG(15, w_x, a_x, R_mid, 0, 0, 0, F, G);
     for (int i = 0; i < 225; i++) Ps[i] = c->P[i] + k1[i] * dt / 2.0;
@@ -352,36 +385,36 @@ static void feed_imu_v1(cpi_t* c, double dt, const double* w_m_0, const double* 
     for (int i = 0; i < 225; i++) c->P[i] = 0.5 * (c->P[i] + Ps[i]);         /* :353 */
 
     memcpy(c->R, R1, sizeof c->R);                                            /* :357 */
-    oracle_rot_2_quat(c->R, c->q);                                            /* :358 */
+    rot_2_quat(c->R, c->q);                                            /* :358 */
 }
 
 /* CpiV2::feed_IMU, CpiV2.h:84-467 */
-static void feed_imu_v2(cpi_t* c, double dt, const double* w_m_0, const double* a_m_0, const double* w_m_1, const double* a_m_1) {
+static void feed_imu_v2(cpi_t* c, real dt, const double* w_m_0, const double* a_m_0, const double* w_m_1, const double* a_m_1) {
     c->DT += dt;
     if (dt == 0) return;
-    double RGk[9], w_hat[3], a_hat[3], w_hatdt[3], t3[3], u3[3];
-    oracle_quat_2_Rot(c->q_lin, RGk);
+    real RGk[9], w_hat[3], a_hat[3], w_hatdt[3], t3[3], u3[3];
+    quat_2_Rot(c->q_lin, RGk);
     m3_vec(RGk, c->grav, t3); m3_vec(c->R, t3, u3);          /* R_k2tau*quat_2_Rot(q_k_lin)*grav, :99 */
     for (int i = 0; i < 3; i++) { w_hat[i] = w_m_0[i] - c->b_w[i]; a_hat[i] = a_m_0[i] - c->b_a[i] - u3[i]; }
     if (c->imu_avg) for (int i = 0; i < 3; i++) { w_hat[i] += w_m_1[i] - c->b_w[i]; w_hat[i] = 0.5 * w_hat[i]; }
     for (int i = 0; i < 3; i++) w_hatdt[i] = w_hat[i] * dt;
-    double mag_w = norm3(w_hat), w_dt = mag_w * dt;
-    int small_w = (mag_w < 0.008726646);
-    double cos_wt = cos(w_dt), sin_wt = sin(w_dt);
-    double w_x[9], a_x[9], w_tx[9], w_x_2[9], R1[9];
+    real mag_w = norm3(w_hat), w_dt = mag_w * dt;
+    int small_w = small_w_branch(w_m_0, w_m_1, c->b_w, c->imu_avg);
+    real cos_wt = cos(w_dt), sin_wt = sin(w_dt);
+    real w_x[9], a_x[9], w_tx[9], w_x_2[9], R1[9];
     skew_x(w_hat, w_x); skew_x(w_hatdt, w_tx); gemm(3, 3, 3, w_x, w_x, w_x_2);
 
     means_and_jacobians(c, 2, dt, w_hat, a_hat, a_m_1, mag_w, w_dt, small_w, sin_wt, cos_wt, w_x, w_tx, w_x_2, R1);
     skew_x(a_hat, a_x);                                      /* :150 (after the optional averaging) */
 
-    double dt_mid = dt / 2.0, w_dt_mid = mag_w * dt_mid, R_mid[9], t9[9];
+    real dt_mid = dt / 2.0, w_dt_mid = mag_w * dt_mid, R_mid[9], t9[9];
     if (small_w) rot_from(dt_mid, pow(dt_mid, 2) / 2, w_x, w_x_2, t9);
     else rot_from(sin(w_dt_mid) / mag_w, (1.0 - cos(w_dt_mid)) / (pow(mag_w, 2.0)), w_x, w_x_2, t9);
     gemm(3, 3, 3, t9, c->R, R_mid);
 
     enum { N = 21, NN = 441 };
-    double F1[NN], F2[NN], F4[NN], G[N * 12], I21[NN];
-    double Pd1[NN], Pd2[NN], Pd3[NN], Pd4[NN], Ph1[NN], Ph2[NN], Ph3[NN], Ph4[NN], Ps[NN], Phs[NN];
+    real F1[NN], F2[NN], F4[NN], G[N * 12], I21[NN];
+    real Pd1[NN], Pd2[NN], Pd3[NN], Pd4[NN], Ph1[NN], Ph2[NN], Ph3[NN], Ph4[NN], Ps[NN], Phs[NN];
     mat_eye(I21, N);
     /* k1 :330-348 */
     build_FG(N, w_x, a_x, c->R, c->R, RGk, c->grav, F1, G);
@@ -402,13 +435,13 @@ static void feed_imu_v2(cpi_t* c, double dt, const double* w_m_0, const double* 
     gemm(N, N, N, F4, Phs, Ph4);
     lyap_rhs(N, F4, G, c->Qc, Ps, Pd4);
     /* combine :421-426 */
-    double Phi[NN];
+    real Phi[NN];
     for (int i = 0; i < NN; i++) c->Pbig[i] += (dt / 6.0) * (Pd1[i] + 2.0 * Pd2[i] + 2.0 * Pd3[i] + Pd4[i]);
     transpose(N, N, c->Pbig, Ps);
     for (int i = 0; i < NN; i++) c->Pbig[i] = 0.5 * (c->Pbig[i] + Ps[i]);
     for (int i = 0; i < NN; i++) Phi[i] = I21[i] + (dt / 6.0) * (Ph1[i] + 2.0 * Ph2[i] + 2.0 * Ph3[i] + Ph4[i]);
     /* clone + marginalise :436-446 */
-    double B[NN], T1[NN], T2[NN];
+    real B[NN], T1[NN], T2[NN];
     mat_eye(B, N);
     for (int i = 0; i < 3; i++) { E(B, N, 15 + i, 15 + i) = 0.0; E(B, N, 15 + i, i) = 1.0; }
     gemm(N, N, N, B, c->Pbig, T1); gemm_nt(N, N, N, T1, B, T2);
@@ -424,7 +457,7 @@ static void feed_imu_v2(cpi_t* c, double dt, const double* w_m_0, const double* 
         get_block(c->D, N, 12, 18, 3, 3, c->O_a); get_block(c->D, N, 6, 18, 3, 3, c->O_b);
     }
     memcpy(c->R, R1, sizeof c->R);
-    oracle_rot_2_quat(c->R, c->q);
+    rot_2_quat(c->R, c->q);
 }
 
 static void window(int model, const double* s, int64_t entries, const double* lin, const double* sig, int flags, double* rec) {
@@ -438,52 +471,55 @@ static void window(int model, const double* s, int64_t entries, const double* li
         if (model == 1) feed_imu_v1(c, e0[6], e0, e0 + 3, e1, e1 + 3);
         else feed_imu_v2(c, e0[6], e0, e0 + 3, e1, e1 + 3);
     }
-    memcpy(rec + CPI_REC_Q, c->q, 32); memcpy(rec + CPI_REC_R, c->R, 72);
-    memcpy(rec + CPI_REC_ALPHA, c->alpha, 24); memcpy(rec + CPI_REC_BETA, c->beta, 24);
-    rec[CPI_REC_DT] = c->DT;
-    memcpy(rec + CPI_REC_JQ, c->J_q, 72); memcpy(rec + CPI_REC_JA, c->J_a, 72); memcpy(rec + CPI_REC_JB, c->J_b, 72);
-    memcpy(rec + CPI_REC_HA, c->H_a, 72); memcpy(rec + CPI_REC_HB, c->H_b, 72);
-    memcpy(rec + CPI_REC_P, c->P, 225 * 8);
-    if (model == 2) { memcpy(rec + CPI_REC_OA, c->O_a, 72); memcpy(rec + CPI_REC_OB, c->O_b, 72); }
+    store(rec + CPI_REC_Q, c->q, 4); store(rec + CPI_REC_R, c->R, 9);
+    store(rec + CPI_REC_ALPHA, c->alpha, 3); store(rec + CPI_REC_BETA, c->beta, 3);
+    rec[CPI_REC_DT] = (double)c->DT;
+    store(rec + CPI_REC_JQ, c->J_q, 9); store(rec + CPI_REC_JA, c->J_a, 9); store(rec + CPI_REC_JB, c->J_b, 9);
+    store(rec + CPI_REC_HA, c->H_a, 9); store(rec + CPI_REC_HB, c->H_b, 9);
+    store(rec + CPI_REC_P, c->P, 225);
+    if (model == 2) { store(rec + CPI_REC_OA, c->O_a, 9); store(rec + CPI_REC_OB, c->O_b, 9); }
     free(c);
 }
 
 /* ------------------------------------------------------------------ gtsam/ImuFactorCPIv1.cpp, ImuFactorCPIv2.cpp -- */
 
 /* w*I - skew(v) (sign = -1) or w*I + skew(v) (sign = +1) */
-static void quat_mat(const double* q, double sign, double* M) {
-    double sk[9]; skew_x(q, sk);
+static void quat_mat(const real* q, real sign, real* M) {
+    real sk[9]; skew_x(q, sk);
     for (int i = 0; i < 9; i++) M[i] = q[3] * (i % 4 == 0 ? 1.0 : 0.0) + sign * sk[i];
 }
 
 /* ImuFactorCPIv1::evaluateError (ImuFactorCPIv1.cpp:37-208); model 2: ImuFactorCPIv2.cpp:38-212 */
-static void factor_eval(int model, const double* xi, const double* xj, const double* r, const double* l,
-                        double* err, double* H1, double* H2) {
-    const double *q_GtoK = xi, *bg_K = xi + 4, *v_K = xi + 7, *ba_K = xi + 10, *p_K = xi + 13;
-    const double *q_GtoK1 = xj, *bg_K1 = xj + 4, *v_K1 = xj + 7, *ba_K1 = xj + 10, *p_K1 = xj + 13;
-    const double *bg_lin = l, *ba_lin = l + 3, *q_K_lin = l + 6, *grav = l + 10;
-    const double *q_KtoK1 = r + CPI_REC_Q, *alpha = r + CPI_REC_ALPHA, *beta = r + CPI_REC_BETA;
-    const double *J_q = r + CPI_REC_JQ, *J_alpha = r + CPI_REC_JA, *J_beta = r + CPI_REC_JB;
-    const double *H_alpha = r + CPI_REC_HA, *H_beta = r + CPI_REC_HB;
-    const double *O_alpha = r + CPI_REC_OA, *O_beta = r + CPI_REC_OB;
-    double deltatime = r[CPI_REC_DT];
+static void factor_eval(int model, const double* xi_in, const double* xj_in, const double* r_in, const double* l_in,
+                        double* err_out, double* H1, double* H2) {
+    real xi[CPI_STATE_DOUBLES], xj[CPI_STATE_DOUBLES], r[CPI_REC_V2_DOUBLES], l[CPI_LIN_DOUBLES], err[15];
+    load(xi, xi_in, CPI_STATE_DOUBLES); load(xj, xj_in, CPI_STATE_DOUBLES); load(l, l_in, CPI_LIN_DOUBLES);
+    load(r, r_in, model == 1 ? CPI_REC_V1_DOUBLES : CPI_REC_V2_DOUBLES);
+    const real *q_GtoK = xi, *bg_K = xi + 4, *v_K = xi + 7, *ba_K = xi + 10, *p_K = xi + 13;
+    const real *q_GtoK1 = xj, *bg_K1 = xj + 4, *v_K1 = xj + 7, *ba_K1 = xj + 10, *p_K1 = xj + 13;
+    const real *bg_lin = l, *ba_lin = l + 3, *q_K_lin = l + 6, *grav = l + 10;
+    const real *q_KtoK1 = r + CPI_REC_Q, *alpha = r + CPI_REC_ALPHA, *beta = r + CPI_REC_BETA;
+    const real *J_q = r + CPI_REC_JQ, *J_alpha = r + CPI_REC_JA, *J_beta = r + CPI_REC_JB;
+    const real *H_alpha = r + CPI_REC_HA, *H_beta = r + CPI_REC_HB;
+    const real *O_alpha = r + CPI_REC_OA, *O_beta = r + CPI_REC_OB;
+    real deltatime = r[CPI_REC_DT];
 
-    double dbg[3], dba[3], t3[3], ExpB[9], q_b[4], qi[4], q_n[4], q_rminus[4], q_r[4], q_m[4];
+    real dbg[3], dba[3], t3[3], ExpB[9], q_b[4], qi[4], q_n[4], q_rminus[4], q_r[4], q_m[4];
     for (int i = 0; i < 3; i++) { dbg[i] = bg_K[i] - bg_lin[i]; dba[i] = ba_K[i] - ba_lin[i]; }
     m3_vec(J_q, dbg, t3); for (int i = 0; i < 3; i++) t3[i] = -t3[i];
-    oracle_Exp(t3, ExpB); oracle_rot_2_quat(ExpB, q_b);                       /* :57-58 */
-    quat_inv(q_GtoK, qi); oracle_quat_multiply(q_GtoK1, qi, q_n);             /* :61 */
-    quat_inv(q_KtoK1, qi); oracle_quat_multiply(q_n, qi, q_rminus);           /* :62 */
-    oracle_quat_multiply(q_rminus, q_b, q_r);                                 /* :63 */
-    quat_inv(q_b, qi); oracle_quat_multiply(qi, q_KtoK1, q_m);                /* :64 */
+    Exp(t3, ExpB); rot_2_quat(ExpB, q_b);                       /* :57-58 */
+    quat_inv(q_GtoK, qi); quat_multiply(q_GtoK1, qi, q_n);             /* :61 */
+    quat_inv(q_KtoK1, qi); quat_multiply(q_n, qi, q_rminus);           /* :62 */
+    quat_multiply(q_rminus, q_b, q_r);                                 /* :63 */
+    quat_inv(q_b, qi); quat_multiply(qi, q_KtoK1, q_m);                /* :64 */
 
-    double q_kR[4] = {0, 0, 0, 1}, dthk[3] = {0, 0, 0};
+    real q_kR[4] = {0, 0, 0, 1}, dthk[3] = {0, 0, 0};
     if (model == 2) {                                                         /* v2 :68-69 */
-        quat_inv(q_K_lin, qi); oracle_quat_multiply(q_GtoK, qi, q_kR);
+        quat_inv(q_K_lin, qi); quat_multiply(q_GtoK, qi, q_kR);
         for (int i = 0; i < 3; i++) dthk[i] = 2 * q_kR[i];
     }
-    double Rk[9], pa[3], pb[3], alphahat[3], betahat[3], u[3], w[3], o[3];
-    oracle_quat_2_Rot(q_GtoK, Rk);
+    real Rk[9], pa[3], pb[3], alphahat[3], betahat[3], u[3], w[3], o[3];
+    quat_2_Rot(q_GtoK, Rk);
     for (int i = 0; i < 3; i++) {
         if (model == 1) {                                                     /* v1 :70, :72 */
             pa[i] = p_K1[i] - p_K[i] - v_K[i] * deltatime + 0.5 * grav[i] * pow(deltatime, 2);
@@ -507,18 +543,18 @@ static void factor_eval(int model, const double* xi, const double* xj, const dou
         err[9 + i] = ba_K1[i] - ba_K[i];
         err[12 + i] = alphahat[i] - alpha[i];
     }
-    double eye[9]; mat_eye(eye, 3);
+    real eye[9]; mat_eye(eye, 3);
     if (H1) {                                                                 /* :98-154 */
-        double Hi[225], A[9], Bm[9], AB[9], blk[9], sk[9], v3[3];
+        real Hi[225], A[9], Bm[9], AB[9], blk[9], sk[9], v3[3];
         mat_zero(Hi, 225);
         quat_mat(q_n, -1.0, A); quat_mat(q_m, -1.0, Bm); gemm(3, 3, 3, A, Bm, AB);
         for (int j = 0; j < 3; j++) for (int i = 0; i < 3; i++) E(blk, 3, i, j) = -(E(AB, 3, i, j) + q_n[i] * q_m[j]);
         set_block(Hi, 15, 0, 0, 3, 3, blk, 1.0);                              /* :109-111 */
         m3_vec(Rk, pb, v3); skew_x(v3, sk);
-        if (model == 2) { double qm[9], t[9]; quat_mat(q_kR, +1.0, qm); gemm(3, 3, 3, O_beta, qm, t); for (int i = 0; i < 9; i++) sk[i] -= t[i]; }
+        if (model == 2) { real qm[9], t[9]; quat_mat(q_kR, +1.0, qm); gemm(3, 3, 3, O_beta, qm, t); for (int i = 0; i < 9; i++) sk[i] -= t[i]; }
         set_block(Hi, 15, 6, 0, 3, 3, sk, 1.0);                               /* :113 / v2 :115-116 */
         m3_vec(Rk, pa, v3); skew_x(v3, sk);
-        if (model == 2) { double qm[9], t[9]; quat_mat(q_kR, +1.0, qm); gemm(3, 3, 3, O_alpha, qm, t); for (int i = 0; i < 9; i++) sk[i] -= t[i]; }
+        if (model == 2) { real qm[9], t[9]; quat_mat(q_kR, +1.0, qm); gemm(3, 3, 3, O_alpha, qm, t); for (int i = 0; i < 9; i++) sk[i] -= t[i]; }
         set_block(Hi, 15, 12, 0, 3, 3, sk, 1.0);                              /* :115 / v2 :118-119 */
         quat_mat(q_rminus, -1.0, A); gemm(3, 3, 3, A, J_q, blk);
         set_block(Hi, 15, 0, 3, 3, 3, blk, 1.0);                              /* :119 */
@@ -531,26 +567,29 @@ static void factor_eval(int model, const double* xi, const double* xj, const dou
         set_block(Hi, 15, 9, 9, 3, 3, eye, -1.0);                             /* :137 */
         set_block(Hi, 15, 12, 9, 3, 3, H_alpha, -1.0);                        /* :139 */
         set_block(Hi, 15, 12, 12, 3, 3, Rk, -1.0);                            /* :143 */
-        memcpy(H1, Hi, sizeof Hi);
+        store(H1, Hi, 225);
     }
     if (H2) {                                                                 /* :158-198 */
-        double Hj[225], A[9];
+        real Hj[225], A[9];
         mat_zero(Hj, 225);
         quat_mat(q_r, +1.0, A); set_block(Hj, 15, 0, 0, 3, 3, A, 1.0);        /* :169 */
         set_block(Hj, 15, 3, 3, 3, 3, eye, 1.0);
         set_block(Hj, 15, 6, 6, 3, 3, Rk, 1.0);
         set_block(Hj, 15, 9, 9, 3, 3, eye, 1.0);
         set_block(Hj, 15, 12, 12, 3, 3, Rk, 1.0);
-        memcpy(H2, Hj, sizeof Hj);
+        store(H2, Hj, 225);
     }
+    store(err_out, err, 15);
 }
 
 /* getpredictedstate_v1 / _v2, solvers/GraphSolver_IMU.cpp:263-307 */
-static void predict_state(int model, const double* x, const double* r, const double* l, double* o) {
-    const double *q_GtoK = x, *bg_K = x + 4, *v_K = x + 7, *ba_K = x + 10, *p_K = x + 13, *grav = l + 10;
-    double dt = r[CPI_REC_DT], qi[4], Rinv[9], rb[3], ra[3];
-    oracle_quat_multiply(r + CPI_REC_Q, q_GtoK, o);
-    quat_inv(q_GtoK, qi); oracle_quat_2_Rot(qi, Rinv);
+static void predict_state(int model, const double* x_in, const double* r_in, const double* l_in, double* o_out) {
+    real x[CPI_STATE_DOUBLES], r[CPI_REC_V2_DOUBLES], l[CPI_LIN_DOUBLES], o[CPI_STATE_DOUBLES];
+    load(x, x_in, CPI_STATE_DOUBLES); load(l, l_in, CPI_LIN_DOUBLES); load(r, r_in, model == 1 ? CPI_REC_V1_DOUBLES : CPI_REC_V2_DOUBLES);
+    const real *q_GtoK = x, *bg_K = x + 4, *v_K = x + 7, *ba_K = x + 10, *p_K = x + 13, *grav = l + 10;
+    real dt = r[CPI_REC_DT], qi[4], Rinv[9], rb[3], ra[3];
+    quat_multiply(r + CPI_REC_Q, q_GtoK, o);
+    quat_inv(q_GtoK, qi); quat_2_Rot(qi, Rinv);
     m3_vec(Rinv, r + CPI_REC_BETA, rb); m3_vec(Rinv, r + CPI_REC_ALPHA, ra);
     for (int i = 0; i < 3; i++) {
         o[4 + i] = bg_K[i]; o[10 + i] = ba_K[i];
@@ -562,19 +601,23 @@ static void predict_state(int model, const double* x, const double* r, const dou
             o[13 + i] = p_K[i] + v_K[i] * dt + ra[i];
         }
     }
+    store(o_out, o, CPI_STATE_DOUBLES);
 }
 
 /* JPLNavState::retract, gtsam/JPLNavState.cpp:37-71 */
-static void retract(const double* x, const double* xi, double* o) {
-    double n = norm3(xi), dq[4];
+static void retract(const double* x_in, const double* xi_in, double* o_out) {
+    real x[CPI_STATE_DOUBLES], xi[15], o[CPI_STATE_DOUBLES];
+    load(x, x_in, CPI_STATE_DOUBLES); load(xi, xi_in, 15);
+    real n = norm3(xi), dq[4];
     for (int i = 0; i < 3; i++) dq[i] = ((sin(n / 2) / n)) * xi[i];
     dq[3] = cos(n / 2);
-    double nn = norm4(dq);
+    real nn = norm4(dq);
     for (int i = 0; i < 4; i++) dq[i] = dq[i] / nn;
     if (dq[3] < 0) for (int i = 0; i < 4; i++) dq[i] = -dq[i];
     if (isnan(norm4(dq))) { dq[0] = dq[1] = dq[2] = 0; dq[3] = 1.0; }
-    oracle_quat_multiply(dq, x, o);
+    quat_multiply(dq, x, o);
     for (int i = 0; i < 12; i++) o[4 + i] = x[4 + i] + xi[3 + i];
+    store(o_out, o, CPI_STATE_DOUBLES);
 }
 
 /* ------------------------------------------------------------------ batch drivers -------------------------------- */

@@ -1,6 +1,7 @@
 """TEST INFRASTRUCTURE ONLY: ctypes loaders for the CPU checkers.
 
   * ``Oracle()``    -> oracle/liboracle.so       (plain-C restatement, oracle/cpi_oracle.c)
+  * ``OracleLD()``  -> oracle/liboracle_ld.so    (the same source in long double arithmetic)
   * ``Reference()`` -> oracle/_ref/libcpi_ref.so (the UNMODIFIED reference compiled in place by oracle/ref_shim.cpp;
                        built only where an rpng/cpi checkout is given: make -C oracle ref REF=...)
 
@@ -135,6 +136,12 @@ class Oracle(_Base):
         out = np.zeros_like(states_k)
         self._pred(model, states_k.shape[0], _d(states_k), _d(records), _d(lin), _d(out))
         return out
+
+
+class OracleLD(Oracle):
+    """The same restatement computed in long double (oracle/liboracle_ld.so): double in, double out, about 1e-19 working
+    precision on x86-64.  The truth of the precision tests; its small_w / dt == 0 branches follow the fp64 code."""
+    path = os.path.join(_HERE, "liboracle_ld.so")
 
 
 class Reference(_Base):

@@ -2,7 +2,9 @@
 
 north_star tolerances: <= 1e-9 relative on dR / alpha / beta, <= 1e-6 on P.  Jacobian gates proposed by the survey:
 1e-9 relative Frobenius, except J_a for windows that touch the ill-conditioned band |w_hat| in [0.0087, 0.05) rad/s,
-where the reference's own closed forms are only determined to ~1e-8 (gate 1e-6 there)."""
+where the reference's own closed forms are only determined to ~1e-8 (gate 1e-6 there).
+
+conditioned_gate: the tighter, conditioning-aware gate against the long-double oracle (DESIGN.md section 5)."""
 import numpy as np
 
 REC = dict(q=(0, 4), R=(4, 13), alpha=(13, 16), beta=(16, 19), DT=(19, 20), J_q=(20, 29), J_a=(29, 38), J_b=(38, 47),
@@ -85,6 +87,63 @@ def compare_records(got, ref, model, in_band=None, tol_mean=1e-9, tol_P=1e-6, to
                     upd("P_block", eb / nr)
                     assert eb <= tol_P * nr + 1e-17, f"window {i}: P block ({I},{J}) err {eb:.3e} vs norm {nr:.3e}"
     return worst
+
+
+GATE_FIELDS = ("q", "R", "alpha", "beta", "J_q", "J_a", "J_b", "H_a", "H_b", "O_a", "O_b")
+
+
+def field_errors(got, truth, model):
+    """Relative Frobenius error per window of every gated field (q up to sign) and of each 3x3 block of P: a dict
+    name -> [n] array, P blocks as "P_IJ".  Where the truth is exactly zero the error is 0 if got is exactly zero too and
+    inf otherwise, so a structural zero that is not exactly zero fails any gate."""
+    g = np.asarray(got, dtype=np.float64); t = np.asarray(truth, dtype=np.float64)
+    n = t.shape[0]
+
+    def rel_rows(d, r):
+        num = np.linalg.norm(d.reshape(n, -1), axis=1); den = np.linalg.norm(r.reshape(n, -1), axis=1)
+        return np.where(den > 0, num / np.where(den > 0, den, 1.0), np.where(num > 0, np.inf, 0.0))
+
+    out = {}
+    for name in GATE_FIELDS:
+        if model == 1 and name in ("O_a", "O_b"):
+            continue
+        a, b = REC[name]
+        d = g[:, a:b] - t[:, a:b]
+        if name == "q":
+            d = np.where(np.linalg.norm(d, axis=1, keepdims=True) <= np.linalg.norm(g[:, a:b] + t[:, a:b], axis=1, keepdims=True), d, g[:, a:b] + t[:, a:b])
+        out[name] = rel_rows(d, t[:, a:b])
+    Pg = g[:, 65:290].reshape(n, 15, 15).transpose(0, 2, 1); Pt = t[:, 65:290].reshape(n, 15, 15).transpose(0, 2, 1)
+    for I in range(5):
+        for J in range(I, 5):
+            sl = (slice(None), slice(3 * I, 3 * I + 3), slice(3 * J, 3 * J + 3))
+            out[f"P_{I}{J}"] = rel_rows(Pg[sl] - Pt[sl], Pt[sl])
+    return out
+
+
+def conditioned_gate(got, o64, truth, model, K, floor, allowance=None):
+    """The conditioning-aware gate: for every window and every field of ``field_errors``,
+        e_dev <= K * max(e_64, floor) + allowance,
+    with e_dev the error of ``got`` against ``truth`` (the long-double oracle) and e_64 that of the fp64 oracle ``o64``: a
+    kernel may be as inaccurate as the fp64 reference computation is on that window, times K, and never worse than
+    K * floor where that computation is exact.  ``allowance`` (dict field -> scalar or [n] array) adds a fixed error budget,
+    e.g. the output rounding and the RK4 accumulation of the fp32 variant ("P" covers every P block).  Returns
+    (ratio, worst, failures): per field the [n] array e_dev / (K max(e_64, floor) + allowance), the worst e_dev / e_64 /
+    ratio per field for reporting, and one message per field whose worst ratio exceeds 1."""
+    g = np.asarray(got, dtype=np.float64)
+    n = g.shape[0]
+    assert np.all(np.isfinite(g)), "non-finite output"
+    ed, e64 = field_errors(g, truth, model), field_errors(o64, truth, model)
+    allowance = allowance or {}
+    ratio, worst, bad = {}, {}, []
+    for k in ed:
+        bound = K * np.maximum(e64[k], floor) + allowance.get(k, allowance.get("P", 0.0) if k.startswith("P_") else 0.0)
+        r = ed[k] / bound
+        ratio[k] = r
+        i = int(np.argmax(r))
+        worst[k] = dict(e_dev=float(ed[k].max()), e_64=float(e64[k].max()), ratio=float(r[i]))
+        if not r[i] <= 1.0:
+            bad.append(f"{k}: window {i} e_dev {ed[k][i]:.3e} e_64 {e64[k][i]:.3e} bound {np.broadcast_to(bound, (n,))[i]:.3e}")
+    return ratio, worst, bad
 
 
 def fp32_errors(got, ref):
