@@ -23,6 +23,9 @@ SYMBOLS = {
     "cpi_preintegrate_batch_host": (c_int, [c_int, c_int, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_int, c_vp]),
     "cpi_merge_records": (c_int, [c_int, c_int, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp]),
     "cpi_merge_records_host": (c_int, [c_int, c_int, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp]),
+    "cpi_scan_records_workspace": (c_i64, [c_i64, c_i64]),
+    "cpi_scan_records": (c_int, [c_int, c_int, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "cpi_scan_records_host": (c_int, [c_int, c_int, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp]),
     "cpi_imu_factor_eval_batch": (c_int, [c_int, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "cpi_imu_factor_eval_batch_host": (c_int, [c_int, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "cpi_imu_factor_hessian_batch": (c_int, [c_int, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),

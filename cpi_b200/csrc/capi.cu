@@ -35,7 +35,7 @@ int capi_fail(int code, const char* fmt, ...) {      // same per-thread error sl
 namespace {
 #define CU(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return fail(CPI_ECUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); } while (0)
 
-struct DevInfo { int sms = 0; int max_smem = 0; bool ok = false; };
+struct DevInfo { int sms = 0; int max_smem = 0; size_t mem = 0; bool ok = false; };
 int device_info(DevInfo& d) {
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);
@@ -50,6 +50,8 @@ int device_info(DevInfo& d) {
     if (major != 9 || minor != 0) return fail(CPI_ENODEVICE, "device %d is sm_%d%d, this library is built for sm_90a (H100) only", dev, major, minor);
     CU(cudaDeviceGetAttribute(&d.sms, cudaDevAttrMultiProcessorCount, dev));
     CU(cudaDeviceGetAttribute(&d.max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+    size_t free_mem = 0;
+    CU(cudaMemGetInfo(&free_mem, &d.mem));
     d.ok = true;
     if (dev < 64) cache[dev] = d;
     return CPI_OK;
@@ -473,15 +475,33 @@ int cpi_predict_state_batch(int model, int64_t n, const double* states_k, const 
 }  // extern "C"
 
 namespace {
-// argument checks shared by both merge entry points (no CUDA call)
-int merge_check(int model, int dtype, int64_t n_groups, const int64_t* group_offsets, int64_t group_uniform) {
+// argument checks shared by the merge and scan entry points (no CUDA call); `what` names the operation ("merged" / "scanned")
+int merge_check(int model, int dtype, int64_t n_groups, const int64_t* group_offsets, int64_t group_uniform, const char* what = "merged") {
     if (model == 2)
-        return fail(CPI_EINVAL, "model 2 records cannot be merged: their gravity removal depends on q_k_lin, which a merge would have to "
-                                "re-linearise (only model 1 is supported)");
+        return fail(CPI_EINVAL, "model 2 records cannot be %s: their gravity removal depends on q_k_lin, which a merge would have to "
+                                "re-linearise (only model 1 is supported)", what);
     if (model != 1) return fail(CPI_EINVAL, "model must be 1 (got %d)", model);
     if (dtype != 64 && dtype != 32) return fail(CPI_EINVAL, "dtype must be 64 or 32 (got %d)", dtype);
     if (n_groups < 0 || (!group_offsets && group_uniform < 0)) return fail(CPI_EINVAL, "negative count");
     if (n_groups > 2147483647) return fail(CPI_EINVAL, "too many groups (%lld; at most 2^31 - 1 per call)", (long long)n_groups);
+    return CPI_OK;
+}
+
+// the host copy of a CSR layout (or the uniform one) is validated before anything reaches the device; *n_rec = records it spans
+int host_layout_check(int dtype, int64_t n_groups, const int64_t* group_offsets, int64_t group_uniform, int64_t* n_rec) {
+    const size_t es = dtype == 32 ? 4 : 8;
+    const int64_t max_records = (int64_t)(((uint64_t)1 << 62) / ((uint64_t)CPI_REC_V1_DOUBLES * es));
+    if (group_offsets) {
+        if (group_offsets[0] < 0) return fail(CPI_EINVAL, "group_offsets out of range: group_offsets[0] = %lld is negative", (long long)group_offsets[0]);
+        for (int64_t g = 0; g < n_groups; g++)
+            if (group_offsets[g + 1] < group_offsets[g])
+                return fail(CPI_EINVAL, "group_offsets must be non-decreasing (group %lld)", (long long)g);
+        if (group_offsets[n_groups] > max_records)
+            return fail(CPI_EINVAL, "group_offsets out of range: %lld records", (long long)group_offsets[n_groups]);
+    } else if (group_uniform > max_records / n_groups) {
+        return fail(CPI_EINVAL, "group_uniform out of range: %lld x %lld records", (long long)n_groups, (long long)group_uniform);
+    }
+    *n_rec = group_offsets ? group_offsets[n_groups] : n_groups * group_uniform;
     return CPI_OK;
 }
 }  // namespace
@@ -514,18 +534,8 @@ int cpi_merge_records_host(int model, int dtype, int64_t n_groups, const int64_t
     if (rc || n_groups == 0) return rc;
     if (!out_records) return fail(CPI_EINVAL, "null pointer argument (out_records)");
     const size_t es = dtype == 32 ? 4 : 8;
-    const int64_t max_records = (int64_t)(((uint64_t)1 << 62) / ((uint64_t)CPI_REC_V1_DOUBLES * es));
-    if (group_offsets) {                        // the host copy of the CSR layout is validated before anything reaches the device
-        if (group_offsets[0] < 0) return fail(CPI_EINVAL, "group_offsets out of range: group_offsets[0] = %lld is negative", (long long)group_offsets[0]);
-        for (int64_t g = 0; g < n_groups; g++)
-            if (group_offsets[g + 1] < group_offsets[g])
-                return fail(CPI_EINVAL, "group_offsets must be non-decreasing (group %lld)", (long long)g);
-        if (group_offsets[n_groups] > max_records)
-            return fail(CPI_EINVAL, "group_offsets out of range: %lld records", (long long)group_offsets[n_groups]);
-    } else if (group_uniform > max_records / n_groups) {
-        return fail(CPI_EINVAL, "group_uniform out of range: %lld x %lld records", (long long)n_groups, (long long)group_uniform);
-    }
-    const int64_t n_rec = group_offsets ? group_offsets[n_groups] : n_groups * group_uniform;
+    int64_t n_rec = 0;
+    if ((rc = host_layout_check(dtype, n_groups, group_offsets, group_uniform, &n_rec))) return rc;
     if (n_rec > 0 && (!records || !lin)) return fail(CPI_EINVAL, "null pointer argument (records / lin)");
     if (n_rec > 0 && out_records == records) return fail(CPI_EINVAL, "out_records must not overlap records");
     DevInfo d;
@@ -549,6 +559,85 @@ int cpi_merge_records_host(int model, int dtype, int64_t n_groups, const int64_t
     rc = cpi_merge_records(model, dtype, n_groups, (const int64_t*)d_off, group_uniform, d_r, d_l, d_o, st);
     if (rc) goto drain;
     CUX(cudaMemcpyAsync(out_records, d_o, (size_t)n_groups * rb, cudaMemcpyDeviceToHost, st));
+drain:
+#undef CUX
+    {
+        cudaError_t e_ = cudaStreamSynchronize(st);
+        if (e_ != cudaSuccess && rc == CPI_OK) rc = fail(CPI_ECUDA, "cudaStreamSynchronize failed: %s", cudaGetErrorString(e_));
+    }
+    return rc;
+}
+
+int64_t cpi_scan_records_workspace(int64_t n_groups, int64_t n_records) {
+    if (n_groups < 0 || n_records < 0) return fail(CPI_EINVAL, "negative count");
+    return cpi::scan_workspace_bytes(n_records);
+}
+
+int cpi_scan_records(int model, int dtype, int64_t n_groups, const int64_t* group_offsets, int64_t group_uniform,
+                     const void* records, const void* lin, void* out_records, void* workspace, void* stream) {
+    int rc = merge_check(model, dtype, n_groups, group_offsets, group_uniform, "scanned");
+    if (rc || n_groups == 0) return rc;
+    if (!out_records) return fail(CPI_EINVAL, "null pointer argument (out_records)");
+    if (!workspace) return fail(CPI_EINVAL, "null pointer argument (workspace: cpi_scan_records_workspace bytes)");
+    if ((!records || !lin) && (group_offsets || group_uniform > 0)) return fail(CPI_EINVAL, "null pointer argument (records / lin)");
+    if (out_records == records) return fail(CPI_EINVAL, "out_records must not overlap records");
+    const size_t es = dtype == 32 ? 4 : 8, rb = (size_t)CPI_REC_V1_DOUBLES * es;
+    if (!group_offsets && records) {           // the uniform layout's extent is known: check the whole range
+        const size_t bytes = (size_t)n_groups * group_uniform * rb;
+        const char *r0 = (const char*)records, *r1 = r0 + bytes, *o0 = (const char*)out_records, *o1 = o0 + bytes;
+        if (o0 < r1 && r0 < o1) return fail(CPI_EINVAL, "out_records must not overlap records");
+    }
+    DevInfo d;
+    if ((rc = device_info(d))) return rc;
+    // device offsets are not read here: the records of one call fit in device memory, which bounds their count
+    const int64_t n_bound = group_offsets ? (int64_t)(d.mem / rb) : n_groups * group_uniform;
+    int launches = 0;
+    cudaError_t e = cpi::scan_launch(dtype, n_groups, group_offsets, group_uniform, n_bound, records, lin, out_records, workspace, d.sms,
+                                     (cudaStream_t)stream, &launches);
+    g_launches += launches;
+    CU(e);
+    return CPI_OK;
+}
+
+int cpi_scan_records_host(int model, int dtype, int64_t n_groups, const int64_t* group_offsets, int64_t group_uniform,
+                          const void* records, const void* lin, void* out_records) {
+    int rc = merge_check(model, dtype, n_groups, group_offsets, group_uniform, "scanned");
+    if (rc || n_groups == 0) return rc;
+    if (!out_records) return fail(CPI_EINVAL, "null pointer argument (out_records)");
+    const size_t es = dtype == 32 ? 4 : 8;
+    int64_t n_end = 0;
+    if ((rc = host_layout_check(dtype, n_groups, group_offsets, group_uniform, &n_end))) return rc;
+    const int64_t b0 = group_offsets ? group_offsets[0] : 0, n_rec = n_end - b0;
+    if (n_rec > 0 && (!records || !lin)) return fail(CPI_EINVAL, "null pointer argument (records / lin)");
+    if (n_rec > 0 && out_records == records) return fail(CPI_EINVAL, "out_records must not overlap records");
+    if (n_rec == 0) return CPI_OK;             // only empty groups: nothing to write
+    DevInfo d;
+    if ((rc = device_info(d))) return rc;
+    std::lock_guard<std::mutex> lk(g_scratch_mu);
+    if ((rc = scratch_prepare())) return rc;
+    const size_t rb = (size_t)CPI_REC_V1_DOUBLES * es, lb = (size_t)CPI_LIN_DOUBLES * es;
+    // the device copies start at record b0; the offsets are shifted to match
+    void *d_r, *d_l, *d_o, *d_ws, *d_off = nullptr;
+    if ((rc = dev_buf(0, (size_t)n_rec * rb, &d_r))) return rc;
+    if ((rc = dev_buf(1, (size_t)n_rec * lb, &d_l))) return rc;
+    if ((rc = dev_buf(2, (size_t)n_rec * rb, &d_o))) return rc;
+    if ((rc = dev_buf(3, (size_t)cpi::scan_workspace_bytes(n_rec), &d_ws))) return rc;
+    std::string shifted;
+    if (group_offsets) {
+        if ((rc = dev_buf(4, (size_t)(n_groups + 1) * 8, &d_off))) return rc;
+        shifted.resize((size_t)(n_groups + 1) * 8);
+        int64_t* so = (int64_t*)&shifted[0];
+        for (int64_t g = 0; g <= n_groups; g++) so[g] = group_offsets[g] - b0;
+    }
+    cudaStream_t st = g_scratch.stream;
+    // every error path drains the stream before returning: async copies from / into the caller's buffers must not outlive the call
+#define CUX(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { rc = fail(CPI_ECUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); goto drain; } } while (0)
+    if (group_offsets) CUX(cudaMemcpyAsync(d_off, shifted.data(), (size_t)(n_groups + 1) * 8, cudaMemcpyHostToDevice, st));
+    CUX(cudaMemcpyAsync(d_r, (const char*)records + (size_t)b0 * rb, (size_t)n_rec * rb, cudaMemcpyHostToDevice, st));
+    CUX(cudaMemcpyAsync(d_l, (const char*)lin + (size_t)b0 * lb, (size_t)n_rec * lb, cudaMemcpyHostToDevice, st));
+    rc = cpi_scan_records(model, dtype, n_groups, (const int64_t*)d_off, group_uniform, d_r, d_l, d_o, d_ws, st);
+    if (rc) goto drain;
+    CUX(cudaMemcpyAsync((char*)out_records + (size_t)b0 * rb, d_o, (size_t)n_rec * rb, cudaMemcpyDeviceToHost, st));
 drain:
 #undef CUX
     {

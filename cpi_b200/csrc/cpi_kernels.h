@@ -49,6 +49,10 @@ cudaError_t chain_solve_launch(int64_t n_states, const double* D, const double* 
 // merge.cu: one merged model-1 record per group (dtype 64 or 32)
 cudaError_t merge_launch(int dtype, int64_t n_groups, const int64_t* offsets, int64_t uniform, const void* records, const void* lin,
                          void* out, cudaStream_t st);
+// scan.cu: inclusive scan of model-1 records within groups, one record per input record (dtype 64 or 32); n_bound >= the record count
+int64_t scan_workspace_bytes(int64_t n_records);
+cudaError_t scan_launch(int dtype, int64_t n_groups, const int64_t* offsets, int64_t uniform, int64_t n_bound, const void* records,
+                        const void* lin, void* out, void* workspace, int sms, cudaStream_t st, int* launches);
 cudaError_t retract_launch(int64_t n, const double* states, const double* xi, double* out, cudaStream_t st);
 
 }  // namespace cpi

@@ -193,6 +193,68 @@ def merge(model, records, lin, group_offsets=None, group=None, out=None, stream=
     return out
 
 
+def scan_host(model, records, lin, group_offsets=None, group=None):
+    """Inclusive scan of consecutive records within groups (``cpi_scan_records_host``): HOST numpy in and out, arguments as
+    ``merge_host``.  Returns an array shaped like ``records``: row i of group g (lo <= i < hi) is the record of records lo .. i, at the
+    linearisation point of record lo (row hi - 1 is the group's ``merge_host`` result up to rounding, row lo a copy of record lo).
+    Rows outside every group are zero."""
+    lib = capi.load()
+    records = np.asarray(records)
+    dtype = np.dtype(np.float32) if records.dtype == np.float32 else np.dtype(np.float64)
+    records = np.ascontiguousarray(records, dtype=dtype).reshape(-1, REC_DOUBLES.get(model, REC_DOUBLES[1]))   # the library rejects model 2
+    lin = np.ascontiguousarray(lin, dtype=dtype).reshape(-1, 13)
+    if lin.shape[0] != records.shape[0]:
+        raise ValueError("lin must hold one linearisation point per record")
+    offs = None if group_offsets is None else np.ascontiguousarray(group_offsets, dtype=np.int64)
+    n, uniform = _merge_layout(records.shape[0], offs, group, 0 if offs is None else offs.shape[0])
+    if offs is not None and offs.shape[0] and offs[-1] > records.shape[0]:
+        raise ValueError("group_offsets run past the record array")
+    out = np.zeros_like(records)
+    capi.check(lib.cpi_scan_records_host(model, 8 * dtype.itemsize, n, _ptr(offs), uniform, _ptr(records), _ptr(lin), _ptr(out)))
+    return out
+
+
+def scan(model, records, lin, group_offsets=None, group=None, out=None, stream=None, workspace=None):
+    """Inclusive scan of consecutive records within groups on the device (``cpi_scan_records``): CUDA tensors as ``merge``; enqueues on
+    ``stream`` (default: torch's current stream) and does not synchronise.  Layout and result as ``scan_host``; ``out`` (shaped like
+    ``records``, default zeros) must not overlap ``records``, and only its rows inside a group are written.  ``workspace``: a CUDA tensor
+    of at least ``cpi_scan_records_workspace`` bytes, allocated here when absent or too small; pass one to keep the call
+    allocation-free."""
+    import torch
+
+    lib = capi.load()
+    if not (records.is_cuda and lin.is_cuda):
+        raise ValueError("scan() takes CUDA tensors; use scan_host() for host arrays")
+    if records.dtype not in (torch.float64, torch.float32) or lin.dtype != records.dtype:
+        raise ValueError("records and lin must both be float64 or both float32")
+    dev = records.device
+    for name, t in (("lin", lin), ("group_offsets", group_offsets), ("out", out), ("workspace", workspace)):
+        if t is not None and t.device != dev:
+            raise ValueError(f"{name} lives on {t.device}, records on {dev}: all tensors of one call must be on the same CUDA device")
+    rd = REC_DOUBLES[1]
+    records = records.contiguous(); lin = lin.contiguous()
+    n_rec = records.numel() // rd
+    if lin.numel() != 13 * n_rec:
+        raise ValueError("lin must hold one linearisation point per record")
+    if group_offsets is not None:
+        group_offsets = group_offsets.contiguous()
+        if group_offsets.dtype != torch.int64:
+            raise ValueError("group_offsets must be int64")
+    n, uniform = _merge_layout(n_rec, group_offsets, group, 0 if group_offsets is None else group_offsets.numel())
+    if out is None:
+        out = torch.zeros((n_rec, rd), dtype=records.dtype, device=dev)
+    elif out.numel() < n_rec * rd or not out.is_contiguous() or out.dtype != records.dtype:
+        raise ValueError("out must be a contiguous tensor of n_records * 290 elements in the records' dtype")
+    nbytes = int(lib.cpi_scan_records_workspace(max(n, 0), n_rec))
+    if workspace is None or workspace.numel() * workspace.element_size() < nbytes or not workspace.is_contiguous():
+        workspace = torch.empty((nbytes + 7) // 8, dtype=torch.float64, device=dev)
+    with torch.cuda.device(dev):
+        st = stream if stream is not None else torch.cuda.current_stream(dev)
+        capi.check(lib.cpi_scan_records(model, 64 if records.dtype == torch.float64 else 32, n, _tptr(group_offsets), uniform,
+                                        _tptr(records), _tptr(lin), _tptr(out), _tptr(workspace), ctypes.c_void_p(st.cuda_stream)))
+    return out
+
+
 # ------------------------------------------------------------------------------------------------------------------
 # reference-shaped objects
 # ------------------------------------------------------------------------------------------------------------------

@@ -177,6 +177,33 @@ int cpi_merge_records(int model, int dtype, int64_t n_groups, const int64_t* gro
 int cpi_merge_records_host(int model, int dtype, int64_t n_groups, const int64_t* group_offsets, int64_t group_uniform,
                            const void* records, const void* lin, void* out_records);
 
+/*
+ * Inclusive scan of consecutive model-1 records within groups: the record from a group's first keyframe to EVERY later boundary.
+ * Used for dead reckoning of a chain from one anchor (cpi_predict_state_batch of the anchor state with every scanned record gives
+ * every keyframe's state in one launch), and for records at intermediate times of a long window (cut it into S segments,
+ * preintegrate them as one CSR batch, scan: a record at every segment boundary, computed in parallel).
+ *   model, dtype, group_offsets, group_uniform, records, lin   as cpi_merge_records
+ *   out_records    device, one record per INPUT record, indexed like `records`: for record i of group g (lo <= i < hi), out[i] is the
+ *                  record of records lo .. i, at the linearisation point of record lo (every record moved there as the merge does it).
+ *                  out[hi-1] is the group's cpi_merge_records result up to rounding; out[lo] is a bitwise copy of records[lo].  An
+ *                  empty group writes nothing, and entries outside every group (before group_offsets[0]) are left untouched.  Must
+ *                  not overlap `records`.
+ *   workspace      device, cpi_scan_records_workspace(n_groups, n_records) bytes, n_records >= the records the groups span
+ *                  (group_offsets[n_groups] - group_offsets[0], or n_groups * group_uniform).  Never NULL.
+ * A segmented reduce-then-scan over chunks of 32 records: every group, however long, is spread over many CTAs, at a depth
+ * logarithmic in the merges (DESIGN.md "Scanning records").  Allocates nothing and does not synchronise; about 2 log32(n) + 1
+ * kernel launches for n records (device offsets: the bound of the records that fit in device memory, the levels the data does not
+ * reach returning at once).
+ */
+int64_t cpi_scan_records_workspace(int64_t n_groups, int64_t n_records);
+int cpi_scan_records(int model, int dtype, int64_t n_groups, const int64_t* group_offsets, int64_t group_uniform,
+                     const void* records, const void* lin, void* out_records, void* workspace, void* stream);
+
+/* Same with HOST buffers (H2D + kernels + D2H through device buffers owned by the library, synchronous); group_offsets is a HOST
+ * array, checked as in cpi_merge_records_host. */
+int cpi_scan_records_host(int model, int dtype, int64_t n_groups, const int64_t* group_offsets, int64_t group_uniform,
+                          const void* records, const void* lin, void* out_records);
+
 /* ---- factor evaluation ------------------------------------------------------------------------------------------- */
 
 /*
