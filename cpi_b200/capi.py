@@ -34,6 +34,8 @@ SYMBOLS = {
     "cpi_imu_chain_solve_workspace": (c_i64, [c_i64]),
     "cpi_imu_chain_solve": (c_int, [c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "cpi_predict_state_batch": (c_int, [c_int, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "cpi_propagate_batch": (c_int, [c_int, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "cpi_propagate_batch_host": (c_int, [c_int, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "cpi_retract_batch": (c_int, [c_i64, c_vp, c_vp, c_vp, c_vp]),
     "cpi_host_last_timing": (c_int, [c_vp, c_vp]),
     "cpi_host_register": (c_int, [c_vp, ctypes.c_size_t]),

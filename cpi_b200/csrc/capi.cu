@@ -647,6 +647,88 @@ drain:
     return rc;
 }
 
+}  // extern "C"
+
+namespace {
+// argument checks shared by the two propagation entry points (no CUDA call)
+int propagate_check(int model, int64_t n, const double* states_k, const double* cov_k, const double* records, const double* lin,
+                    const double* states_k1, const double* cov_k1, const double* cross) {
+    if (model != 1 && model != 2) return fail(CPI_EINVAL, "model must be 1 or 2 (got %d)", model);
+    if (n < 0) return fail(CPI_EINVAL, "negative count");
+    if (n == 0) return CPI_OK;
+    if (!states_k || !cov_k || !records || !lin || !states_k1 || !cov_k1) return fail(CPI_EINVAL, "null pointer argument");
+    const void* ins[4] = {states_k, cov_k, records, lin};
+    const void* outs[3] = {states_k1, cov_k1, cross};
+    for (const void* o : outs)
+        for (const void* q : ins)
+            if (o && o == q) return fail(CPI_EINVAL, "outputs must not overlap inputs");
+    if (states_k1 == cov_k1 || (cross && (cross == states_k1 || cross == cov_k1))) return fail(CPI_EINVAL, "outputs must not overlap each other");
+    return CPI_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int cpi_propagate_batch(int model, int64_t n, const double* states_k, const double* cov_k, const int64_t* anchor, const double* records,
+                        const double* lin, double* states_k1, double* cov_k1, double* cross, void* stream) {
+    int rc = propagate_check(model, n, states_k, cov_k, records, lin, states_k1, cov_k1, cross);
+    if (rc || n == 0) return rc;
+    DevInfo d;
+    if ((rc = device_info(d))) return rc;
+    cpi::PropagateParams p{n, states_k, cov_k, anchor, records, lin, states_k1, cov_k1, cross};
+    CU(cpi::propagate_launch(model, p, (cudaStream_t)stream));
+    g_launches += 1;
+    return CPI_OK;
+}
+
+int cpi_propagate_batch_host(int model, int64_t n, int64_t n_anchors, const double* states_k, const double* cov_k, const int64_t* anchor,
+                             const double* records, const double* lin, double* states_k1, double* cov_k1, double* cross) {
+    if (n_anchors < 0) return fail(CPI_EINVAL, "negative count");
+    int rc = propagate_check(model, n, states_k, cov_k, records, lin, states_k1, cov_k1, cross);
+    if (rc || n == 0) return rc;
+    if (!anchor && n_anchors < n) return fail(CPI_EINVAL, "without an anchor array window i starts from entry i: n_anchors must be >= n");
+    if (anchor)
+        for (int64_t i = 0; i < n; i++)
+            if (anchor[i] < 0 || anchor[i] >= n_anchors)
+                return fail(CPI_EINVAL, "window %lld: anchor index %lld out of range [0, %lld)", (long long)i, (long long)anchor[i], (long long)n_anchors);
+    const int64_t na = anchor ? n_anchors : n;           // anchor entries the windows read
+    const size_t rb = (size_t)cpi_record_doubles(model) * 8;
+    DevInfo d;
+    if ((rc = device_info(d))) return rc;
+    std::lock_guard<std::mutex> lk(g_scratch_mu);
+    if ((rc = scratch_prepare())) return rc;
+    void *d_x, *d_c, *d_r, *d_l, *d_a = nullptr, *d_x1, *d_c1, *d_cr = nullptr;
+    if ((rc = dev_buf(0, (size_t)na * CPI_STATE_DOUBLES * 8, &d_x))) return rc;
+    if ((rc = dev_buf(1, (size_t)na * 225 * 8, &d_c))) return rc;
+    if ((rc = dev_buf(2, (size_t)n * rb, &d_r))) return rc;
+    if ((rc = dev_buf(3, (size_t)n * CPI_LIN_DOUBLES * 8, &d_l))) return rc;
+    if (anchor && (rc = dev_buf(4, (size_t)n * 8, &d_a))) return rc;
+    if ((rc = dev_buf(5, (size_t)n * CPI_STATE_DOUBLES * 8, &d_x1))) return rc;
+    if ((rc = dev_buf(6, (size_t)n * 225 * 8, &d_c1))) return rc;
+    if (cross && (rc = dev_buf(7, (size_t)n * 225 * 8, &d_cr))) return rc;
+    cudaStream_t st = g_scratch.stream;
+    // every error path drains the stream before returning: async copies from / into the caller's buffers must not outlive the call
+#define CUX(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { rc = fail(CPI_ECUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); goto drain; } } while (0)
+    CUX(cudaMemcpyAsync(d_x, states_k, (size_t)na * CPI_STATE_DOUBLES * 8, cudaMemcpyHostToDevice, st));
+    CUX(cudaMemcpyAsync(d_c, cov_k, (size_t)na * 225 * 8, cudaMemcpyHostToDevice, st));
+    CUX(cudaMemcpyAsync(d_r, records, (size_t)n * rb, cudaMemcpyHostToDevice, st));
+    CUX(cudaMemcpyAsync(d_l, lin, (size_t)n * CPI_LIN_DOUBLES * 8, cudaMemcpyHostToDevice, st));
+    if (anchor) CUX(cudaMemcpyAsync(d_a, anchor, (size_t)n * 8, cudaMemcpyHostToDevice, st));
+    rc = cpi_propagate_batch(model, n, (const double*)d_x, (const double*)d_c, (const int64_t*)d_a, (const double*)d_r, (const double*)d_l,
+                             (double*)d_x1, (double*)d_c1, (double*)d_cr, st);
+    if (rc) goto drain;
+    CUX(cudaMemcpyAsync(states_k1, d_x1, (size_t)n * CPI_STATE_DOUBLES * 8, cudaMemcpyDeviceToHost, st));
+    CUX(cudaMemcpyAsync(cov_k1, d_c1, (size_t)n * 225 * 8, cudaMemcpyDeviceToHost, st));
+    if (cross) CUX(cudaMemcpyAsync(cross, d_cr, (size_t)n * 225 * 8, cudaMemcpyDeviceToHost, st));
+drain:
+#undef CUX
+    {
+        cudaError_t e_ = cudaStreamSynchronize(st);
+        if (e_ != cudaSuccess && rc == CPI_OK) rc = fail(CPI_ECUDA, "cudaStreamSynchronize failed: %s", cudaGetErrorString(e_));
+    }
+    return rc;
+}
+
 int cpi_retract_batch(int64_t n, const double* states, const double* xi, double* states_out, void* stream) {
     if (n < 0) return fail(CPI_EINVAL, "negative count");
     if (n == 0) return CPI_OK;

@@ -5,6 +5,18 @@
 
 namespace cpi {
 
+struct PropagateParams {
+    int64_t n;
+    const double* states;     // anchor states (CPI_STATE_DOUBLES each)
+    const double* cov;        // anchor covariances (225 each, column-major)
+    const int64_t* anchor;    // may be null: window i starts from entry i
+    const double* records;
+    const double* lin;
+    double* states_k1;
+    double* cov_k1;
+    double* cross;            // may be null
+};
+
 struct PreintParams {
     int64_t n_windows;
     const int64_t* offsets;   // device, may be null (uniform windows)
@@ -53,6 +65,8 @@ cudaError_t merge_launch(int dtype, int64_t n_groups, const int64_t* offsets, in
 int64_t scan_workspace_bytes(int64_t n_records);
 cudaError_t scan_launch(int dtype, int64_t n_groups, const int64_t* offsets, int64_t uniform, int64_t n_bound, const void* records,
                         const void* lin, void* out, void* workspace, int sms, cudaStream_t st, int* launches);
+// propagate.cu: prediction and covariance propagation through one record per window (fp64)
+cudaError_t propagate_launch(int model, const PropagateParams& p, cudaStream_t st);
 cudaError_t retract_launch(int64_t n, const double* states, const double* xi, double* out, cudaStream_t st);
 
 }  // namespace cpi

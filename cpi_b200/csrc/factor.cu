@@ -9,6 +9,7 @@
 // CTA's 32 consecutive factors are three contiguous ranges).
 #include "cpi_common.cuh"
 #include "cpi_kernels.h"
+#include "factor_blocks.cuh"
 
 namespace cpi {
 
@@ -23,22 +24,6 @@ constexpr int FTHREADS = 64;
 constexpr int FTILE = 15 + 225 + 225;   // doubles per factor in the staging tile
 
 
-// w*I - [v x]  (sign = -1)   or   w*I + [v x]  (sign = +1),  row-major
-CPI_DEV void quat_mat(const double* q, double sign, double* M) {
-    M[0] = q[3];            M[1] = -sign * q[2];   M[2] = sign * q[1];
-    M[3] = sign * q[2];     M[4] = q[3];           M[5] = -sign * q[0];
-    M[6] = -sign * q[1];    M[7] = sign * q[0];    M[8] = q[3];
-}
-CPI_DEV void skew(const double* v, double* M) {
-    M[0] = 0.0; M[1] = -v[2]; M[2] = v[1]; M[3] = v[2]; M[4] = 0.0; M[5] = -v[0]; M[6] = -v[1]; M[7] = v[0]; M[8] = 0.0;
-}
-// record 3x3 (column-major in global memory) -> row-major registers
-CPI_DEV void ldrec33(const double* r, double* M) {
-#pragma unroll
-    for (int i = 0; i < 3; i++)
-#pragma unroll
-        for (int j = 0; j < 3; j++) M[3 * i + j] = __ldg(r + i + 3 * j);
-}
 // write a row-major 3x3 (scaled) into a column-major 15x15 tile at block (r0, c0)
 CPI_DEV void put33(double* H, int r0, int c0, const double* M, double s) {
 #pragma unroll
@@ -227,23 +212,7 @@ __global__ void k_predict(int64_t n, const double* states, const double* records
     const double* x = states + i * CPI_STATE_DOUBLES;
     const double* r = records + i * (int64_t)RD;
     const double* l = lin + i * CPI_LIN_DOUBLES;
-    double* o = out + i * CPI_STATE_DOUBLES;
-    const double q[4] = {x[0], x[1], x[2], x[3]}, qm[4] = {r[0], r[1], r[2], r[3]}, qi[4] = {-x[0], -x[1], -x[2], x[3]};
-    const double dt = r[CPI_REC_DT];
-    double qn[4], Rinv[9], rb[3], ra[3];
-    quat_multiply(qm, q, qn);
-    quat_2_Rot(qi, Rinv);
-    const double be[3] = {r[CPI_REC_BETA], r[CPI_REC_BETA + 1], r[CPI_REC_BETA + 2]}, al[3] = {r[CPI_REC_ALPHA], r[CPI_REC_ALPHA + 1], r[CPI_REC_ALPHA + 2]};
-    mv33(Rinv, be, rb); mv33(Rinv, al, ra);
-#pragma unroll
-    for (int k = 0; k < 4; k++) o[k] = qn[k];
-#pragma unroll
-    for (int k = 0; k < 3; k++) {
-        const double v = x[7 + k], g = l[10 + k];
-        o[4 + k] = x[4 + k]; o[10 + k] = x[10 + k];
-        if (MODEL == 1) { o[7 + k] = v - g * dt + rb[k]; o[13 + k] = x[13 + k] + v * dt - 0.5 * g * (dt * dt) + ra[k]; }
-        else { o[7 + k] = v + rb[k]; o[13 + k] = x[13 + k] + v * dt + ra[k]; }
-    }
+    predict_state<MODEL>(x, r, l, out + i * CPI_STATE_DOUBLES);
 }
 
 // ---- JPLNavState::retract (JPLNavState.cpp:37-71) -----------------------------------------------------------------------

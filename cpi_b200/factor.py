@@ -192,6 +192,64 @@ def predict_state(model, states_k, records, lin, stream=None):
     return out.cpu().numpy() if host else out
 
 
+def propagate(model, states_k, cov_k, records, lin, anchor=None, want_cross=False, stream=None):
+    """Prediction with covariance (cpi_propagate_batch): x_k1 = predict_state(x_k, record), cov_k1 = A cov_k A^T + B P_meas B^T with
+    A = -H2^-1 H1, B = H2^-1 the factor Jacobians at (x_k, x_k1); cross = cov_k A^T.  DEVICE float64 tensors: states_k [m,16],
+    cov_k [m,225] (column-major 15x15), records [n,RD], lin [n,13], anchor int64 [n] or None (window i starts from entry anchor[i],
+    None: from entry i).  Enqueues on ``stream`` (default: torch's current stream) without synchronising.
+    Returns (states_k1 [n,16], cov_k1 [n,225], cross [n,225] or None)."""
+    import torch
+
+    lib = capi.load()
+    n = records.numel() // REC_DOUBLES[model]
+    dev = records.device
+    for name, t in (("states_k", states_k), ("cov_k", cov_k), ("lin", lin), ("anchor", anchor)):
+        if t is not None and (not t.is_cuda or t.device != dev):
+            raise ValueError(f"{name} must be a CUDA tensor on {dev}")
+    for name, t in (("states_k", states_k), ("cov_k", cov_k), ("records", records), ("lin", lin)):
+        if t.dtype != torch.float64:
+            raise ValueError(f"{name} must be float64")
+    m = states_k.numel() // 16
+    if cov_k.numel() != 225 * m or lin.numel() != 13 * n:
+        raise ValueError("cov_k needs 225 doubles per anchor state and lin 13 per record")
+    if anchor is None:
+        if m < n:
+            raise ValueError("without an anchor array window i starts from entry i: states_k needs one entry per record")
+    else:
+        if anchor.dtype != torch.int64 or anchor.numel() != n:
+            raise ValueError("anchor must be an int64 tensor with one entry per record")
+        anchor = anchor.contiguous()
+    x1 = torch.empty((n, 16), dtype=torch.float64, device=dev)
+    c1 = torch.empty((n, 225), dtype=torch.float64, device=dev)
+    cr = torch.empty((n, 225), dtype=torch.float64, device=dev) if want_cross else None
+    with torch.cuda.device(dev):
+        st = stream if stream is not None else torch.cuda.current_stream(dev)
+        capi.check(lib.cpi_propagate_batch(model, n, _tptr(states_k.contiguous()), _tptr(cov_k.contiguous()), _tptr(anchor),
+                                           _tptr(records.contiguous()), _tptr(lin.contiguous()), _tptr(x1), _tptr(c1), _tptr(cr),
+                                           ctypes.c_void_p(st.cuda_stream)))
+    return x1, c1, cr
+
+
+def propagate_host(model, states_k, cov_k, records, lin, anchor=None, want_cross=False):
+    """HOST numpy in/out through ``cpi_propagate_batch_host`` (synchronous); arguments and results as ``propagate``."""
+    lib = capi.load()
+    states_k = np.ascontiguousarray(states_k, dtype=np.float64).reshape(-1, 16)
+    cov_k = np.ascontiguousarray(cov_k, dtype=np.float64).reshape(-1, 225)
+    records = np.ascontiguousarray(records, dtype=np.float64).reshape(-1, REC_DOUBLES[model])
+    lin = np.ascontiguousarray(lin, dtype=np.float64).reshape(-1, 13)
+    n, m = records.shape[0], states_k.shape[0]
+    if lin.shape[0] != n or cov_k.shape[0] != m:
+        raise ValueError("one linearisation point per record and one covariance per anchor state required")
+    if anchor is not None:
+        anchor = np.ascontiguousarray(anchor, dtype=np.int64)
+        if anchor.shape != (n,):
+            raise ValueError("anchor must have one entry per record")
+    x1 = np.empty((n, 16)); c1 = np.empty((n, 225)); cr = np.empty((n, 225)) if want_cross else None
+    capi.check(lib.cpi_propagate_batch_host(model, n, m, _ptr(states_k), _ptr(cov_k), _ptr(anchor), _ptr(records), _ptr(lin),
+                                            _ptr(x1), _ptr(c1), _ptr(cr)))
+    return x1, c1, cr
+
+
 def retract(states, xi, stream=None):
     """JPLNavState::retract (gtsam/JPLNavState.cpp:37-71), batched."""
     import torch

@@ -277,6 +277,34 @@ int cpi_imu_chain_solve(int64_t n_states, const double* D, const double* E, cons
 int cpi_predict_state_batch(int model, int64_t n, const double* states_k, const double* records, const double* lin,
                             double* states_k1, void* stream);
 
+/*
+ * Prediction with covariance: the state x_{k+1} predicted from an anchor x_k and a record, and its 15x15 error covariance, for
+ * n windows at once.  Errors live in the tangent space of JPLNavState::retract (cpi_retract_batch; the factor Jacobians' convention).
+ * With H1, H2 the Jacobians cpi_imu_factor_eval_batch gives at (x_k, x_{k+1}):
+ *     A = -H2^-1 H1,  B = H2^-1,  cov_k1 = A cov_k A^T + B P_meas B^T,  cross = (A cov_k)^T  (= cov_k A^T, the x_k - x_{k+1} block)
+ * the linearisation of e(x_k, x_{k+1}) = 0 with the factor's own noise model (covariance P_meas).  One step of an EKF / MSCKF
+ * propagation, or, with every window anchored at one state and the records of cpi_scan_records, dead reckoning of a whole chain with
+ * its uncertainty in one launch (DESIGN.md "Propagating the covariance").
+ *   model      1 or 2 (fp64)
+ *   states_k   device, CPI_STATE_DOUBLES per anchor entry;  cov_k  device, 225 doubles (column-major 15x15) per anchor entry,
+ *              symmetric (it is read whole)
+ *   anchor     device int64[n], or NULL: window i starts from entry anchor[i] of states_k / cov_k (NULL: entry i).  Device-resident
+ *              indices cannot be validated by this entry point (the _host variant checks them)
+ *   records    device, one record per window;  lin  device, CPI_LIN_DOUBLES per window
+ *   states_k1  device, CPI_STATE_DOUBLES per window: bit for bit what cpi_predict_state_batch writes for the same inputs
+ *   cov_k1     device, 225 per window, exactly symmetric
+ *   cross      device, 225 per window, or NULL
+ * Outputs must not overlap inputs.  One kernel launch; does not synchronise.
+ */
+int cpi_propagate_batch(int model, int64_t n, const double* states_k, const double* cov_k, const int64_t* anchor,
+                        const double* records, const double* lin, double* states_k1, double* cov_k1, double* cross, void* stream);
+
+/* Same with HOST buffers (H2D + kernel + D2H through device buffers owned by the library, synchronous).  states_k / cov_k hold
+ * n_anchors entries; anchor (HOST, may be NULL: then n_anchors >= n) is checked against n_anchors before anything reaches the device. */
+int cpi_propagate_batch_host(int model, int64_t n, int64_t n_anchors, const double* states_k, const double* cov_k,
+                             const int64_t* anchor, const double* records, const double* lin,
+                             double* states_k1, double* cov_k1, double* cross);
+
 /* JPLNavState::retract (JPLNavState.cpp:37-71): states_out[i] = states[i] (+) xi[i], xi = 15 doubles each. */
 int cpi_retract_batch(int64_t n, const double* states, const double* xi, double* states_out, void* stream);
 
