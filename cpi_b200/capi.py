@@ -33,6 +33,9 @@ SYMBOLS = {
     "cpi_imu_chain_assemble": (c_int, [c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, ctypes.c_double, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "cpi_imu_chain_solve_workspace": (c_i64, [c_i64]),
     "cpi_imu_chain_solve": (c_int, [c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "cpi_imu_chains_assemble": (c_int, [c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, ctypes.c_double, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "cpi_imu_chain_marginalize": (c_int, [c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "cpi_imu_prior_at": (c_int, [c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "cpi_predict_state_batch": (c_int, [c_int, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "cpi_propagate_batch": (c_int, [c_int, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "cpi_propagate_batch_host": (c_int, [c_int, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),

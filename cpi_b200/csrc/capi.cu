@@ -439,7 +439,78 @@ int cpi_imu_chain_assemble(int64_t n_factors, const double* G11, const double* G
     DevInfo d;
     int rc = device_info(d);
     if (rc) return rc;
-    CU(cpi::chain_assemble_launch(n_factors, G11, G12, G22, g1, g2, lambda, diagonal_damping != 0, prior_info0, prior_rhs0, D, E, rhs, (cudaStream_t)stream));
+    CU(cpi::chains_assemble_launch(1, nullptr, n_factors + 1, G11, G12, G22, g1, g2, lambda, diagonal_damping != 0, prior_info0, prior_rhs0, D, E, rhs,
+                                   d.sms, (cudaStream_t)stream));
+    g_launches += 1;
+    return CPI_OK;
+}
+
+}  // extern "C"
+
+namespace {
+// the chain layout shared by the many-chain entry points: chain_offsets (device, not inspected here) or chain_uniform >= 1 states per chain
+int chain_layout_check(int64_t n_chains, const int64_t* chain_offsets, int64_t chain_uniform) {
+    if (n_chains < 0) return fail(CPI_EINVAL, "negative count");
+    if (n_chains > ((int64_t)1 << 31)) return fail(CPI_EINVAL, "too many chains (%lld; at most 2^31 per call)", (long long)n_chains);
+    if (!chain_offsets && chain_uniform < 1) return fail(CPI_EINVAL, "chain_uniform must be >= 1 state per chain (got %lld)", (long long)chain_uniform);
+    if (!chain_offsets && n_chains > 0 && chain_uniform > ((int64_t)1 << 40) / n_chains)
+        return fail(CPI_EINVAL, "chain_uniform out of range: %lld x %lld states", (long long)n_chains, (long long)chain_uniform);
+    return CPI_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int cpi_imu_chains_assemble(int64_t n_chains, const int64_t* chain_offsets, int64_t chain_uniform, const double* G11, const double* G12,
+                            const double* G22, const double* g1, const double* g2, double lambda, int diagonal_damping,
+                            const double* prior_info, const double* prior_rhs, double* D, double* E, double* rhs, void* stream) {
+    int rc = chain_layout_check(n_chains, chain_offsets, chain_uniform);
+    if (rc || n_chains == 0) return rc;
+    const bool any_factor = chain_offsets || chain_uniform > 1;   // a device layout may hold factors
+    if (!D || !rhs) return fail(CPI_EINVAL, "null pointer argument (D / rhs)");
+    if (any_factor && (!G11 || !G12 || !G22 || !g1 || !g2)) return fail(CPI_EINVAL, "null pointer argument (G11 / G12 / G22 / g1 / g2)");
+    if ((chain_offsets || n_chains * chain_uniform > 1) && !E) return fail(CPI_EINVAL, "null pointer argument (E)");
+    if (!(lambda >= 0.0)) return fail(CPI_EINVAL, "lambda must be >= 0 (got %g)", lambda);
+    DevInfo d;
+    if ((rc = device_info(d))) return rc;
+    CU(cpi::chains_assemble_launch(n_chains, chain_offsets, chain_uniform, G11, G12, G22, g1, g2, lambda, diagonal_damping != 0, prior_info, prior_rhs,
+                                   D, E, rhs, d.sms, (cudaStream_t)stream));
+    g_launches += 1;
+    return CPI_OK;
+}
+
+int cpi_imu_chain_marginalize(int64_t n_chains, const int64_t* chain_offsets, int64_t chain_uniform, const int64_t* n_marg, int64_t n_marg_uniform,
+                              const double* G11, const double* G12, const double* G22, const double* g1, const double* g2, const double* f,
+                              const double* prior_info, const double* prior_rhs, const double* prior_f,
+                              double* out_info, double* out_rhs, double* out_f, void* stream) {
+    int rc = chain_layout_check(n_chains, chain_offsets, chain_uniform);
+    if (rc || n_chains == 0) return rc;
+    if (!n_marg && n_marg_uniform < 0) return fail(CPI_EINVAL, "negative count (n_marg_uniform)");
+    if (!n_marg && !chain_offsets && n_marg_uniform >= chain_uniform)
+        return fail(CPI_EINVAL, "n_marg_uniform (%lld) must be < the states per chain (%lld): a chain keeps at least one state",
+                    (long long)n_marg_uniform, (long long)chain_uniform);
+    if (!out_info || !out_rhs) return fail(CPI_EINVAL, "null pointer argument (out_info / out_rhs)");
+    if ((prior_info == nullptr) != (prior_rhs == nullptr)) return fail(CPI_EINVAL, "prior_info and prior_rhs must both be given or both be null");
+    const bool any_factor = n_marg || n_marg_uniform > 0;
+    if (any_factor && (!G11 || !G12 || !G22 || !g1 || !g2 || !f)) return fail(CPI_EINVAL, "null pointer argument (G11 / G12 / G22 / g1 / g2 / f)");
+    DevInfo d;
+    if ((rc = device_info(d))) return rc;
+    CU(cpi::marginalize_launch(n_chains, chain_offsets, chain_uniform, n_marg, n_marg_uniform, G11, G12, G22, g1, g2, f, prior_info, prior_rhs, prior_f,
+                               out_info, out_rhs, out_f, (cudaStream_t)stream));
+    g_launches += 1;
+    return CPI_OK;
+}
+
+int cpi_imu_prior_at(int64_t n, const double* info, const double* rhs, const double* f, const double* lin_states, const double* states,
+                     double* rhs_out, double* f_out, void* stream) {
+    if (n < 0) return fail(CPI_EINVAL, "negative count");
+    if (n == 0) return CPI_OK;
+    if (n > ((int64_t)1 << 31)) return fail(CPI_EINVAL, "too many priors (%lld; at most 2^31 per call)", (long long)n);
+    if (!info || !rhs || !lin_states || !states || !rhs_out) return fail(CPI_EINVAL, "null pointer argument");
+    DevInfo d;
+    int rc = device_info(d);
+    if (rc) return rc;
+    CU(cpi::prior_at_launch(n, info, rhs, f, lin_states, states, rhs_out, f_out, (cudaStream_t)stream));
     g_launches += 1;
     return CPI_OK;
 }

@@ -54,8 +54,10 @@ cudaError_t predict_launch(int model, int64_t n, const double* states, const dou
 cudaError_t hessian_launch(int rd, int64_t n, const double* records, const double* e, const double* H1, const double* H2,
                            double* G11, double* G12, double* G22, double* g1, double* g2, double* f, cudaStream_t st);
 cudaError_t whiten_launch(int rd, int64_t n, const double* records, const double* e, const double* H1, const double* H2, double* A1, double* A2, double* b, cudaStream_t st);
-cudaError_t chain_assemble_launch(int64_t nf, const double* G11, const double* G12, const double* G22, const double* g1, const double* g2, double lambda,
-                                  int diagonal_damping, const double* prior_info, const double* prior_rhs, double* D, double* E, double* rhs, cudaStream_t st);
+// solve.cu: block-tridiagonal normal equations of n_chains chains (offs: device int64[n_chains+1], or NULL and `uniform` states per chain)
+cudaError_t chains_assemble_launch(int64_t n_chains, const int64_t* offs, int64_t uniform, const double* G11, const double* G12, const double* G22,
+                                   const double* g1, const double* g2, double lambda, int diagonal_damping, const double* prior_info,
+                                   const double* prior_rhs, double* D, double* E, double* rhs, int sms, cudaStream_t st);
 int64_t chain_solve_workspace_bytes(int64_t n_states);
 cudaError_t chain_solve_launch(int64_t n_states, const double* D, const double* E, const double* b, double* x, double* ws, cudaStream_t st, int* launches);
 // merge.cu: one merged model-1 record per group (dtype 64 or 32)
@@ -67,6 +69,13 @@ cudaError_t scan_launch(int dtype, int64_t n_groups, const int64_t* offsets, int
                         const void* lin, void* out, void* workspace, int sms, cudaStream_t st, int* launches);
 // propagate.cu: prediction and covariance propagation through one record per window (fp64)
 cudaError_t propagate_launch(int model, const PropagateParams& p, cudaStream_t st);
+// marginalize.cu: elimination of the leading states of every chain into a prior (K8), and a prior moved to other states
+cudaError_t marginalize_launch(int64_t n_chains, const int64_t* offs, int64_t uniform, const int64_t* n_marg, int64_t marg_uniform,
+                               const double* G11, const double* G12, const double* G22, const double* g1, const double* g2, const double* f,
+                               const double* prior_info, const double* prior_rhs, const double* prior_f, double* out_info, double* out_rhs,
+                               double* out_f, cudaStream_t st);
+cudaError_t prior_at_launch(int64_t n, const double* info, const double* rhs, const double* f, const double* lin, const double* x,
+                            double* rhs_out, double* f_out, cudaStream_t st);
 cudaError_t retract_launch(int64_t n, const double* states, const double* xi, double* out, cudaStream_t st);
 
 }  // namespace cpi

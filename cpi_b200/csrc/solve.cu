@@ -10,47 +10,9 @@
 // CPU solves of the same system (tests/test_gpu_parity.py).
 #include "cpi_common.cuh"
 #include "cpi_kernels.h"
+#include "chol15.cuh"
 
 namespace cpi {
-
-// ---- warp-level 15x15 helpers (matrix in shared memory, row-major with pitch 16) ---------------------------------------------------
-// in-place lower Cholesky; a non-positive pivot gives NaN (GTSAM throws there)
-CPI_DEV void warp_chol15(double* L, int lane) {
-    for (int k = 0; k < 15; k++) {
-        const double d = sqrt(L[k * 16 + k]);
-        __syncwarp();
-        if (lane == 0) L[k * 16 + k] = d;
-        if (lane > k && lane < 15) L[lane * 16 + k] = L[lane * 16 + k] / d;
-        __syncwarp();
-        for (int t = lane; t < 120; t += 32) {
-            int i = 0, acc = 0;
-            while (acc + i + 1 <= t) { acc += i + 1; i++; }      // t -> (i, j) in the lower triangle incl. diagonal
-            const int j = t - acc;
-            if (j > k && i > k) L[i * 16 + j] -= L[i * 16 + k] * L[j * 16 + k];
-        }
-        __syncwarp();
-    }
-}
-// y = L^-1 b  for a per-lane right-hand side held in registers (b -> y in place)
-CPI_DEV void fwd15(const double* L, double* y) {
-#pragma unroll
-    for (int i = 0; i < 15; i++) {
-        double t = y[i];
-#pragma unroll
-        for (int k = 0; k < i; k++) t = fma(-L[i * 16 + k], y[k], t);
-        y[i] = t / L[i * 16 + i];
-    }
-}
-// x = L^-T r : lane k (< 15) passes r_k and receives x_k; column-oriented backward substitution with shuffles
-CPI_DEV double warp_bwd15(const double* L, double r, int lane) {
-    double x = 0.0;
-    for (int k = 14; k >= 0; k--) {
-        const double xk = __shfl_sync(0xffffffffu, r, k) / L[k * 16 + k];
-        if (lane == k) x = xk;
-        if (lane < k) r = fma(-L[k * 16 + lane], xk, r);          // (L^T)[lane, k] = L[k, lane]
-    }
-    return x;
-}
 
 // ---- explicitly whitened Jacobian form --------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(128) k_factor_whiten(int64_t n, int rd, const double* records, const double* e, const double* H1, const double* H2,
@@ -103,25 +65,44 @@ __global__ void __launch_bounds__(128) k_factor_whiten(int64_t n, int rd, const 
 }
 
 // ---- chain assembly ---------------------------------------------------------------------------------------------------------------
-// Factor f links states f and f+1:  D[k] = G22[k-1] + G11[k] (+ prior on x_0) + damping,  E[k] = G12[k] (block (k, k+1)),  rhs[k] = g2[k-1] + g1[k].
+// Many independent chains in one block-tridiagonal system.  Chain c holds states o[c] .. o[c+1]-1 of the concatenated states
+// (o = offs, or o[c] = c * uniform); its factors are stored back to back from index o[c] - c, so state k of chain c is linked to
+// state k+1 by factor k - c.  One chain (o = {0, nf+1}) is the chain x_0 - ... - x_nf with factor f linking states f and f+1.
+//   D[k] = G22[k-1-c] (k not first) + G11[k-c] (k not last) (+ prior_info[c] on the chain's first state) + damping
+//   E[k] = G12[k-c] (block (k, k+1)), exactly 0 where k is the last state of its chain,   rhs[k] = g2[k-1-c] + g1[k-c] (+ prior_rhs[c])
 // Damping as in GTSAM's LevenbergMarquardtParams: lambda I, or with diagonalDamping lambda * clamp(diag, minDiagonal 1e-6, maxDiagonal 1e32).
-__global__ void k_chain_assemble(int64_t nf, const double* G11, const double* G12, const double* G22, const double* g1, const double* g2, double lambda,
-                                 int diagonal_damping, const double* prior_info, const double* prior_rhs, double* D, double* E, double* rhs) {
-    const int64_t k = blockIdx.x;                                  // state index 0..nf
-    for (int t = threadIdx.x; t < 225; t += blockDim.x) {
-        double d = 0.0;
-        if (k > 0) d += G22[(k - 1) * 225 + t];
-        if (k < nf) { d += G11[k * 225 + t]; E[k * 225 + t] = G12[k * 225 + t]; }
-        if (k == 0 && prior_info) d += prior_info[t];
-        if (t % 16 == 0) d += diagonal_damping ? lambda * fmin(fmax(d, 1e-6), 1e32) : lambda;     // t = r + 15 c: diagonal when r == c  <=>  t % 16 == 0
-        D[k * 225 + t] = d;
-    }
-    for (int t = threadIdx.x; t < 15; t += blockDim.x) {
-        double v = 0.0;
-        if (k > 0) v += g2[(k - 1) * 15 + t];
-        if (k < nf) v += g1[k * 15 + t];
-        if (k == 0 && prior_rhs) v += prior_rhs[t];
-        rhs[k * 15 + t] = v;
+// Grid-stride over the states: the state count o[n_chains] of a device-resident layout is read here, not on the host.
+__global__ void k_chain_assemble(int64_t n_chains, const int64_t* offs, int64_t uniform, const double* G11, const double* G12, const double* G22,
+                                 const double* g1, const double* g2, double lambda, int diagonal_damping, const double* prior_info,
+                                 const double* prior_rhs, double* D, double* E, double* rhs) {
+    const int64_t ns = offs ? offs[n_chains] : n_chains * uniform;
+    for (int64_t k = blockIdx.x; k < ns; k += gridDim.x) {
+        int64_t c, lo, hi;
+        if (offs) {                                                // the chain holding k: last c with o[c] <= k (chains are non-empty)
+            int64_t a = 0, b = n_chains - 1;
+            while (a < b) { const int64_t mid = (a + b + 1) >> 1; if (offs[mid] <= k) a = mid; else b = mid - 1; }
+            c = a; lo = offs[c]; hi = offs[c + 1];
+        } else {
+            c = k / uniform; lo = c * uniform; hi = lo + uniform;
+        }
+        const bool first = k == lo, last = k == hi - 1;
+        const int64_t fr = k - c;                                  // the factor to the right of state k (if k is not last)
+        for (int t = threadIdx.x; t < 225; t += blockDim.x) {
+            double d = 0.0;
+            if (!first) d += G22[(fr - 1) * 225 + t];
+            if (!last) d += G11[fr * 225 + t];
+            if (k + 1 < ns) E[k * 225 + t] = last ? 0.0 : G12[fr * 225 + t];
+            if (first && prior_info) d += prior_info[c * 225 + t];
+            if (t % 16 == 0) d += diagonal_damping ? lambda * fmin(fmax(d, 1e-6), 1e32) : lambda;     // t = r + 15 c: diagonal when r == c  <=>  t % 16 == 0
+            D[k * 225 + t] = d;
+        }
+        for (int t = threadIdx.x; t < 15; t += blockDim.x) {
+            double v = 0.0;
+            if (!first) v += g2[(fr - 1) * 15 + t];
+            if (!last) v += g1[fr * 15 + t];
+            if (first && prior_rhs) v += prior_rhs[c * 15 + t];
+            rhs[k * 15 + t] = v;
+        }
     }
 }
 
@@ -250,9 +231,13 @@ cudaError_t whiten_launch(int rd, int64_t n, const double* records, const double
     return cudaGetLastError();
 }
 
-cudaError_t chain_assemble_launch(int64_t nf, const double* G11, const double* G12, const double* G22, const double* g1, const double* g2, double lambda,
-                                  int diagonal_damping, const double* prior_info, const double* prior_rhs, double* D, double* E, double* rhs, cudaStream_t st) {
-    k_chain_assemble<<<(int)(nf + 1), 128, 0, st>>>(nf, G11, G12, G22, g1, g2, lambda, diagonal_damping, prior_info, prior_rhs, D, E, rhs);
+cudaError_t chains_assemble_launch(int64_t n_chains, const int64_t* offs, int64_t uniform, const double* G11, const double* G12, const double* G22,
+                                   const double* g1, const double* g2, double lambda, int diagonal_damping, const double* prior_info,
+                                   const double* prior_rhs, double* D, double* E, double* rhs, int sms, cudaStream_t st) {
+    // uniform layout: one CTA per state (capped); device offsets: enough CTAs to fill the device, each striding over the states
+    const int64_t ns = offs ? (int64_t)sms * 16 : n_chains * uniform;
+    const int grid = (int)(ns < 2147483647 ? ns : 2147483647);
+    k_chain_assemble<<<grid, 128, 0, st>>>(n_chains, offs, uniform, G11, G12, G22, g1, g2, lambda, diagonal_damping, prior_info, prior_rhs, D, E, rhs);
     return cudaGetLastError();
 }
 

@@ -154,6 +154,179 @@ def chain_solve(D, E, rhs, stream=None, workspace=None):
     return x
 
 
+def _check_f64(dev, **tensors):
+    import torch
+
+    for name, t in tensors.items():
+        if t is None:
+            continue
+        if not t.is_cuda or t.device != dev:
+            raise ValueError(f"{name} must be a CUDA tensor on {dev}")
+        if t.dtype != torch.float64:
+            raise ValueError(f"{name} must be float64")
+
+
+def _chain_layout(chain_offsets, dev, n_factors=None, n_states=None, n_chains=None):
+    """(n_chains, offsets tensor or None, states per chain) of a chain layout: a device int64 tensor [n_chains+1] of state offsets
+    (offsets[0] = 0, every chain non-empty), or an int, the states per chain, with the chain count taken from n_chains, n_states or
+    n_factors (each chain of S states has S - 1 factors)."""
+    import torch
+
+    if isinstance(chain_offsets, torch.Tensor):
+        if not chain_offsets.is_cuda or chain_offsets.device != dev or chain_offsets.dtype != torch.int64 or chain_offsets.dim() != 1:
+            raise ValueError(f"chain_offsets must be a 1-d int64 CUDA tensor on {dev}")
+        if chain_offsets.numel() < 1:
+            raise ValueError("chain_offsets needs n_chains + 1 entries")
+        return chain_offsets.numel() - 1, chain_offsets.contiguous(), 0
+    S = int(chain_offsets)
+    if S < 1:
+        raise ValueError("a chain holds at least one state")
+    if n_chains is None:
+        if n_states is not None:
+            n_chains = n_states // S
+        elif S > 1:
+            n_chains = n_factors // (S - 1)
+        else:
+            raise ValueError("single-state chains hold no factor: pass n_chains")
+    if (n_states is not None and n_states != n_chains * S) or (n_factors is not None and n_factors != n_chains * (S - 1)):
+        raise ValueError(f"{n_chains} chains of {S} states do not match the given states / factors")
+    return int(n_chains), None, S
+
+
+def chains_assemble(G11, G12, G22, g1, g2, chain_offsets, lam=0.0, prior_info=None, prior_rhs=None, diagonal_damping=False, n_chains=None,
+                    stream=None):
+    """Block-tridiagonal normal equations of many independent chains at once (cpi_imu_chains_assemble).  chain_offsets: device int64
+    [n_chains+1] state offsets, or an int (states per chain; n_chains is then taken from the factor count unless given).  Chain c's
+    factors are stored back to back from index offsets[c] - c.  prior_info [n_chains,225] / prior_rhs [n_chains,15] (each may be None) go
+    on every chain's first state; damping as chain_assemble.  E is exactly 0 at chain boundaries, so chain_solve(D, E, rhs) solves every
+    chain at once -- provided every chain is SPD (a NaN pivot spreads into the neighbouring chains).
+    Returns (D [N,225], E [N-1,225], rhs [N,15]) for the N = n_factors + n_chains states."""
+    import torch
+
+    dev = G11.device
+    _check_f64(dev, G11=G11, G12=G12, G22=G22, g1=g1, g2=g2, prior_info=prior_info, prior_rhs=prior_rhs)
+    nf = G11.numel() // 225
+    C, offs, S = _chain_layout(chain_offsets, dev, n_factors=nf, n_chains=n_chains)
+    if any(t.numel() != k * nf for t, k in ((G11, 225), (G12, 225), (G22, 225), (g1, 15), (g2, 15))):
+        raise ValueError("G11 / G12 / G22 need 225 doubles and g1 / g2 15 per factor")
+    if (prior_info is not None and prior_info.numel() != 225 * C) or (prior_rhs is not None and prior_rhs.numel() != 15 * C):
+        raise ValueError("prior_info needs 225 doubles and prior_rhs 15 per chain")
+    N = nf + C
+    D = torch.empty((N, 225), dtype=torch.float64, device=dev)
+    E = torch.empty((max(N - 1, 1), 225), dtype=torch.float64, device=dev)
+    rhs = torch.empty((N, 15), dtype=torch.float64, device=dev)
+    with torch.cuda.device(dev):
+        st = stream if stream is not None else torch.cuda.current_stream(dev)
+        capi.check(capi.load().cpi_imu_chains_assemble(C, _tptr(offs), S, _tptr(G11.contiguous()), _tptr(G12.contiguous()), _tptr(G22.contiguous()),
+                                                       _tptr(g1.contiguous()), _tptr(g2.contiguous()), float(lam), int(bool(diagonal_damping)),
+                                                       _tptr(None if prior_info is None else prior_info.contiguous()),
+                                                       _tptr(None if prior_rhs is None else prior_rhs.contiguous()), _tptr(D), _tptr(E), _tptr(rhs),
+                                                       ctypes.c_void_p(st.cuda_stream)))
+    return D, E[:N - 1], rhs
+
+
+def chain_marginalize(G11, G12, G22, g1, g2, f, chain_offsets, n_marg, prior=None, n_chains=None, stream=None):
+    """Eliminate the first n_marg states of every chain into a dense prior on the first state it keeps (cpi_imu_chain_marginalize,
+    kernel K8): the Schur complement a fixed-lag smoother keeps of the states that leave its window, at the linearisation point of the
+    blocks, undamped.  Blocks as factor_hessian returns them (chain layout as chains_assemble); n_marg: int or device int64 [n_chains]
+    (0 <= n_marg < states of the chain); prior: (info [n_chains,225], rhs [n_chains,15], f [n_chains]) on every chain's first state, or
+    None.  Returns the prior on state offsets[c] + n_marg[c]: (info [n_chains,225] exactly symmetric, rhs [n_chains,15], f [n_chains])."""
+    import torch
+
+    dev = G11.device
+    _check_f64(dev, G11=G11, G12=G12, G22=G22, g1=g1, g2=g2, f=f)
+    nf = G11.numel() // 225
+    C, offs, S = _chain_layout(chain_offsets, dev, n_factors=nf, n_chains=n_chains)
+    if any(t.numel() != k * nf for t, k in ((G11, 225), (G12, 225), (G22, 225), (g1, 15), (g2, 15), (f, 1))):
+        raise ValueError("G11 / G12 / G22 need 225 doubles, g1 / g2 15 and f 1 per factor")
+    pi = pr = pf = None
+    if prior is not None:
+        pi, pr, pf = prior
+        _check_f64(dev, prior_info=pi, prior_rhs=pr, prior_f=pf)
+        if pi.numel() != 225 * C or pr.numel() != 15 * C or (pf is not None and pf.numel() != C):
+            raise ValueError("the prior needs info [n_chains,225], rhs [n_chains,15] and f [n_chains]")
+        pi, pr, pf = pi.contiguous(), pr.contiguous(), (None if pf is None else pf.contiguous())
+    if isinstance(n_marg, torch.Tensor):
+        if not n_marg.is_cuda or n_marg.device != dev or n_marg.dtype != torch.int64 or n_marg.numel() != C:
+            raise ValueError(f"n_marg must be an int64 CUDA tensor on {dev} with one entry per chain")
+        nm, nmu = n_marg.contiguous(), 0
+    else:
+        nm, nmu = None, int(n_marg)
+    info = torch.empty((C, 225), dtype=torch.float64, device=dev)
+    rhs = torch.empty((C, 15), dtype=torch.float64, device=dev)
+    fo = torch.empty((C,), dtype=torch.float64, device=dev)
+    with torch.cuda.device(dev):
+        st = stream if stream is not None else torch.cuda.current_stream(dev)
+        capi.check(capi.load().cpi_imu_chain_marginalize(C, _tptr(offs), S, _tptr(nm), nmu, _tptr(G11.contiguous()), _tptr(G12.contiguous()),
+                                                         _tptr(G22.contiguous()), _tptr(g1.contiguous()), _tptr(g2.contiguous()), _tptr(f.contiguous()),
+                                                         _tptr(pi), _tptr(pr), _tptr(pf), _tptr(info), _tptr(rhs), _tptr(fo),
+                                                         ctypes.c_void_p(st.cuda_stream)))
+    return info, rhs, fo
+
+
+def prior_at(info, rhs, f, lin_states, states, stream=None):
+    """A prior (info [n,225], rhs [n,15], f [n] or None) linearised at lin_states [n,16], moved to the states [n,16]
+    (cpi_imu_prior_at): delta = local(lin, x) (the inverse of retract), rhs' = rhs - info delta, f' = f - 2 rhs^T delta + delta^T info delta;
+    info is unchanged (the Jacobian of local taken as I, as GTSAM's LinearContainerFactor does).  Returns (rhs' [n,15], f' [n])."""
+    import torch
+
+    dev = info.device
+    _check_f64(dev, info=info, rhs=rhs, f=f, lin_states=lin_states, states=states)
+    n = info.numel() // 225
+    if info.numel() != 225 * n or rhs.numel() != 15 * n or (f is not None and f.numel() != n) or lin_states.numel() != 16 * n or states.numel() != 16 * n:
+        raise ValueError("prior_at needs info [n,225], rhs [n,15], f [n], lin_states and states [n,16]")
+    rhs_out = torch.empty((n, 15), dtype=torch.float64, device=dev)
+    f_out = torch.empty((n,), dtype=torch.float64, device=dev)
+    with torch.cuda.device(dev):
+        st = stream if stream is not None else torch.cuda.current_stream(dev)
+        capi.check(capi.load().cpi_imu_prior_at(n, _tptr(info.contiguous()), _tptr(rhs.contiguous()), _tptr(None if f is None else f.contiguous()),
+                                                _tptr(lin_states.contiguous()), _tptr(states.contiguous()), _tptr(rhs_out), _tptr(f_out),
+                                                ctypes.c_void_p(st.cuda_stream)))
+    return rhs_out, f_out
+
+
+def chains_lm_step(model, states, records, lin, chain_offsets, prior=None, lam=1e-5, diagonal_damping=True, stream=None):
+    """One damped Gauss-Newton step of many independent IMU-only chains at once (a fixed-lag smoother's windows), on the device:
+    evaluateError -> information blocks -> prior_at (every chain's prior moved to its current first state) -> chains_assemble ->
+    ONE block-cyclic-reduction solve over all chains -> retract.  states [N,16]; records / lin: the N - n_chains factors, chain c's
+    stored back to back from index offsets[c] - c; chain_offsets as chains_assemble (device int64 [n_chains+1], or states per chain);
+    prior: (info [n_chains,225], rhs [n_chains,15], f [n_chains], lin_states [n_chains,16]) or None.  lin_states = None: the prior is
+    linearised at the chains' current first states, so it is used as given without prior_at (rhs and f may then be None: zero).
+    Returns (new_states, delta [N,15], cost per chain before the step [n_chains] = sum of e^T P^-1 e + the moved prior's f')."""
+    import torch
+
+    dev = states.device
+    N = states.numel() // 16
+    C, offs, S = _chain_layout(chain_offsets, dev, n_states=N)
+    nf = N - C
+    if records.numel() != REC_DOUBLES[model] * nf:
+        raise ValueError(f"{C} chains over {N} states hold {nf} factors: one record each")
+    idx_i = idx_j = chain_of = None
+    if C > 1:                                                        # one chain: the eval kernel's own chain indexing
+        ar = torch.arange(nf, dtype=torch.int64, device=dev)
+        if offs is not None:
+            chain_of = torch.repeat_interleave(torch.arange(C, dtype=torch.int64, device=dev), offs[1:] - offs[:-1] - 1, output_size=nf)
+        else:
+            chain_of = ar // (S - 1) if S > 1 else ar
+        idx_i = ar + chain_of
+        idx_j = idx_i + 1
+    e, H1, H2 = factor_eval(model, states, records, lin, idx_i=idx_i, idx_j=idx_j, stream=stream)
+    G11, G12, G22, g1, g2, f = factor_hessian(model, records, e, H1, H2, stream=stream)
+    pi = pr = pf = None
+    if prior is not None:
+        pi, pr, pf, lin0 = prior
+        if lin0 is not None:
+            first = states.reshape(N, 16)[offs[:-1]] if offs is not None else states.reshape(N, 16)[::S]
+            pr, pf = prior_at(pi, pr, pf, lin0, first, stream=stream)
+    D, E, rhs = chains_assemble(G11, G12, G22, g1, g2, chain_offsets, lam, pi, pr, diagonal_damping=diagonal_damping, n_chains=C, stream=stream)
+    dx = chain_solve(D, E, rhs, stream=stream)
+    # per-chain cost: one chain sums like chain_lm_step always has; many chains scatter-add their factors' f
+    cost = f.sum().reshape(1) if C == 1 else torch.zeros(C, dtype=torch.float64, device=dev).index_add_(0, chain_of, f)
+    if pf is not None:
+        cost = cost + pf
+    return retract(states, dx, stream=stream), dx, cost
+
+
 _PRIOR = {}
 
 
@@ -162,18 +335,17 @@ def chain_lm_step(model, states, records, lin, lam=1e-5, prior_sigma=1e-4, strea
     evaluateError for every factor -> information blocks -> block-tridiagonal assembly (prior 1/prior_sigma^2 on x_0: the
     reference initialises with cov = 1e-8 I, GraphSolver.cpp:331; Marquardt damping lam * diag by default, lam = GTSAM's lambdaInitial:
     an undamped IMU-only chain of thousands of keyframes is numerically singular in fp64) -> block-cyclic-reduction solve -> JPLNavState::retract.
+    chains_lm_step on one chain, with the prior linearised at the current x_0 (no rhs, no constant: nothing to move).
     Returns (new_states, delta, cost = sum e^T P^-1 e before the step)."""
     import torch
 
     dev = states.device
     key = (dev, prior_sigma)
     if key not in _PRIOR:
-        _PRIOR[key] = (torch.eye(15, dtype=torch.float64, device=dev) / (prior_sigma * prior_sigma)).reshape(-1).contiguous()
-    e, H1, H2 = factor_eval(model, states, records, lin, stream=stream)
-    G11, G12, G22, g1, g2, f = factor_hessian(model, records, e, H1, H2, stream=stream)
-    D, E, rhs = chain_assemble(G11, G12, G22, g1, g2, lam, _PRIOR[key], None, stream=stream, diagonal_damping=diagonal_damping)
-    dx = chain_solve(D, E, rhs, stream=stream)
-    return retract(states, dx, stream=stream), dx, f.sum()
+        _PRIOR[key] = (torch.eye(15, dtype=torch.float64, device=dev) / (prior_sigma * prior_sigma)).reshape(1, 225).contiguous()
+    new_states, dx, cost = chains_lm_step(model, states, records, lin, states.numel() // 16, (_PRIOR[key], None, None, None), lam=lam,
+                                          diagonal_damping=diagonal_damping, stream=stream)
+    return new_states, dx, cost[0]
 
 
 def predict_state(model, states_k, records, lin, stream=None):

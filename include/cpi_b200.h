@@ -270,6 +270,49 @@ int64_t cpi_imu_chain_solve_workspace(int64_t n_states);
 int cpi_imu_chain_solve(int64_t n_states, const double* D, const double* E, const double* rhs,
                         double* x, void* workspace, void* stream);
 
+/*
+ * Many independent chains, and the fixed-lag smoother's marginalisation (BatchFixedLagSmoother, solvers/GraphSolver.h:93-97):
+ * DESIGN.md section 3e.  fp64, DEVICE pointers, asynchronous on `stream`, no allocation.  Models 1 and 2 alike (only the
+ * information blocks of cpi_imu_factor_hessian_batch are read).  PARITY UNPINNED (GTSAM is not in the reference tree); the numpy
+ * statements of tests/test_marginalize.py are the references.
+ *
+ * Chain layout: chain_offsets = device int64[n_chains+1] with chain_offsets[0] = 0, chain c holding the states o[c] .. o[c+1]-1
+ * of the concatenated states (at least one state each), or chain_offsets = NULL and chain_uniform (>= 1) states per chain.  Chain c
+ * has S_c - 1 factors, stored back to back from factor index o[c] - c: its factor k links states o[c]+k and o[c]+k+1 (n_states -
+ * n_chains factors in all).  A prior on a chain is (info[225] column-major, rhs[15], f), one of each per chain, in the HessianFactor
+ * convention: cost = 1/2 (f - 2 rhs^T delta + delta^T info delta).  A device-resident layout cannot be inspected by these entry points.
+ *
+ *   cpi_imu_chain_marginalize   eliminates the first m = n_marg[c] states of every chain (n_marg: device int64[n_chains], or NULL
+ *       and n_marg_uniform; 0 <= m < S_c) into a prior on state o[c] + m, at the linearisation point of the blocks, undamped:
+ *           Lambda, eta, f = the prior (or 0); for each eliminated factor k:  M = Lambda + G11_k = L L^T,  Z = L^-1 G12_k,
+ *           z = L^-1 (eta + g1_k);  Lambda <- G22_k - Z^T Z,  eta <- g2_k - Z^T z,  f <- f + f_k - z^T z
+ *       out_info is exactly symmetric.  m = 0 copies the prior bit for bit (zeros without one).  A non-positive pivot, or a
+ *       device-resident m out of range, gives NaN for that chain only.  G11 / G12 / G22 / g1 / g2 / f (the factors' constants) are
+ *       all required whenever a factor may be read (n_marg given, or n_marg_uniform > 0); prior_info / prior_rhs: both or neither;
+ *       prior_f, out_f may be NULL.  One warp per chain, sequential over its m factors: a long head (thousands of states) runs at
+ *       sequential depth.
+ *   cpi_imu_prior_at            the prior moved to the states x (one per prior): delta = local(lin_states, x), the exact inverse of
+ *       cpi_retract_batch (rotation vector of q_x (x) q_lin^-1, JPL, w >= 0; differences for the other 12 entries; exactly 0 at
+ *       x == lin_states), rhs_out = rhs - info delta, f_out = f - 2 rhs^T delta + delta^T info delta, info unchanged.  The Jacobian
+ *       of local is taken as the identity, as LinearContainerFactor does (UNPINNED).  f, f_out may be NULL; rhs_out may be rhs.
+ *   cpi_imu_chains_assemble     one block-tridiagonal system over all states: as cpi_imu_chain_assemble per chain (same damping),
+ *       prior c on chain c's first state (prior_info / prior_rhs may be NULL), E exactly 0 at chain boundaries, E = n_states - 1
+ *       blocks.  cpi_imu_chain_assemble is its n_chains = 1 case.  cpi_imu_chain_solve(n_states, D, E, rhs, ...) then solves every
+ *       chain at once: the zero couplings keep the chains exactly decoupled -- PROVIDED EVERY CHAIN IS SPD: a NaN pivot of one chain
+ *       spreads into its neighbours through 0 * NaN in the reduction.
+ */
+int cpi_imu_chain_marginalize(int64_t n_chains, const int64_t* chain_offsets, int64_t chain_uniform,
+                              const int64_t* n_marg, int64_t n_marg_uniform,
+                              const double* G11, const double* G12, const double* G22, const double* g1, const double* g2, const double* f,
+                              const double* prior_info, const double* prior_rhs, const double* prior_f,
+                              double* out_info, double* out_rhs, double* out_f, void* stream);
+int cpi_imu_prior_at(int64_t n, const double* info, const double* rhs, const double* f,
+                     const double* lin_states, const double* states, double* rhs_out, double* f_out, void* stream);
+int cpi_imu_chains_assemble(int64_t n_chains, const int64_t* chain_offsets, int64_t chain_uniform,
+                            const double* G11, const double* G12, const double* G22, const double* g1, const double* g2,
+                            double lambda, int diagonal_damping, const double* prior_info, const double* prior_rhs,
+                            double* D, double* E, double* rhs, void* stream);
+
 /* ---- callers either side of the factor ("next" rows) ----------------------------------------------------------------- */
 
 /* x_{k+1} prediction from x_k and a record: getpredictedstate_v1/_v2 (GraphSolver_IMU.cpp:263-307).
