@@ -146,6 +146,35 @@ def conditioned_gate(got, o64, truth, model, K, floor, allowance=None):
     return ratio, worst, bad
 
 
+def scaled_errors(got, truth, scale=None, sign_free=None):
+    """Per row [n, ...]: ||got - truth|| / scale, with scale = ||truth|| by default or an [n] array (the size of the terms that
+    cancel into the value).  Where the scale is 0 the error is 0 if got equals truth exactly and inf otherwise.  sign_free: [n] bool,
+    rows compared up to sign (a quaternion whose w is near 0)."""
+    g = np.asarray(got, dtype=np.float64); t = np.asarray(truth, dtype=np.float64)
+    n = t.shape[0]
+    g = g.reshape(n, -1); t = t.reshape(n, -1)
+    num = np.linalg.norm(g - t, axis=1)
+    if sign_free is not None:
+        num = np.where(sign_free, np.minimum(num, np.linalg.norm(g + t, axis=1)), num)
+    den = np.linalg.norm(t, axis=1) if scale is None else np.broadcast_to(np.asarray(scale, dtype=np.float64), (n,))
+    return np.where(den > 0, num / np.where(den > 0, den, 1.0), np.where(num > 0, np.inf, 0.0))
+
+
+def gate_errors(ed, e64, K, floor):
+    """The rule of ``conditioned_gate`` on precomputed per-field error arrays (dicts name -> [n]): e_dev <= K max(e_64, floor).
+    Returns (ratio, worst, failures) as conditioned_gate does; a non-finite e_dev fails."""
+    ratio, worst, bad = {}, {}, []
+    for k in ed:
+        bound = K * np.maximum(e64[k], floor)
+        r = np.where(np.isnan(ed[k]), np.inf, ed[k] / bound)
+        ratio[k] = r
+        i = int(np.argmax(r))
+        worst[k] = dict(e_dev=float(np.max(ed[k])), e_64=float(np.max(e64[k])), ratio=float(r[i]))
+        if not r[i] <= 1.0:
+            bad.append(f"{k}: row {i} e_dev {ed[k][i]:.3e} e_64 {e64[k][i]:.3e} bound {bound[i]:.3e}")
+    return ratio, worst, bad
+
+
 def fp32_errors(got, ref):
     """Worst relative error per record field of the fp32-storage variant against the fp64 oracle run on the same float-rounded
     inputs, plus the worst 3x3 block of P (relative to that block's norm; blocks that are exactly zero in the reference must
