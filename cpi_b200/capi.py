@@ -36,6 +36,12 @@ SYMBOLS = {
     "cpi_imu_chains_assemble": (c_int, [c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, ctypes.c_double, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "cpi_imu_chain_marginalize": (c_int, [c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "cpi_imu_prior_at": (c_int, [c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "cpi_imu_factor_cost_batch": (c_int, [c_int, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "cpi_imu_chains_assemble_lm": (c_int, [c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "cpi_imu_chains_solve_workspace": (c_i64, [c_i64, c_i64]),
+    "cpi_imu_chains_solve": (c_int, [c_i64, c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "cpi_imu_chains_lm_workspace": (c_i64, [c_i64]),
+    "cpi_imu_chains_lm_update": (c_int, [c_i64, c_vp, c_i64, c_i64, c_vp] + [c_vp] * 19),
     "cpi_predict_state_batch": (c_int, [c_int, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "cpi_propagate_batch": (c_int, [c_int, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "cpi_propagate_batch_host": (c_int, [c_int, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
@@ -62,6 +68,20 @@ SYMBOLS = {
 }
 
 REC_DOUBLES = {1: 290, 2: 308}
+# Levenberg-Marquardt chain status (CPI_LM_*)
+LM_RUNNING, LM_CONVERGED, LM_MAX_ITERATIONS, LM_LAMBDA_EXHAUSTED, LM_NONFINITE = 0, 1, 2, 3, 4
+
+
+class LMParams(ctypes.Structure):
+    """cpi_lm_params: GTSAM's LevenbergMarquardtParams defaults (useFixedLambdaFactor); the tolerances apply to GTSAM's error, half
+    the cost of factor.chains_lm."""
+    _fields_ = [("lambda_factor", ctypes.c_double), ("lambda_lower", ctypes.c_double), ("lambda_upper", ctypes.c_double),
+                ("min_model_fidelity", ctypes.c_double), ("absolute_error_tol", ctypes.c_double), ("relative_error_tol", ctypes.c_double),
+                ("max_iterations", c_i64)]
+
+    def __init__(self, lambda_factor=10.0, lambda_lower=0.0, lambda_upper=1e5, min_model_fidelity=1e-3, absolute_error_tol=1e-5,
+                 relative_error_tol=1e-5, max_iterations=100):
+        super().__init__(lambda_factor, lambda_lower, lambda_upper, min_model_fidelity, absolute_error_tol, relative_error_tol, max_iterations)
 SAMPLE_DOUBLES, LIN_DOUBLES, STATE_DOUBLES = 7, 13, 16
 FLAG_IMU_AVG, FLAG_ANALYTIC_JACOBIANS = 1, 2
 # record field slices (include/cpi_b200.h)

@@ -479,6 +479,102 @@ int cpi_imu_chains_assemble(int64_t n_chains, const int64_t* chain_offsets, int6
     return CPI_OK;
 }
 
+int cpi_imu_factor_cost_batch(int model, int64_t n_factors, const double* states, const int64_t* idx_i, const int64_t* idx_j,
+                              const double* records, const double* lin, double* f, void* stream) {
+    if (model != 1 && model != 2) return fail(CPI_EINVAL, "model must be 1 or 2 (got %d)", model);
+    if (n_factors < 0) return fail(CPI_EINVAL, "negative count");
+    if (n_factors == 0) return CPI_OK;
+    if (n_factors >= ((int64_t)1 << 33)) return fail(CPI_EINVAL, "too many factors (%lld)", (long long)n_factors);
+    if (!states || !records || !lin || !f) return fail(CPI_EINVAL, "null pointer argument");
+    if ((idx_i == nullptr) != (idx_j == nullptr)) return fail(CPI_EINVAL, "idx_i and idx_j must both be given or both be null");
+    DevInfo d;
+    int rc = device_info(d);
+    if (rc) return rc;
+    CU(cpi::factor_cost_launch(model, n_factors, states, idx_i, idx_j, records, lin, f, (cudaStream_t)stream));
+    g_launches += 1;
+    return CPI_OK;
+}
+
+int cpi_imu_chains_assemble_lm(int64_t n_chains, const int64_t* chain_offsets, int64_t chain_uniform, const double* G11, const double* G12,
+                               const double* G22, const double* g1, const double* g2, const double* lambda, int diagonal_damping,
+                               const double* prior_info, const double* prior_rhs, double* D, double* E, double* rhs, double* damp, void* stream) {
+    int rc = chain_layout_check(n_chains, chain_offsets, chain_uniform);
+    if (rc || n_chains == 0) return rc;
+    const bool any_factor = chain_offsets || chain_uniform > 1;
+    if (!lambda) return fail(CPI_EINVAL, "null pointer argument (lambda: one per chain)");
+    if (!D || !rhs) return fail(CPI_EINVAL, "null pointer argument (D / rhs)");
+    if (any_factor && (!G11 || !G12 || !G22 || !g1 || !g2)) return fail(CPI_EINVAL, "null pointer argument (G11 / G12 / G22 / g1 / g2)");
+    if ((chain_offsets || n_chains * chain_uniform > 1) && !E) return fail(CPI_EINVAL, "null pointer argument (E)");
+    DevInfo d;
+    if ((rc = device_info(d))) return rc;
+    CU(cpi::chains_assemble_lm_launch(n_chains, chain_offsets, chain_uniform, G11, G12, G22, g1, g2, lambda, diagonal_damping != 0, prior_info,
+                                      prior_rhs, D, E, rhs, damp, d.sms, (cudaStream_t)stream));
+    g_launches += 1;
+    return CPI_OK;
+}
+
+int64_t cpi_imu_chains_solve_workspace(int64_t n_chains, int64_t n_states) {
+    if (n_chains < 0 || n_states < 0 || n_states < n_chains) return (int64_t)CPI_EINVAL;
+    return cpi::chains_solve_workspace_bytes(n_states);
+}
+
+int cpi_imu_chains_solve(int64_t n_chains, const int64_t* chain_offsets, int64_t chain_uniform, int64_t n_states, const double* D, const double* E,
+                         const double* rhs, double* x, void* workspace, void* stream) {
+    int rc = chain_layout_check(n_chains, chain_offsets, chain_uniform);
+    if (rc) return rc;
+    if (n_states < n_chains) return fail(CPI_EINVAL, "n_states (%lld) below n_chains (%lld): every chain holds a state", (long long)n_states,
+                                         (long long)n_chains);
+    if (!chain_offsets && n_states != n_chains * chain_uniform)
+        return fail(CPI_EINVAL, "n_states (%lld) must be n_chains x chain_uniform (%lld)", (long long)n_states, (long long)(n_chains * chain_uniform));
+    if (n_chains == 0) return CPI_OK;
+    if (!D || !rhs || !x || !workspace || (n_states > 1 && !E)) return fail(CPI_EINVAL, "null pointer argument");
+    DevInfo d;
+    if ((rc = device_info(d))) return rc;
+    int launches = 0;
+    CU(cpi::chains_solve_launch(n_chains, chain_offsets, chain_uniform, n_states, D, E, rhs, x, (double*)workspace, d.sms, (cudaStream_t)stream,
+                                &launches));
+    g_launches += launches;
+    return CPI_OK;
+}
+
+int64_t cpi_imu_chains_lm_workspace(int64_t n_states) { return n_states < 0 ? (int64_t)CPI_EINVAL : cpi::lm_workspace_bytes(n_states); }
+
+int cpi_imu_chains_lm_update(int64_t n_chains, const int64_t* chain_offsets, int64_t chain_uniform, int64_t n_states, const cpi_lm_params* params,
+                             const double* f_cur, const double* prior_f_cur, const double* f_new, const double* prior_f_new, const double* rhs,
+                             const double* D, const double* E, const double* damp, const double* delta, const double* states_new, double* states,
+                             double* lambda, double* cost, int32_t* status, int32_t* iterations, int32_t* tries, int32_t* any_running,
+                             void* workspace, void* stream) {
+    int rc = chain_layout_check(n_chains, chain_offsets, chain_uniform);
+    if (rc) return rc;
+    if (n_states < n_chains) return fail(CPI_EINVAL, "n_states (%lld) below n_chains (%lld): every chain holds a state", (long long)n_states,
+                                         (long long)n_chains);
+    if (!chain_offsets && n_states != n_chains * chain_uniform)
+        return fail(CPI_EINVAL, "n_states (%lld) must be n_chains x chain_uniform (%lld)", (long long)n_states, (long long)(n_chains * chain_uniform));
+    if (!params) return fail(CPI_EINVAL, "null pointer argument (params)");
+    const cpi_lm_params& p = *params;
+    if (!(p.lambda_factor > 1.0)) return fail(CPI_EINVAL, "lambda_factor must be > 1 (got %g)", p.lambda_factor);
+    if (!(p.lambda_lower >= 0.0)) return fail(CPI_EINVAL, "lambda_lower must be >= 0 (got %g)", p.lambda_lower);
+    if (!(p.lambda_upper >= p.lambda_lower)) return fail(CPI_EINVAL, "lambda_upper (%g) must be >= lambda_lower (%g)", p.lambda_upper, p.lambda_lower);
+    if (!(p.min_model_fidelity >= 0.0 && p.min_model_fidelity < 1.0))
+        return fail(CPI_EINVAL, "min_model_fidelity must be in [0, 1) (got %g)", p.min_model_fidelity);
+    if (!(p.absolute_error_tol >= 0.0)) return fail(CPI_EINVAL, "absolute_error_tol must be >= 0 (got %g)", p.absolute_error_tol);
+    if (!(p.relative_error_tol >= 0.0)) return fail(CPI_EINVAL, "relative_error_tol must be >= 0 (got %g)", p.relative_error_tol);
+    if (p.max_iterations < 1 || p.max_iterations > 2147483647)
+        return fail(CPI_EINVAL, "max_iterations must be in [1, 2^31) (got %lld)", (long long)p.max_iterations);
+    if (n_chains == 0) return CPI_OK;
+    if (n_states > n_chains && (!f_cur || !f_new || !E)) return fail(CPI_EINVAL, "null pointer argument (f_cur / f_new / E)");
+    if (!rhs || !D || !damp || !delta || !states_new || !states || !workspace)
+        return fail(CPI_EINVAL, "null pointer argument (rhs / D / damp / delta / states_new / states / workspace)");
+    if (!lambda || !cost || !status || !iterations || !tries) return fail(CPI_EINVAL, "null pointer argument (lambda / cost / status / iterations / tries)");
+    if ((prior_f_cur == nullptr) != (prior_f_new == nullptr)) return fail(CPI_EINVAL, "prior_f_cur and prior_f_new must both be given or both be null");
+    DevInfo d;
+    if ((rc = device_info(d))) return rc;
+    CU(cpi::lm_update_launch(n_chains, chain_offsets, chain_uniform, n_states, p, f_cur, prior_f_cur, f_new, prior_f_new, rhs, D, E, damp, delta,
+                             states_new, states, lambda, cost, status, iterations, tries, any_running, (double*)workspace, (cudaStream_t)stream));
+    g_launches += 2;
+    return CPI_OK;
+}
+
 int cpi_imu_chain_marginalize(int64_t n_chains, const int64_t* chain_offsets, int64_t chain_uniform, const int64_t* n_marg, int64_t n_marg_uniform,
                               const double* G11, const double* G12, const double* G22, const double* g1, const double* g2, const double* f,
                               const double* prior_info, const double* prior_rhs, const double* prior_f,

@@ -3,6 +3,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "../../include/cpi_b200.h"
+
 namespace cpi {
 
 struct PropagateParams {
@@ -59,7 +61,16 @@ cudaError_t chains_assemble_launch(int64_t n_chains, const int64_t* offs, int64_
                                    const double* g1, const double* g2, double lambda, int diagonal_damping, const double* prior_info,
                                    const double* prior_rhs, double* D, double* E, double* rhs, int sms, cudaStream_t st);
 int64_t chain_solve_workspace_bytes(int64_t n_states);
-cudaError_t chain_solve_launch(int64_t n_states, const double* D, const double* E, const double* b, double* x, double* ws, cudaStream_t st, int* launches);
+// cid (device int64[n_states], may be NULL): every state's chain; given, couplings between chains are never loaded (the isolated solve)
+cudaError_t chain_solve_launch(int64_t n_states, const double* D, const double* E, const double* b, double* x, double* ws, cudaStream_t st, int* launches,
+                               const int64_t* cid = nullptr);
+// the per-chain-lambda assembly and the isolated solve of many chains (cpi_imu_chains_assemble_lm / cpi_imu_chains_solve)
+cudaError_t chains_assemble_lm_launch(int64_t n_chains, const int64_t* offs, int64_t uniform, const double* G11, const double* G12, const double* G22,
+                                      const double* g1, const double* g2, const double* lams, int diagonal_damping, const double* prior_info,
+                                      const double* prior_rhs, double* D, double* E, double* rhs, double* damp, int sms, cudaStream_t st);
+int64_t chains_solve_workspace_bytes(int64_t n_states);
+cudaError_t chains_solve_launch(int64_t n_chains, const int64_t* offs, int64_t uniform, int64_t n_states, const double* D, const double* E, const double* b,
+                                double* x, double* ws, int sms, cudaStream_t st, int* launches);
 // merge.cu: one merged model-1 record per group (dtype 64 or 32)
 cudaError_t merge_launch(int dtype, int64_t n_groups, const int64_t* offsets, int64_t uniform, const void* records, const void* lin,
                          void* out, cudaStream_t st);
@@ -76,6 +87,14 @@ cudaError_t marginalize_launch(int64_t n_chains, const int64_t* offs, int64_t un
                                double* out_f, cudaStream_t st);
 cudaError_t prior_at_launch(int64_t n, const double* info, const double* rhs, const double* f, const double* lin, const double* x,
                             double* rhs_out, double* f_out, cudaStream_t st);
+// lm.cu: the factor cost (K9) and the per-chain Levenberg-Marquardt decision
+cudaError_t factor_cost_launch(int model, int64_t n, const double* states, const int64_t* idx_i, const int64_t* idx_j, const double* records,
+                               const double* lin, double* f, cudaStream_t st);
+int64_t lm_workspace_bytes(int64_t n_states);
+cudaError_t lm_update_launch(int64_t n_chains, const int64_t* offs, int64_t uniform, int64_t n_states, const cpi_lm_params& p, const double* f_cur,
+                             const double* pf_cur, const double* f_new, const double* pf_new, const double* rhs, const double* D, const double* E,
+                             const double* damp, const double* delta, const double* states_new, double* states, double* lam, double* cost,
+                             int32_t* status, int32_t* iterations, int32_t* tries, int32_t* any_running, double* ws, cudaStream_t st);
 cudaError_t retract_launch(int64_t n, const double* states, const double* xi, double* out, cudaStream_t st);
 
 }  // namespace cpi

@@ -72,9 +72,12 @@ __global__ void __launch_bounds__(128) k_factor_whiten(int64_t n, int rd, const 
 //   E[k] = G12[k-c] (block (k, k+1)), exactly 0 where k is the last state of its chain,   rhs[k] = g2[k-1-c] + g1[k-c] (+ prior_rhs[c])
 // Damping as in GTSAM's LevenbergMarquardtParams: lambda I, or with diagonalDamping lambda * clamp(diag, minDiagonal 1e-6, maxDiagonal 1e32).
 // Grid-stride over the states: the state count o[n_chains] of a device-resident layout is read here, not on the host.
-__global__ void k_chain_assemble(int64_t n_chains, const int64_t* offs, int64_t uniform, const double* G11, const double* G12, const double* G22,
-                                 const double* g1, const double* g2, double lambda, int diagonal_damping, const double* prior_info,
-                                 const double* prior_rhs, double* D, double* E, double* rhs) {
+// PER_CHAIN: lambda is lams[c] per chain, and damp (may be NULL) receives the diagonal the damping added, [N, 15]
+// (cpi_imu_chains_assemble_lm, lm.cu); otherwise the scalar lambda.
+template <bool PER_CHAIN>
+CPI_DEV void chain_assemble_body(int64_t n_chains, const int64_t* offs, int64_t uniform, const double* G11, const double* G12, const double* G22,
+                                 const double* g1, const double* g2, double lambda, const double* lams, int diagonal_damping,
+                                 const double* prior_info, const double* prior_rhs, double* D, double* E, double* rhs, double* damp) {
     const int64_t ns = offs ? offs[n_chains] : n_chains * uniform;
     for (int64_t k = blockIdx.x; k < ns; k += gridDim.x) {
         int64_t c, lo, hi;
@@ -87,13 +90,18 @@ __global__ void k_chain_assemble(int64_t n_chains, const int64_t* offs, int64_t 
         }
         const bool first = k == lo, last = k == hi - 1;
         const int64_t fr = k - c;                                  // the factor to the right of state k (if k is not last)
+        const double lam = PER_CHAIN ? lams[c] : lambda;
         for (int t = threadIdx.x; t < 225; t += blockDim.x) {
             double d = 0.0;
             if (!first) d += G22[(fr - 1) * 225 + t];
             if (!last) d += G11[fr * 225 + t];
             if (k + 1 < ns) E[k * 225 + t] = last ? 0.0 : G12[fr * 225 + t];
             if (first && prior_info) d += prior_info[c * 225 + t];
-            if (t % 16 == 0) d += diagonal_damping ? lambda * fmin(fmax(d, 1e-6), 1e32) : lambda;     // t = r + 15 c: diagonal when r == c  <=>  t % 16 == 0
+            if (t % 16 == 0) {                                     // t = r + 15 c: diagonal when r == c  <=>  t % 16 == 0
+                const double a = diagonal_damping ? lam * fmin(fmax(d, 1e-6), 1e32) : lam;
+                if (PER_CHAIN && damp) damp[k * 15 + t / 16] = a;
+                d += a;
+            }
             D[k * 225 + t] = d;
         }
         for (int t = threadIdx.x; t < 15; t += blockDim.x) {
@@ -106,10 +114,31 @@ __global__ void k_chain_assemble(int64_t n_chains, const int64_t* offs, int64_t 
     }
 }
 
+__global__ void k_chain_assemble(int64_t n_chains, const int64_t* offs, int64_t uniform, const double* G11, const double* G12, const double* G22,
+                                 const double* g1, const double* g2, double lambda, int diagonal_damping, const double* prior_info,
+                                 const double* prior_rhs, double* D, double* E, double* rhs) {
+    chain_assemble_body<false>(n_chains, offs, uniform, G11, G12, G22, g1, g2, lambda, nullptr, diagonal_damping, prior_info, prior_rhs, D, E, rhs,
+                               nullptr);
+}
+
+__global__ void k_chain_assemble_lm(int64_t n_chains, const int64_t* offs, int64_t uniform, const double* G11, const double* G12, const double* G22,
+                                    const double* g1, const double* g2, const double* lams, int diagonal_damping, const double* prior_info,
+                                    const double* prior_rhs, double* D, double* E, double* rhs, double* damp) {
+    chain_assemble_body<true>(n_chains, offs, uniform, G11, G12, G22, g1, g2, 0.0, lams, diagonal_damping, prior_info, prior_rhs, D, E, rhs, damp);
+}
+
 // ---- block cyclic reduction ---------------------------------------------------------------------------------------------------------
 // Level with m nodes: row i reads  E[i-1]^T x_{i-1} + D[i] x_i + E[i] x_{i+1} = b[i].
+// ISO (cpi_imu_chains_solve): node i of the level sits at original state i * stride, cid[] holds each original state's chain, and a
+// coupling between nodes of different chains is structurally absent: not loaded, not multiplied, written as exact 0.  With finite
+// input those couplings are exact zeros anyway, so the ISO kernels give the plain kernels' bits; a NaN stays inside its chain.
+#define CPI_SAME(p, q) (!ISO || cid[(p) * stride] == cid[(q) * stride])
+#define SAME(p, q) (cid[(p) * stride] == cid[(q) * stride])
+
 // Odd node i = 2t+1:  D_i = Lc Lc^T,  Za = Lc^-1 E[i-1]^T,  Zb = Lc^-1 E[i] (if i+1 < m),  zb = Lc^-1 b_i      (kept for the back-substitution)
-__global__ void __launch_bounds__(128) k_bcr_eliminate(int64_t m, const double* D, const double* E, const double* b, double* Lc, double* Za, double* Zb, double* zb) {
+template <bool ISO>
+CPI_DEV void bcr_eliminate(int64_t m, int64_t stride, const int64_t* cid, const double* D, const double* E, const double* b, double* Lc, double* Za,
+                           double* Zb, double* zb) {
     __shared__ double sL[4][15 * 16];
     const int wib = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int64_t t = (int64_t)blockIdx.x * 4 + wib;
@@ -120,12 +149,13 @@ __global__ void __launch_bounds__(128) k_bcr_eliminate(int64_t m, const double* 
     __syncwarp();
     warp_chol15(L, lane);
     for (int k = lane; k < 225; k += 32) { const int r = k % 15, c = k / 15; Lc[t * 225 + k] = (r >= c) ? L[r * 16 + c] : 0.0; }
-    const bool has_right = i + 1 < m;
+    const bool has_left = CPI_SAME(i - 1, i);
+    const bool has_right = i + 1 < m && CPI_SAME(i + 1, i);
     if (lane < 31) {
         double y[15];
         if (lane < 15) {
 #pragma unroll
-            for (int r = 0; r < 15; r++) y[r] = E[(i - 1) * 225 + lane + 15 * r];          // column `lane` of E[i-1]^T = row `lane` of E[i-1]
+            for (int r = 0; r < 15; r++) y[r] = has_left ? E[(i - 1) * 225 + lane + 15 * r] : 0.0;      // column `lane` of E[i-1]^T = row `lane` of E[i-1]
         } else if (lane < 30) {
 #pragma unroll
             for (int r = 0; r < 15; r++) y[r] = has_right ? E[i * 225 + r + 15 * (lane - 15)] : 0.0;
@@ -135,6 +165,10 @@ __global__ void __launch_bounds__(128) k_bcr_eliminate(int64_t m, const double* 
         }
         fwd15(L, y);
         double* dst = lane < 15 ? Za + t * 225 + 15 * lane : (lane < 30 ? Zb + t * 225 + 15 * (lane - 15) : zb + t * 15);
+        if (ISO && ((lane < 15 && !has_left) || (lane >= 15 && lane < 30 && !has_right))) {
+#pragma unroll
+            for (int r = 0; r < 15; r++) y[r] = 0.0;
+        }
 #pragma unroll
         for (int r = 0; r < 15; r++) dst[r] = y[r];
     }
@@ -142,6 +176,48 @@ __global__ void __launch_bounds__(128) k_bcr_eliminate(int64_t m, const double* 
 
 // Even node j = 2u -> node u of the next level:
 //   D' = D_j - Zb_{j-1}^T Zb_{j-1} - Za_{j+1}^T Za_{j+1},   b' = b_j - Zb_{j-1}^T zb_{j-1} - Za_{j+1}^T zb_{j+1},   E' = -Za_{j+1}^T Zb_{j+1}  (couples x_j and x_{j+2})
+CPI_DEV void bcr_reduce_iso(int64_t m, int64_t stride, const int64_t* cid, const double* D, const double* b, const double* Za, const double* Zb,
+                        const double* zb, double* Dn, double* En, double* bn) {
+    __shared__ double sZ[4][4][225 + 15];      // [warp][ZbL | ZaR | ZbR | (zbL, zbR)]
+    const int wib = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int64_t u = (int64_t)blockIdx.x * 4 + wib;
+    const int64_t j = 2 * u;
+    if (j >= m) return;
+    const bool hasL = j >= 1 && SAME(j - 1, j), hasR = j + 1 < m && SAME(j + 1, j), hasRR = j + 2 < m;
+    const bool linkRR = hasRR && SAME(j + 2, j);                   // x_j and x_{j+2} in one chain (then x_{j+1} too)
+    const int64_t tl = (j - 2) / 2, tr = j / 2;                     // odd-node slots of j-1 and j+1
+    double *ZbL = sZ[wib][0], *ZaR = sZ[wib][1], *ZbR = sZ[wib][2], *zz = sZ[wib][3];
+    for (int k = lane; k < 225; k += 32) {
+        ZbL[k] = hasL ? Zb[tl * 225 + k] : 0.0;
+        ZaR[k] = hasR ? Za[tr * 225 + k] : 0.0;
+        ZbR[k] = linkRR ? Zb[tr * 225 + k] : 0.0;
+    }
+    if (lane < 15) { zz[lane] = hasL ? zb[tl * 15 + lane] : 0.0; zz[15 + lane] = hasR ? zb[tr * 15 + lane] : 0.0; }
+    __syncwarp();
+    for (int k = lane; k < 225; k += 32) {
+        const int r = k % 15, c = k / 15;                          // column-major 15x15; Z matrices are column-major: Z[q + 15 col]
+        double d = D[j * 225 + k], en = 0.0;
+#pragma unroll
+        for (int q = 0; q < 15; q++) {
+            d = fma(-ZbL[q + 15 * r], ZbL[q + 15 * c], d);
+            d = fma(-ZaR[q + 15 * r], ZaR[q + 15 * c], d);
+            en = fma(-ZaR[q + 15 * r], ZbR[q + 15 * c], en);
+        }
+        Dn[u * 225 + k] = d;
+        if (hasRR) En[u * 225 + k] = linkRR ? en : 0.0;
+    }
+    if (lane < 15) {
+        double v = b[j * 15 + lane];
+#pragma unroll
+        for (int q = 0; q < 15; q++) { v = fma(-ZbL[q + 15 * lane], zz[q], v); v = fma(-ZaR[q + 15 * lane], zz[15 + q], v); }
+        bn[u * 15 + lane] = v;
+    }
+}
+
+__global__ void __launch_bounds__(128) k_bcr_eliminate(int64_t m, const double* D, const double* E, const double* b, double* Lc, double* Za, double* Zb, double* zb) {
+    bcr_eliminate<false>(m, 0, nullptr, D, E, b, Lc, Za, Zb, zb);
+}
+// (k_bcr_reduce keeps its own copy of the body: through bcr_reduce<false> its register allocation changes)
 __global__ void __launch_bounds__(128) k_bcr_reduce(int64_t m, const double* D, const double* b, const double* Za, const double* Zb, const double* zb,
                                                     double* Dn, double* En, double* bn) {
     __shared__ double sZ[4][4][225 + 15];      // [warp][ZbL | ZaR | ZbR | (zbL, zbR)]
@@ -178,6 +254,14 @@ __global__ void __launch_bounds__(128) k_bcr_reduce(int64_t m, const double* D, 
         bn[u * 15 + lane] = v;
     }
 }
+__global__ void __launch_bounds__(128) k_bcr_eliminate_iso(int64_t m, int64_t stride, const int64_t* cid, const double* D, const double* E, const double* b,
+                                                           double* Lc, double* Za, double* Zb, double* zb) {
+    bcr_eliminate<true>(m, stride, cid, D, E, b, Lc, Za, Zb, zb);
+}
+__global__ void __launch_bounds__(128) k_bcr_reduce_iso(int64_t m, int64_t stride, const int64_t* cid, const double* D, const double* b, const double* Za,
+                                                        const double* Zb, const double* zb, double* Dn, double* En, double* bn) {
+    bcr_reduce_iso(m, stride, cid, D, b, Za, Zb, zb, Dn, En, bn);
+}
 
 // last level (one node): x = D^-1 b
 __global__ void k_bcr_root(const double* D, const double* b, double* x, int64_t stride) {
@@ -199,7 +283,8 @@ __global__ void k_bcr_root(const double* D, const double* b, double* x, int64_t 
 }
 
 // odd node i = 2t+1 of a level whose nodes sit at original indices i * stride:  Lc^T x_i = zb - Za x_{i-1} - Zb x_{i+1}
-__global__ void __launch_bounds__(128) k_bcr_backsub(int64_t m, int64_t stride, const double* Lc, const double* Za, const double* Zb, const double* zb, double* x) {
+template <bool ISO>
+CPI_DEV void bcr_backsub(int64_t m, int64_t stride, const int64_t* cid, const double* Lc, const double* Za, const double* Zb, const double* zb, double* x) {
     __shared__ double sL[4][15 * 16];
     const int wib = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int64_t t = (int64_t)blockIdx.x * 4 + wib;
@@ -208,7 +293,8 @@ __global__ void __launch_bounds__(128) k_bcr_backsub(int64_t m, int64_t stride, 
     double* L = sL[wib];
     for (int k = lane; k < 225; k += 32) { const int r = k % 15, c = k / 15; if (r >= c) L[r * 16 + c] = Lc[t * 225 + k]; }
     __syncwarp();
-    const bool has_right = i + 1 < m;
+    const bool has_left = CPI_SAME(i - 1, i);
+    const bool has_right = i + 1 < m && CPI_SAME(i + 1, i);
     double r = 0.0;
     if (lane < 15) {
         r = zb[t * 15 + lane];
@@ -216,12 +302,37 @@ __global__ void __launch_bounds__(128) k_bcr_backsub(int64_t m, int64_t stride, 
         const double* xr = x + (i + 1) * stride * 15;
 #pragma unroll
         for (int q = 0; q < 15; q++) {
-            r = fma(-Za[t * 225 + lane + 15 * q], xl[q], r);
+            if (has_left) r = fma(-Za[t * 225 + lane + 15 * q], xl[q], r);
             if (has_right) r = fma(-Zb[t * 225 + lane + 15 * q], xr[q], r);
         }
     }
     const double xv = warp_bwd15(L, r, lane);
     if (lane < 15) x[i * stride * 15 + lane] = xv;
+}
+#undef CPI_SAME
+#undef SAME
+
+__global__ void __launch_bounds__(128) k_bcr_backsub(int64_t m, int64_t stride, const double* Lc, const double* Za, const double* Zb, const double* zb, double* x) {
+    bcr_backsub<false>(m, stride, nullptr, Lc, Za, Zb, zb, x);
+}
+__global__ void __launch_bounds__(128) k_bcr_backsub_iso(int64_t m, int64_t stride, const int64_t* cid, const double* Lc, const double* Za, const double* Zb,
+                                                         const double* zb, double* x) {
+    bcr_backsub<true>(m, stride, cid, Lc, Za, Zb, zb, x);
+}
+
+// the chain of every state, for the ISO kernels (grid-stride; a device-resident layout is searched per state)
+__global__ void k_chain_ids(int64_t n_chains, const int64_t* offs, int64_t uniform, int64_t n_states, int64_t* cid) {
+    for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < n_states; k += (int64_t)gridDim.x * blockDim.x) {
+        int64_t c;
+        if (offs) {
+            int64_t a = 0, b = n_chains - 1;
+            while (a < b) { const int64_t mid = (a + b + 1) >> 1; if (offs[mid] <= k) a = mid; else b = mid - 1; }
+            c = a;
+        } else {
+            c = k / uniform;
+        }
+        cid[k] = c;
+    }
 }
 
 // ---- launchers ----------------------------------------------------------------------------------------------------------------------
@@ -241,6 +352,15 @@ cudaError_t chains_assemble_launch(int64_t n_chains, const int64_t* offs, int64_
     return cudaGetLastError();
 }
 
+cudaError_t chains_assemble_lm_launch(int64_t n_chains, const int64_t* offs, int64_t uniform, const double* G11, const double* G12, const double* G22,
+                                      const double* g1, const double* g2, const double* lams, int diagonal_damping, const double* prior_info,
+                                      const double* prior_rhs, double* D, double* E, double* rhs, double* damp, int sms, cudaStream_t st) {
+    const int64_t ns = offs ? (int64_t)sms * 16 : n_chains * uniform;
+    const int grid = (int)(ns < 2147483647 ? ns : 2147483647);
+    k_chain_assemble_lm<<<grid, 128, 0, st>>>(n_chains, offs, uniform, G11, G12, G22, g1, g2, lams, diagonal_damping, prior_info, prior_rhs, D, E, rhs, damp);
+    return cudaGetLastError();
+}
+
 // workspace layout: for every level l >= 1 the reduced system (D, E, b), for every level l >= 0 the eliminated nodes (Lc, Za, Zb, zb)
 static int64_t bcr_doubles(int64_t m) {
     int64_t tot = 0;
@@ -253,8 +373,21 @@ static int64_t bcr_doubles(int64_t m) {
     return tot + 16;
 }
 int64_t chain_solve_workspace_bytes(int64_t n_states) { return bcr_doubles(n_states) * 8; }
+// the isolated solve: the same, followed by the chain id of every state
+int64_t chains_solve_workspace_bytes(int64_t n_states) { return bcr_doubles(n_states) * 8 + n_states * 8; }
 
-cudaError_t chain_solve_launch(int64_t n_states, const double* D, const double* E, const double* b, double* x, double* ws, cudaStream_t st, int* launches) {
+cudaError_t chains_solve_launch(int64_t n_chains, const int64_t* offs, int64_t uniform, int64_t n_states, const double* D, const double* E, const double* b,
+                                double* x, double* ws, int sms, cudaStream_t st, int* launches) {
+    int64_t* cid = reinterpret_cast<int64_t*>(ws + bcr_doubles(n_states));
+    const int64_t blocks = (n_states + 255) / 256, cap = (int64_t)sms * 8;
+    k_chain_ids<<<(int)(blocks < cap ? blocks : cap), 256, 0, st>>>(n_chains, offs, uniform, n_states, cid);
+    const cudaError_t e = chain_solve_launch(n_states, D, E, b, x, ws, st, launches, cid);
+    if (launches) *launches += 1;
+    return e;
+}
+
+cudaError_t chain_solve_launch(int64_t n_states, const double* D, const double* E, const double* b, double* x, double* ws, cudaStream_t st, int* launches,
+                               const int64_t* cid) {
     struct Level { int64_t m; const double *D, *E, *b; double *Lc, *Za, *Zb, *zb; };
     Level lv[64];
     int nl = 0;
@@ -268,8 +401,14 @@ cudaError_t chain_solve_launch(int64_t n_states, const double* D, const double* 
         L.m = m; L.D = cD; L.E = cE; L.b = cb;
         L.Lc = p; p += odd * 225; L.Za = p; p += odd * 225; L.Zb = p; p += odd * 225; L.zb = p; p += odd * 15;
         double* nD = p; p += even * 225; double* nE = p; p += even * 225; double* nb = p; p += even * 15;
-        k_bcr_eliminate<<<(int)((odd + 3) / 4), 128, 0, st>>>(m, cD, cE, cb, L.Lc, L.Za, L.Zb, L.zb);
-        k_bcr_reduce<<<(int)((even + 3) / 4), 128, 0, st>>>(m, cD, cb, L.Za, L.Zb, L.zb, nD, nE, nb);
+        const int64_t stride = (int64_t)1 << (nl - 1);              // level nl - 1: node i is original state i * 2^(nl-1)
+        if (cid) {
+            k_bcr_eliminate_iso<<<(int)((odd + 3) / 4), 128, 0, st>>>(m, stride, cid, cD, cE, cb, L.Lc, L.Za, L.Zb, L.zb);
+            k_bcr_reduce_iso<<<(int)((even + 3) / 4), 128, 0, st>>>(m, stride, cid, cD, cb, L.Za, L.Zb, L.zb, nD, nE, nb);
+        } else {
+            k_bcr_eliminate<<<(int)((odd + 3) / 4), 128, 0, st>>>(m, cD, cE, cb, L.Lc, L.Za, L.Zb, L.zb);
+            k_bcr_reduce<<<(int)((even + 3) / 4), 128, 0, st>>>(m, cD, cb, L.Za, L.Zb, L.zb, nD, nE, nb);
+        }
         nk += 2;
         cD = nD; cE = nE; cb = nb; m = even;
     }
@@ -279,7 +418,8 @@ cudaError_t chain_solve_launch(int64_t n_states, const double* D, const double* 
     for (int l = nl - 1; l >= 0; l--) {
         stride >>= 1;
         const int64_t odd = lv[l].m / 2;
-        k_bcr_backsub<<<(int)((odd + 3) / 4), 128, 0, st>>>(lv[l].m, stride, lv[l].Lc, lv[l].Za, lv[l].Zb, lv[l].zb, x);
+        if (cid) k_bcr_backsub_iso<<<(int)((odd + 3) / 4), 128, 0, st>>>(lv[l].m, stride, cid, lv[l].Lc, lv[l].Za, lv[l].Zb, lv[l].zb, x);
+        else k_bcr_backsub<<<(int)((odd + 3) / 4), 128, 0, st>>>(lv[l].m, stride, lv[l].Lc, lv[l].Za, lv[l].Zb, lv[l].zb, x);
         nk++;
     }
     if (launches) *launches = nk;

@@ -348,6 +348,174 @@ def chain_lm_step(model, states, records, lin, lam=1e-5, prior_sigma=1e-4, strea
     return new_states, dx, cost[0]
 
 
+def factor_cost(model, states, records, lin, idx_i=None, idx_j=None, out=None, stream=None):
+    """Whitened cost f = e^T P_meas^-1 e of every factor at the states (cpi_imu_factor_cost_batch, kernel K9): factor_hessian's f
+    without evaluating or writing e and the blocks; NaN where P_meas is not positive definite.  Indexing as factor_eval.
+    Device tensors; returns f [n]."""
+    import torch
+
+    n = records.numel() // REC_DOUBLES[model]
+    dev = records.device
+    for name, t in (("states", states), ("lin", lin), ("idx_i", idx_i), ("idx_j", idx_j)):
+        if t is not None and (not t.is_cuda or t.device != dev):
+            raise ValueError(f"{name} must be a CUDA tensor on {dev}")
+    if (idx_i is None) != (idx_j is None):
+        raise ValueError("idx_i and idx_j must both be given or both be None")
+    if idx_i is not None:
+        if idx_i.dtype != torch.int64 or idx_j.dtype != torch.int64 or idx_i.numel() != n or idx_j.numel() != n:
+            raise ValueError("idx_i / idx_j must be int64 tensors with one entry per factor")
+        idx_i = idx_i.contiguous(); idx_j = idx_j.contiguous()
+    f = torch.empty((n,), dtype=torch.float64, device=dev) if out is None else out
+    with torch.cuda.device(dev):
+        st = stream if stream is not None else torch.cuda.current_stream(dev)
+        capi.check(capi.load().cpi_imu_factor_cost_batch(model, n, _tptr(states.contiguous()), _tptr(idx_i), _tptr(idx_j), _tptr(records.contiguous()),
+                                                         _tptr(lin.contiguous()), _tptr(f), ctypes.c_void_p(st.cuda_stream)))
+    return f
+
+
+def chains_assemble_lm(G11, G12, G22, g1, g2, chain_offsets, lam, prior_info=None, prior_rhs=None, diagonal_damping=True, n_chains=None,
+                       stream=None):
+    """chains_assemble with one lambda per chain (cpi_imu_chains_assemble_lm): lam is a device float64 [n_chains].
+    Returns (D [N,225], E [N-1,225], rhs [N,15], damp [N,15]) -- damp the diagonal the damping added."""
+    import torch
+
+    dev = G11.device
+    _check_f64(dev, G11=G11, G12=G12, G22=G22, g1=g1, g2=g2, prior_info=prior_info, prior_rhs=prior_rhs, lam=lam)
+    nf = G11.numel() // 225
+    C, offs, S = _chain_layout(chain_offsets, dev, n_factors=nf, n_chains=n_chains)
+    if lam is None or lam.numel() != C:
+        raise ValueError("lam needs one float64 CUDA entry per chain")
+    if (prior_info is not None and prior_info.numel() != 225 * C) or (prior_rhs is not None and prior_rhs.numel() != 15 * C):
+        raise ValueError("prior_info needs 225 doubles and prior_rhs 15 per chain")
+    N = nf + C
+    D = torch.empty((N, 225), dtype=torch.float64, device=dev)
+    E = torch.empty((max(N - 1, 1), 225), dtype=torch.float64, device=dev)
+    rhs = torch.empty((N, 15), dtype=torch.float64, device=dev)
+    damp = torch.empty((N, 15), dtype=torch.float64, device=dev)
+    with torch.cuda.device(dev):
+        st = stream if stream is not None else torch.cuda.current_stream(dev)
+        capi.check(capi.load().cpi_imu_chains_assemble_lm(C, _tptr(offs), S, _tptr(G11.contiguous()), _tptr(G12.contiguous()), _tptr(G22.contiguous()),
+                                                          _tptr(g1.contiguous()), _tptr(g2.contiguous()), _tptr(lam.contiguous()),
+                                                          int(bool(diagonal_damping)),
+                                                          _tptr(None if prior_info is None else prior_info.contiguous()),
+                                                          _tptr(None if prior_rhs is None else prior_rhs.contiguous()), _tptr(D), _tptr(E), _tptr(rhs),
+                                                          _tptr(damp), ctypes.c_void_p(st.cuda_stream)))
+    return D, E[:N - 1], rhs, damp
+
+
+def chains_solve(D, E, rhs, chain_offsets, n_chains=None, workspace=None, stream=None):
+    """chain_solve with every coupling between two chains structurally absent (cpi_imu_chains_solve): a chain that is not SPD gets NaN
+    and leaves every other chain as it is; on SPD input bitwise chain_solve.  chain_offsets as chains_assemble."""
+    import torch
+
+    dev = D.device
+    N = D.numel() // 225
+    C, offs, S = _chain_layout(chain_offsets, dev, n_states=N, n_chains=n_chains)
+    lib = capi.load()
+    x = torch.empty((N, 15), dtype=torch.float64, device=dev)
+    nbytes = int(lib.cpi_imu_chains_solve_workspace(C, N))
+    if workspace is None or workspace.numel() * 8 < nbytes:
+        workspace = torch.empty((nbytes + 7) // 8, dtype=torch.float64, device=dev)
+    with torch.cuda.device(dev):
+        st = stream if stream is not None else torch.cuda.current_stream(dev)
+        capi.check(lib.cpi_imu_chains_solve(C, _tptr(offs), S, N, _tptr(D.contiguous()), _tptr(E.contiguous()), _tptr(rhs.contiguous()), _tptr(x),
+                                            _tptr(workspace), ctypes.c_void_p(st.cuda_stream)))
+    return x
+
+
+def chains_lm(model, states, records, lin, chain_offsets, prior=None, lam=1e-5, diagonal_damping=True, params=None, max_rounds=200, check_every=8,
+              stream=None):
+    """Levenberg-Marquardt of many independent IMU-only chains at once, to convergence, on the device (GTSAM's
+    LevenbergMarquardtOptimizer rule per chain: include/cpi_b200.h, DESIGN.md section 3f).  Arguments as chains_lm_step; lam: the
+    initial lambda of every chain; params: capi.LMParams (None: GTSAM's defaults).  A prior without a linearisation point is taken as
+    linearised at the initial first states.  Per round: eval -> information blocks -> prior_at -> chains_assemble_lm (lambda per chain)
+    -> chains_solve (chains isolated) -> retract -> factor_cost + prior_at at the candidate -> cpi_imu_chains_lm_update.  No host
+    synchronisation inside the loop except one 4-byte "any chain running" read every check_every rounds (0: max_rounds rounds, fully
+    asynchronous).  Returns (states [N,16], cost [C] at them, lam [C], status [C] int32 (capi.LM_*), iterations [C] (accepted steps),
+    tries [C] (rounds the chain ran)), all int32 counters."""
+    import torch
+
+    lib = capi.load()
+    dev = states.device
+    _check_f64(dev, states=states, records=records, lin=lin)
+    N = states.numel() // 16
+    C, offs, S = _chain_layout(chain_offsets, dev, n_states=N)
+    nf = N - C
+    if records.numel() != REC_DOUBLES[model] * nf or lin.numel() != 13 * nf:
+        raise ValueError(f"{C} chains over {N} states hold {nf} factors: one record and one linearisation point each")
+    params = capi.LMParams() if params is None else params
+    if max_rounds < 0 or check_every < 0:
+        raise ValueError("max_rounds and check_every must be >= 0")
+    f64 = dict(dtype=torch.float64, device=dev)
+    i32 = dict(dtype=torch.int32, device=dev)
+    X = states.reshape(N, 16).clone()
+    records, lin = records.contiguous(), lin.contiguous()
+    idx_i = idx_j = None
+    if C > 1:                                                        # as chains_lm_step
+        ar = torch.arange(nf, dtype=torch.int64, device=dev)
+        if offs is not None:
+            chain_of = torch.repeat_interleave(torch.arange(C, dtype=torch.int64, device=dev), offs[1:] - offs[:-1] - 1, output_size=nf)
+        else:
+            chain_of = ar // (S - 1) if S > 1 else ar
+        idx_i = ar + chain_of
+        idx_j = idx_i + 1
+    first = offs[:-1] if offs is not None else torch.arange(C, dtype=torch.int64, device=dev) * S
+    pi = pr = pf = lin0 = None
+    if prior is not None:
+        pi, pr, pf, lin0 = prior
+        _check_f64(dev, prior_info=pi, prior_rhs=pr, prior_f=pf, prior_lin=lin0)
+        pi = pi.contiguous()
+        pr = torch.zeros((C, 15), **f64) if pr is None else pr.contiguous()
+        pf = torch.zeros(C, **f64) if pf is None else pf.contiguous()
+        lin0 = X.index_select(0, first) if lin0 is None else lin0.contiguous()
+    lam_t = torch.full((C,), float(lam), **f64)
+    cost = torch.zeros(C, **f64)
+    status, iters, tries = torch.zeros(C, **i32), torch.zeros(C, **i32), torch.zeros(C, **i32)
+    flag = torch.zeros(1, **i32)
+    # round buffers, allocated once
+    e, H1, H2 = torch.empty((nf, 15), **f64), torch.empty((nf, 225), **f64), torch.empty((nf, 225), **f64)
+    G11, G12, G22 = (torch.empty((nf, 225), **f64) for _ in range(3))
+    g1, g2, f_cur, f_new = torch.empty((nf, 15), **f64), torch.empty((nf, 15), **f64), torch.empty(nf, **f64), torch.empty(nf, **f64)
+    D, E, rhs, damp = torch.empty((N, 225), **f64), torch.empty((max(N - 1, 1), 225), **f64), torch.empty((N, 15), **f64), torch.empty((N, 15), **f64)
+    dx, Xn, x0 = torch.empty((N, 15), **f64), torch.empty((N, 16), **f64), torch.empty((C, 16), **f64)
+    pr_c, pf_c, pr_n, pf_n = torch.empty((C, 15), **f64), torch.empty(C, **f64), torch.empty((C, 15), **f64), torch.empty(C, **f64)
+    ws_solve = torch.empty((int(lib.cpi_imu_chains_solve_workspace(C, N)) + 7) // 8, **f64)
+    ws_lm = torch.empty((int(lib.cpi_imu_chains_lm_workspace(N)) + 7) // 8, **f64)
+    p = _tptr
+    rd = REC_DOUBLES[model]
+    with torch.cuda.device(dev):
+        st = stream if stream is not None else torch.cuda.current_stream(dev)
+        sp = ctypes.c_void_p(st.cuda_stream)
+        with torch.cuda.stream(st):
+            for r in range(max_rounds):
+                check = check_every > 0 and (r + 1) % check_every == 0
+                if nf:
+                    capi.check(lib.cpi_imu_factor_eval_batch(model, nf, p(X), p(idx_i), p(idx_j), p(records), p(lin), p(e), p(H1), p(H2), sp))
+                    capi.check(lib.cpi_imu_factor_hessian_batch(model, nf, p(records), p(e), p(H1), p(H2), p(G11), p(G12), p(G22), p(g1), p(g2),
+                                                                p(f_cur), sp))
+                if prior is not None:
+                    torch.index_select(X, 0, first, out=x0)
+                    capi.check(lib.cpi_imu_prior_at(C, p(pi), p(pr), p(pf), p(lin0), p(x0), p(pr_c), p(pf_c), sp))
+                capi.check(lib.cpi_imu_chains_assemble_lm(C, p(offs), S, p(G11), p(G12), p(G22), p(g1), p(g2), p(lam_t), int(bool(diagonal_damping)),
+                                                          p(pi), p(pr_c if prior is not None else None), p(D), p(E), p(rhs), p(damp), sp))
+                capi.check(lib.cpi_imu_chains_solve(C, p(offs), S, N, p(D), p(E), p(rhs), p(dx), p(ws_solve), sp))
+                capi.check(lib.cpi_retract_batch(N, p(X), p(dx), p(Xn), sp))
+                if nf:
+                    capi.check(lib.cpi_imu_factor_cost_batch(model, nf, p(Xn), p(idx_i), p(idx_j), p(records), p(lin), p(f_new), sp))
+                if prior is not None:
+                    torch.index_select(Xn, 0, first, out=x0)
+                    capi.check(lib.cpi_imu_prior_at(C, p(pi), p(pr), p(pf), p(lin0), p(x0), p(pr_n), p(pf_n), sp))
+                if check:
+                    flag.zero_()
+                capi.check(lib.cpi_imu_chains_lm_update(C, p(offs), S, N, ctypes.byref(params), p(f_cur), p(pf_c if prior is not None else None),
+                                                        p(f_new), p(pf_n if prior is not None else None), p(rhs), p(D), p(E), p(damp), p(dx), p(Xn),
+                                                        p(X), p(lam_t), p(cost), p(status), p(iters), p(tries), p(flag if check else None),
+                                                        p(ws_lm), sp))
+                if check and int(flag.item()) == 0:
+                    break
+    return X, cost, lam_t, status, iters, tries
+
+
 def predict_state(model, states_k, records, lin, stream=None):
     """getpredictedstate_v1/_v2 (solvers/GraphSolver_IMU.cpp:263-307), batched.  Device tensors, or numpy (staged via torch)."""
     import torch

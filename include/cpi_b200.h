@@ -313,6 +313,71 @@ int cpi_imu_chains_assemble(int64_t n_chains, const int64_t* chain_offsets, int6
                             double lambda, int diagonal_damping, const double* prior_info, const double* prior_rhs,
                             double* D, double* E, double* rhs, void* stream);
 
+/*
+ * Levenberg-Marquardt over many chains (DESIGN.md section 3f): the optimiser of BatchFixedLagSmoother (GraphSolver.cpp:202-203), run
+ * for every chain at once with its own lambda and stopping state.  Chain layout and priors as above; fp64, DEVICE pointers,
+ * asynchronous on `stream`, no allocation.  PARITY UNPINNED (GTSAM is not in the reference tree); the numpy statement of
+ * tests/test_chains_lm.py is the reference.  Costs follow factor.chains_lm_step: cost = sum_k f_k + f'_prior, twice GTSAM's error.
+ *
+ * The rule (GTSAM's LevenbergMarquardtOptimizer with its defaults, useFixedLambdaFactor): one round, for every chain still RUNNING:
+ *   linearise at x_c (cost_cur = sum f + the prior's f' moved to x_c); assemble with lambda_c; solve; retract to the candidate x~_c;
+ *   cost_new at x~_c (cpi_imu_factor_cost_batch + cpi_imu_prior_at); model decrease m_c = sum_k delta_k^T (2 rhs_k - (H delta)_k) of the
+ *   UNDAMPED system.  Then
+ *     cost_cur or m_c not finite                        -> NONFINITE (the chain keeps its last accepted states)
+ *     delta = 0 exactly                                 -> CONVERGED
+ *     cost_new finite, m_c > 0, rho = (cost_cur - cost_new) / m_c > min_model_fidelity
+ *                                                       -> accept: x_c = x~_c, lambda_c = max(lambda_c / lambda_factor, lambda_lower),
+ *                                                          iterations += 1; CONVERGED if (cost_cur - cost_new) / 2 <= absolute_error_tol
+ *                                                          or cost_cur - cost_new <= relative_error_tol * cost_cur, else MAX_ITERATIONS
+ *                                                          once iterations = max_iterations
+ *     otherwise                                         -> reject: LAMBDA_EXHAUSTED if lambda_c >= lambda_upper, else lambda_c *= lambda_factor
+ *   and tries += 1 in every case.  A chain that is not RUNNING is never touched again (states, lambda, cost bitwise frozen).
+ *
+ *   cpi_imu_factor_cost_batch    (K9) f = e^T P_meas^-1 e of n factors at the states (indexing as cpi_imu_factor_eval_batch): the
+ *       residual of evaluateError and one Cholesky + forward substitution, no e / H written; bitwise cpi_imu_factor_hessian_batch's f.
+ *       A factor whose P_meas is not positive definite gets NaN.
+ *   cpi_imu_chains_assemble_lm   cpi_imu_chains_assemble with lambda[n_chains] (device) per chain; damp (device double[n_states*15],
+ *       may be NULL) receives the diagonal the damping added.
+ *   cpi_imu_chains_solve         the block cyclic reduction of cpi_imu_chain_solve over n_states = the layout's state count, with every
+ *       coupling between two chains structurally absent (not loaded, not multiplied, written as exact 0): a NaN stays in its chain, and
+ *       on SPD input the result is cpi_imu_chain_solve's bit for bit.  workspace: cpi_imu_chains_solve_workspace(n_chains, n_states) bytes.
+ *   cpi_imu_chains_lm_update     the decision above for every RUNNING chain: f_cur / f_new per factor, prior_f_cur / prior_f_new per chain
+ *       (NULL: no prior), rhs / D / E / damp / delta of the round, states_new the candidate states; writes lambda, cost, status,
+ *       iterations, tries, copies states_new into `states` for the accepted chains, and sets *any_running = 1 (may be NULL; the caller
+ *       zeroes it) if a chain is still RUNNING.  Per-chain sums in a fixed order (no atomics).  workspace: cpi_imu_chains_lm_workspace
+ *       (n_states) bytes.  Parameters are checked on the host: lambda_factor > 1, 0 <= lambda_lower <= lambda_upper, tolerances >= 0,
+ *       0 <= min_model_fidelity < 1, max_iterations >= 1; CPI_EINVAL otherwise, before the device is touched.
+ */
+#define CPI_LM_RUNNING           0
+#define CPI_LM_CONVERGED         1
+#define CPI_LM_MAX_ITERATIONS    2
+#define CPI_LM_LAMBDA_EXHAUSTED  3
+#define CPI_LM_NONFINITE         4
+typedef struct cpi_lm_params {
+    double lambda_factor;        /* 10    */
+    double lambda_lower;         /* 0     */
+    double lambda_upper;         /* 1e5   */
+    double min_model_fidelity;   /* 1e-3  */
+    double absolute_error_tol;   /* 1e-5  (on GTSAM's error, half the cost) */
+    double relative_error_tol;   /* 1e-5  */
+    int64_t max_iterations;      /* 100   */
+} cpi_lm_params;
+int cpi_imu_factor_cost_batch(int model, int64_t n_factors, const double* states, const int64_t* idx_i, const int64_t* idx_j,
+                              const double* records, const double* lin, double* f, void* stream);
+int cpi_imu_chains_assemble_lm(int64_t n_chains, const int64_t* chain_offsets, int64_t chain_uniform,
+                               const double* G11, const double* G12, const double* G22, const double* g1, const double* g2,
+                               const double* lambda, int diagonal_damping, const double* prior_info, const double* prior_rhs,
+                               double* D, double* E, double* rhs, double* damp, void* stream);
+int64_t cpi_imu_chains_solve_workspace(int64_t n_chains, int64_t n_states);
+int cpi_imu_chains_solve(int64_t n_chains, const int64_t* chain_offsets, int64_t chain_uniform, int64_t n_states,
+                         const double* D, const double* E, const double* rhs, double* x, void* workspace, void* stream);
+int64_t cpi_imu_chains_lm_workspace(int64_t n_states);
+int cpi_imu_chains_lm_update(int64_t n_chains, const int64_t* chain_offsets, int64_t chain_uniform, int64_t n_states,
+                             const cpi_lm_params* params, const double* f_cur, const double* prior_f_cur, const double* f_new,
+                             const double* prior_f_new, const double* rhs, const double* D, const double* E, const double* damp,
+                             const double* delta, const double* states_new, double* states, double* lambda, double* cost,
+                             int32_t* status, int32_t* iterations, int32_t* tries, int32_t* any_running, void* workspace, void* stream);
+
 /* ---- callers either side of the factor ("next" rows) ----------------------------------------------------------------- */
 
 /* x_{k+1} prediction from x_k and a record: getpredictedstate_v1/_v2 (GraphSolver_IMU.cpp:263-307).
