@@ -620,6 +620,204 @@ static void retract(const double* x_in, const double* xi_in, double* o_out) {
     store(o_out, o, CPI_STATE_DOUBLES);
 }
 
+/* ------------------------------------------------------------------ merging model-1 records (DESIGN.md 3b, 3c) ---- */
+/* Not a reference routine: a dense, literal statement of the composition of two consecutive model-1 records, with the full
+ * 15x15 Phi~ and T and dense products (as tests/test_merge.py's numpy merge2 writes it), so that it checks the kernels' sparse
+ * lane algebra (cpi_b200/csrc/record_merge.cuh) instead of repeating it.  A record is the [290] layout of include/cpi_b200.h
+ * held in `real`; 3x3 blocks are column-major, as everywhere in this file. */
+enum { RD1 = CPI_REC_V1_DOUBLES };
+
+static void rec_zero(real* r) {
+    mat_zero(r, RD1);
+    r[CPI_REC_Q + 3] = 1.0;
+    mat_eye(r + CPI_REC_R, 3);
+}
+
+/* Move a record from its linearisation point lin_k to lin_0, to first order: R <- Exp(J_q db_w) R, alpha += J_a db_w + H_a db_a,
+ * beta += J_b db_w + H_b db_a, with db = lin_0 - lin_k from the double values; nothing moves when all six differences are 0.
+ * q, the Jacobians and P are left as they are (the merge recomputes q from R). */
+static void rec_relinearise(real* r, const double* lin0, const double* link) {
+    real dbw[3], dba[3], t[3], Ex[9], Rn[9], u[3], w[3];
+    int moved = 0;
+    for (int i = 0; i < 3; i++) {
+        dbw[i] = (real)lin0[i] - (real)link[i];
+        dba[i] = (real)lin0[3 + i] - (real)link[3 + i];
+        moved |= dbw[i] != 0 || dba[i] != 0;
+    }
+    if (!moved) return;
+    m3_vec(r + CPI_REC_JQ, dbw, t);
+    Exp(t, Ex);
+    gemm(3, 3, 3, Ex, r + CPI_REC_R, Rn);
+    memcpy(r + CPI_REC_R, Rn, sizeof Rn);
+    m3_vec(r + CPI_REC_JA, dbw, u); m3_vec(r + CPI_REC_HA, dba, w);
+    for (int i = 0; i < 3; i++) r[CPI_REC_ALPHA + i] += u[i] + w[i];
+    m3_vec(r + CPI_REC_JB, dbw, u); m3_vec(r + CPI_REC_HB, dba, w);
+    for (int i = 0; i < 3; i++) r[CPI_REC_BETA + i] += u[i] + w[i];
+}
+
+/* A^-1 of a 3x3 matrix: adjugate over determinant */
+static void m3_inv(const real* A, real* Ai) {
+    real c[9];
+    for (int j = 0; j < 3; j++) for (int i = 0; i < 3; i++) {
+        int i1 = (i + 1) % 3, i2 = (i + 2) % 3, j1 = (j + 1) % 3, j2 = (j + 2) % 3;
+        E(c, 3, i, j) = E(A, 3, i1, j1) * E(A, 3, i2, j2) - E(A, 3, i1, j2) * E(A, 3, i2, j1);   /* cofactor (i, j) */
+    }
+    real det = E(A, 3, 0, 0) * E(c, 3, 0, 0) + E(A, 3, 0, 1) * E(c, 3, 0, 1) + E(A, 3, 0, 2) * E(c, 3, 0, 2);
+    for (int j = 0; j < 3; j++) for (int i = 0; i < 3; i++) E(Ai, 3, i, j) = E(c, 3, j, i) / det;
+}
+
+/* out = A (+) B: A covers k -> m, B covers m -> j, both at one linearisation point.  out may not alias A or B. */
+static void rec_merge(const real* A, const real* B, real* out) {
+    const real *R1 = A + CPI_REC_R, *R2 = B + CPI_REC_R;
+    const real dt2 = B[CPI_REC_DT];
+    real R1T[9], sk[9], t9[9], u9[9], t3[3], eye[9];
+    mat_eye(eye, 3);
+    transpose(3, 3, R1, R1T);
+    mat_zero(out, RD1);
+    gemm(3, 3, 3, R2, R1, out + CPI_REC_R);                                          /* R = R2 R1 */
+    out[CPI_REC_DT] = A[CPI_REC_DT] + dt2;
+    m3_vec(R1T, B + CPI_REC_BETA, t3);                                               /* beta = b1 + R1^T b2 */
+    for (int i = 0; i < 3; i++) out[CPI_REC_BETA + i] = A[CPI_REC_BETA + i] + t3[i];
+    m3_vec(R1T, B + CPI_REC_ALPHA, t3);                                              /* alpha = a1 + b1 DT2 + R1^T a2 */
+    for (int i = 0; i < 3; i++) out[CPI_REC_ALPHA + i] = A[CPI_REC_ALPHA + i] + A[CPI_REC_BETA + i] * dt2 + t3[i];
+    gemm(3, 3, 3, R2, A + CPI_REC_JQ, t9);                                           /* J_q = R2 J_q1 + J_q2 */
+    for (int e = 0; e < 9; e++) out[CPI_REC_JQ + e] = t9[e] + B[CPI_REC_JQ + e];
+    gemm(3, 3, 3, R1T, B + CPI_REC_HB, t9);                                          /* H_b = H_b1 + R1^T H_b2 */
+    for (int e = 0; e < 9; e++) out[CPI_REC_HB + e] = A[CPI_REC_HB + e] + t9[e];
+    gemm(3, 3, 3, R1T, B + CPI_REC_HA, t9);                                          /* H_a = H_a1 + H_b1 DT2 + R1^T H_a2 */
+    for (int e = 0; e < 9; e++) out[CPI_REC_HA + e] = A[CPI_REC_HA + e] + A[CPI_REC_HB + e] * dt2 + t9[e];
+    skew_x(B + CPI_REC_BETA, sk); gemm(3, 3, 3, sk, A + CPI_REC_JQ, u9);             /* J_b = J_b1 + R1^T([b2] J_q1 + J_b2) */
+    for (int e = 0; e < 9; e++) u9[e] += B[CPI_REC_JB + e];
+    gemm(3, 3, 3, R1T, u9, t9);
+    for (int e = 0; e < 9; e++) out[CPI_REC_JB + e] = A[CPI_REC_JB + e] + t9[e];
+    skew_x(B + CPI_REC_ALPHA, sk); gemm(3, 3, 3, sk, A + CPI_REC_JQ, u9);            /* J_a = J_a1 + J_b1 DT2 + R1^T([a2] J_q1 + J_a2) */
+    for (int e = 0; e < 9; e++) u9[e] += B[CPI_REC_JA + e];
+    gemm(3, 3, 3, R1T, u9, t9);
+    for (int e = 0; e < 9; e++) out[CPI_REC_JA + e] = A[CPI_REC_JA + e] + A[CPI_REC_JB + e] * dt2 + t9[e];
+
+    /* Phi2 over [theta, b_g, v, b_a, p], T = blockdiag(I, I, R1^T, I, R1^T) (window 2's v and p error states are in frame m),
+     * Phi~ = T Phi2 T^-1, P = Phi~ P1 Phi~^T + T P2 T^T.  T^-1 = T^T for an orthogonal R1; a stored R1 is orthogonal only to its
+     * rounding (2^-24 in fp32 storage), and the similarity transform is the one that composes: Phi~ x = T Phi2 (T^-1 x). */
+    real Phi2[225], T[225], Ti[225], X[225], Phi[225], Y[225], R1Ti[9];
+    m3_inv(R1T, R1Ti);
+    mat_eye(Phi2, 15);
+    set_block(Phi2, 15, 0, 0, 3, 3, R2, 1.0);
+    set_block(Phi2, 15, 0, 3, 3, 3, B + CPI_REC_JQ, -1.0);
+    skew_x(B + CPI_REC_BETA, sk); set_block(Phi2, 15, 6, 0, 3, 3, sk, -1.0);
+    set_block(Phi2, 15, 6, 3, 3, 3, B + CPI_REC_JB, 1.0);
+    set_block(Phi2, 15, 6, 9, 3, 3, B + CPI_REC_HB, 1.0);
+    skew_x(B + CPI_REC_ALPHA, sk); set_block(Phi2, 15, 12, 0, 3, 3, sk, -1.0);
+    set_block(Phi2, 15, 12, 3, 3, 3, B + CPI_REC_JA, 1.0);
+    set_block(Phi2, 15, 12, 6, 3, 3, eye, dt2);
+    set_block(Phi2, 15, 12, 9, 3, 3, B + CPI_REC_HA, 1.0);
+    mat_eye(T, 15);
+    set_block(T, 15, 6, 6, 3, 3, R1T, 1.0);
+    set_block(T, 15, 12, 12, 3, 3, R1T, 1.0);
+    mat_eye(Ti, 15);
+    set_block(Ti, 15, 6, 6, 3, 3, R1Ti, 1.0);
+    set_block(Ti, 15, 12, 12, 3, 3, R1Ti, 1.0);
+    gemm(15, 15, 15, T, Phi2, X); gemm(15, 15, 15, X, Ti, Phi);
+    gemm(15, 15, 15, Phi, A + CPI_REC_P, X); gemm_nt(15, 15, 15, X, Phi, Y);
+    gemm(15, 15, 15, T, B + CPI_REC_P, X); gemm_nt(15, 15, 15, X, T, Phi2);
+    for (int e = 0; e < 225; e++) out[CPI_REC_P + e] = Y[e] + Phi2[e];
+    rot_2_quat(out + CPI_REC_R, out + CPI_REC_Q);
+}
+
+/* The left fold of records lo .. hi-1 (global indices into rec / lin), every later record first moved to lin[lo]; merged: the
+ * fold (an empty group gives the zero-step record, a group of one a copy), prefix: every prefix fold at its record's row. */
+static void fold_group(const double* rec, const double* lin, int64_t lo, int64_t hi, double* merged, double* prefix) {
+    if (hi <= lo) {
+        if (merged) { real z[RD1]; rec_zero(z); store(merged, z, RD1); }
+        return;
+    }
+    real* acc = (real*)malloc(3 * RD1 * sizeof(real));
+    real *nx = acc + RD1, *tmp = acc + 2 * RD1;
+    load(acc, rec + lo * RD1, RD1);
+    if (prefix) store(prefix + lo * RD1, acc, RD1);
+    for (int64_t k = lo + 1; k < hi; k++) {
+        load(nx, rec + k * RD1, RD1);
+        rec_relinearise(nx, lin + lo * CPI_LIN_DOUBLES, lin + k * CPI_LIN_DOUBLES);
+        rec_merge(acc, nx, tmp);
+        memcpy(acc, tmp, RD1 * sizeof(real));
+        if (prefix) store(prefix + k * RD1, acc, RD1);
+    }
+    if (merged) store(merged, acc, RD1);
+    free(acc);
+}
+
+typedef struct {
+    int kind, t, nt; int64_t n;                  /* kind 0: pairs, 1: relinearise, 2: merge groups, 3: scan groups */
+    const int64_t* offsets; int64_t uniform;
+    const double *a, *b, *lin, *lin0;
+    double* out;
+} rjob_t;
+
+static void* rworker(void* arg) {
+    rjob_t* j = (rjob_t*)arg;
+    int64_t lo = j->n * j->t / j->nt, hi = j->n * (j->t + 1) / j->nt;
+    real* x = (real*)malloc(3 * RD1 * sizeof(real));
+    for (int64_t i = lo; i < hi; i++) {
+        if (j->kind == 0) {
+            load(x, j->a + i * RD1, RD1); load(x + RD1, j->b + i * RD1, RD1);
+            rec_merge(x, x + RD1, x + 2 * RD1);
+            store(j->out + i * RD1, x + 2 * RD1, RD1);
+        } else if (j->kind == 1) {
+            load(x, j->a + i * RD1, RD1);
+            rec_relinearise(x, j->lin0 + i * CPI_LIN_DOUBLES, j->lin + i * CPI_LIN_DOUBLES);
+            store(j->out + i * RD1, x, RD1);
+        } else {
+            int64_t g0 = j->offsets ? j->offsets[i] : i * j->uniform, g1 = j->offsets ? j->offsets[i + 1] : g0 + j->uniform;
+            if (j->kind == 2) fold_group(j->a, j->lin, g0, g1, j->out + i * RD1, 0);
+            else fold_group(j->a, j->lin, g0, g1, 0, j->out);
+        }
+    }
+    free(x);
+    return 0;
+}
+
+static void rrun(rjob_t* proto, int nthreads) {
+    if (nthreads < 1) nthreads = 1;
+    if (nthreads > 256) nthreads = 256;
+    rjob_t jobs[256]; pthread_t th[256];
+    for (int t = 0; t < nthreads; t++) { jobs[t] = *proto; jobs[t].t = t; jobs[t].nt = nthreads; }
+    if (nthreads == 1) { rworker(&jobs[0]); return; }
+    for (int t = 0; t < nthreads; t++) pthread_create(&th[t], 0, rworker, &jobs[t]);
+    for (int t = 0; t < nthreads; t++) pthread_join(th[t], 0);
+}
+
+int oracle_merge_pair(int64_t n, const double* a, const double* b, double* out, int nthreads) {
+    rjob_t j; memset(&j, 0, sizeof j);
+    j.kind = 0; j.n = n; j.a = a; j.b = b; j.out = out;
+    rrun(&j, nthreads);
+    return 0;
+}
+
+int oracle_relinearise_records(int64_t n, const double* records, const double* lin, const double* lin0, double* out) {
+    rjob_t j; memset(&j, 0, sizeof j);
+    j.kind = 1; j.n = n; j.a = records; j.lin = lin; j.lin0 = lin0; j.out = out;
+    rrun(&j, 1);
+    return 0;
+}
+
+static int group_job(int kind, int64_t n_groups, const int64_t* offsets, int64_t uniform, const double* records, const double* lin,
+                     double* out, int nthreads) {
+    if (n_groups < 0 || (!offsets && uniform < 0)) return -1;
+    rjob_t j; memset(&j, 0, sizeof j);
+    j.kind = kind; j.n = n_groups; j.offsets = offsets; j.uniform = uniform; j.a = records; j.lin = lin; j.out = out;
+    rrun(&j, nthreads);
+    return 0;
+}
+
+int oracle_merge_records(int64_t n_groups, const int64_t* offsets, int64_t uniform, const double* records, const double* lin,
+                         double* out, int nthreads) {
+    return group_job(2, n_groups, offsets, uniform, records, lin, out, nthreads);
+}
+
+int oracle_scan_records(int64_t n_groups, const int64_t* offsets, int64_t uniform, const double* records, const double* lin,
+                        double* out, int nthreads) {
+    return group_job(3, n_groups, offsets, uniform, records, lin, out, nthreads);
+}
+
 /* ------------------------------------------------------------------ batch drivers -------------------------------- */
 typedef struct {
     int kind, model, flags, t, nt; int64_t n;

@@ -17,6 +17,18 @@ int oracle_predict_state(int model, int64_t n, const double* states_k, const dou
                          double* states_k1);
 int oracle_retract(int64_t n, const double* states, const double* xi, double* out);
 
+/* Model-1 record composition (DESIGN.md 3b, 3c), dense.  merge_pair: out[i] = a[i] (+) b[i], both at one linearisation point.
+ * relinearise_records: out[i] = records[i] moved from lin[i] to lin0[i] to first order.  merge_records / scan_records: the left
+ * fold of every group (CSR offsets, or groups of `uniform` records when offsets is NULL), every later record moved to the
+ * group's first linearisation point; merge writes one record per group (empty group: the zero-step record), scan writes every
+ * prefix fold at its record's row of out (shaped like records; rows outside every group are not written). */
+int oracle_merge_pair(int64_t n, const double* a, const double* b, double* out, int nthreads);
+int oracle_relinearise_records(int64_t n, const double* records, const double* lin, const double* lin0, double* out);
+int oracle_merge_records(int64_t n_groups, const int64_t* offsets, int64_t uniform, const double* records, const double* lin,
+                         double* out, int nthreads);
+int oracle_scan_records(int64_t n_groups, const int64_t* offsets, int64_t uniform, const double* records, const double* lin,
+                        double* out, int nthreads);
+
 /* quat_ops.h helpers (col-major 3x3) */
 void oracle_rot_2_quat(const double* R, double* q);
 void oracle_quat_2_Rot(const double* q, double* R);

@@ -137,6 +137,73 @@ class Oracle(_Base):
         self._pred(model, states_k.shape[0], _d(states_k), _d(records), _d(lin), _d(out))
         return out
 
+    # ---- model-1 record composition (merge / scan).  Bound on first use, so that a library built before these entry points
+    # existed still serves everything above.
+    def _rec_fn(self, name, argtypes):
+        f = getattr(self.lib, name, None)
+        if f is None:
+            # dlopen hands back the image this process already mapped for the same path, even after a rebuild: load the file
+            # on disk under another name if it has the symbol
+            import shutil
+            import tempfile
+            tmp = os.path.join(tempfile.mkdtemp(prefix="cpi_oracle_"), os.path.basename(self.path))
+            shutil.copyfile(self.path, tmp)
+            lib = ctypes.CDLL(tmp)
+            f = getattr(lib, name, None)
+            if f is None:
+                raise AttributeError(f"{self.path} has no {name}: rebuild it (make -C oracle)")
+            self.lib = lib
+        f.argtypes = argtypes
+        f.restype = ctypes.c_int
+        return f
+
+    @staticmethod
+    def _groups(n_rec, group_offsets, group):
+        if group_offsets is not None:
+            offs = np.ascontiguousarray(group_offsets, dtype=np.int64)
+            assert offs.ndim == 1 and offs.shape[0] >= 1 and offs[-1] <= n_rec
+            return offs.shape[0] - 1, offs, 0
+        assert group is not None and group >= 1 and n_rec % group == 0
+        return n_rec // group, None, int(group)
+
+    def merge_pair(self, a, b, nthreads=1):
+        """out[i] = a[i] (+) b[i]: two consecutive model-1 records at one linearisation point."""
+        f = self._rec_fn("oracle_merge_pair", [ctypes.c_int64, _P, _P, _P, ctypes.c_int])
+        a = np.ascontiguousarray(a, dtype=np.float64).reshape(-1, REC_DOUBLES[1])
+        b = np.ascontiguousarray(b, dtype=np.float64).reshape(-1, REC_DOUBLES[1])
+        assert a.shape == b.shape
+        out = np.zeros_like(a)
+        assert f(a.shape[0], _d(a), _d(b), _d(out), int(nthreads)) == 0
+        return out
+
+    def relinearise(self, records, lin, lin0):
+        """records[i], preintegrated at lin[i], moved to lin0[i] to first order (q, Jacobians and P unchanged)."""
+        f = self._rec_fn("oracle_relinearise_records", [ctypes.c_int64, _P, _P, _P, _P])
+        records = np.ascontiguousarray(records, dtype=np.float64).reshape(-1, REC_DOUBLES[1])
+        lin = np.ascontiguousarray(lin, dtype=np.float64).reshape(-1, 13)
+        lin0 = np.ascontiguousarray(lin0, dtype=np.float64).reshape(-1, 13)
+        out = np.zeros_like(records)
+        assert f(records.shape[0], _d(records), _d(lin), _d(lin0), _d(out)) == 0
+        return out
+
+    def _fold(self, name, records, lin, group_offsets, group, nthreads, scan):
+        f = self._rec_fn(name, [ctypes.c_int64, _PI, ctypes.c_int64, _P, _P, _P, ctypes.c_int])
+        records = np.ascontiguousarray(records, dtype=np.float64).reshape(-1, REC_DOUBLES[1])
+        lin = np.ascontiguousarray(lin, dtype=np.float64).reshape(-1, 13)
+        assert lin.shape[0] == records.shape[0]
+        n, offs, uniform = self._groups(records.shape[0], group_offsets, group)
+        out = np.zeros_like(records) if scan else np.zeros((n, REC_DOUBLES[1]))
+        assert f(n, _i(offs), uniform, _d(records), _d(lin), _d(out), int(nthreads)) == 0
+        return out
+
+    def merge_records(self, records, lin, group_offsets=None, group=None, nthreads=1):
+        """The left fold of every group (layout as cpi_merge_records_host): one record per group."""
+        return self._fold("oracle_merge_records", records, lin, group_offsets, group, nthreads, False)
+
+    def scan_records(self, records, lin, group_offsets=None, group=None, nthreads=1):
+        """Every prefix of the left fold of every group (layout as cpi_scan_records_host); rows outside every group are zero."""
+        return self._fold("oracle_scan_records", records, lin, group_offsets, group, nthreads, True)
+
 
 class OracleLD(Oracle):
     """The same restatement computed in long double (oracle/liboracle_ld.so): double in, double out, about 1e-19 working

@@ -146,12 +146,12 @@ def test_long_groups_spread_over_many_ctas(cuda):
     """One group of 5 000 records and one of 10^5 (tiled from the pool, each at a different linearisation point): sampled prefixes (the
     first, around chunk edges of every level, the last) against the numpy fold.  Observed on one H100 80GB HBM3 (700 W): means,
     Jacobians, q and DT <= 4.2e-14 and 1.5e-13; P 7.1e-11 at 5 000 and 3.5e-8 at 10^5 records.  P is ill-conditioned in the
-    bracketing over such chains: the numpy fold and a numpy pairwise tree of the same records differ by 1.9e-10 and 5.3e-8 on P.
-    The P gate is about 5x the observed value at each length."""
+    bracketing over such chains (the numpy fold and a numpy pairwise tree of the same records differ by 1.9e-10 and 5.3e-8), so
+    P is gated per block against the long-double fold in test_record_precision.test_long_groups, not here."""
     from cpi_b200 import preint
     torch = cuda
     pool, Lp = _record_pool(n=2048, first_window=74000)
-    for n, seed, tol_P in ((5000, 6, 5e-10), (100_000, 7, 2e-7)):
+    for n, seed in ((5000, 6), (100_000, 7)):
         rng = np.random.default_rng(seed)
         rec = pool[np.arange(n) % len(pool)]; lin = Lp[rng.integers(0, len(pool), size=n)]
         edges = [e + k for e in (CHUNK, CHUNK ** 2, CHUNK ** 3) for k in (-1, 0, 1) if e + k < n]
@@ -165,7 +165,6 @@ def test_long_groups_spread_over_many_ctas(cuda):
         print(n, {k: f"{v:.1e}" for k, v in err.items()})
         for k in FIELDS + ("q", "DT"):
             assert err[k] <= 1e-12, (n, k, err[k])
-        assert err["P"] <= tol_P, (n, err["P"])
 
 
 @pytest.mark.gpu
