@@ -109,6 +109,7 @@ int preintegrate_dev(int model, int dtype, int64_t n_windows, const int64_t* sam
     if (model != 1 && model != 2) return fail(CPI_EINVAL, "model must be 1 or 2 (got %d)", model);
     if (dtype != 64 && dtype != 32) return fail(CPI_EINVAL, "dtype must be 64 or 32 (got %d)", dtype);
     if (n_windows < 0 || (!sample_offsets && ns_uniform < 0)) return fail(CPI_EINVAL, "negative count");
+    if (n_windows >= 2147483647) return fail(CPI_EINVAL, "too many windows (%lld; at most 2^31 - 2 per call)", (long long)n_windows);
     if (n_windows == 0) return CPI_OK;
     if (!lin || !sigmas || !out_records) return fail(CPI_EINVAL, "null pointer argument");
     // device-resident CSR offsets cannot be inspected here: a NULL samples pointer is only rejected when the layout is uniform and
@@ -121,7 +122,7 @@ int preintegrate_dev(int model, int dtype, int64_t n_windows, const int64_t* sam
     cpi::PreintParams p;
     p.n_windows = n_windows; p.offsets = sample_offsets; p.ns_uniform = ns_uniform;
     p.samples = samples; p.lin = lin; p.out = out_records; p.init = init_records;
-    if (init_records && (!cpi::preint_tri_supported(model, flags) || getenv("CPI_B200_LEGACY")))
+    if (init_records && !cpi::preint_tri_supported(model, flags))
         return fail(CPI_EINVAL, "continuation is implemented for the default modes only (no imu_avg, model 2 with state_transition_jacobians)");
     p.q_w = sigmas[0] * sigmas[0]; p.q_wb = sigmas[1] * sigmas[1]; p.q_a = sigmas[2] * sigmas[2]; p.q_ab = sigmas[3] * sigmas[3];
     p.wpb = wpb;
@@ -240,7 +241,7 @@ int cpi_preintegrate_batch_host(int model, int dtype, int64_t n_windows, const i
         const int nf = sscanf(e, "%d,%d,%d", &a_, &b_, &c_);
         if (nf >= 2 && a_ >= 0 && a_ <= 256 && b_ >= 0 && b_ <= 64 && c_ >= 0 && c_ < 100) { wave_G = a_; wave_S = b_; wave_H = nf == 3 ? c_ : 0; }
     }
-    const bool wave = dtype == 64 && !sample_offsets && !avg && small_ctas && cpi::preint_tri_supported(model, flags) && !getenv("CPI_B200_LEGACY") &&
+    const bool wave = dtype == 64 && !sample_offsets && !avg && small_ctas && cpi::preint_tri_supported(model, flags) &&
                       wave_G >= 1 && wave_S >= 2 && ns_uniform >= 2 * (int64_t)wave_S;
     const int64_t head_blocks = wave ? blocks * wave_H / 100 : blocks;
     const int64_t head_hi = wave ? head_blocks * wpb : n_windows;    // windows [0, head_hi) travel whole, [head_hi, n) as the wavefront

@@ -44,7 +44,6 @@ struct FactorParams {
 };
 
 int preint_pick_wpb(int model, int dtype, int64_t n_windows, int num_sms);
-int preint_ws_cap(int dtype);
 int preint_cap(int model, int dtype, int flags, int num_sms);
 // tri-lane kernels (preintegrate_tri.cu)
 bool preint_tri_supported(int model, int flags);

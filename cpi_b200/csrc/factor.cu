@@ -18,9 +18,8 @@ namespace cpi {
 // 6 CTAs per SM (round 1: 16 x 128 threads at 255 registers -> 2 per SM).  625 CTAs for a 5k chain: all resident in one wave.
 constexpr int FPB = 8;
 constexpr int FTHREADS = 64;
-#ifndef CPI_K3_MINB
-#define CPI_K3_MINB 6        /* resident CTAs per SM the register allocation aims at: 6 (168 registers, ~400 B of spills) measured faster than 4 (255, none): 789 vs 671 M factors/s at 1M */
-#endif
+// resident CTAs per SM the register allocation aims at: 6 (168 registers, ~400 B of spills) measured faster than 4 (255, none): 789 vs 671 M factors/s at 1M
+constexpr int K3_MIN_BLOCKS = 6;
 constexpr int FTILE = 15 + 225 + 225;   // doubles per factor in the staging tile
 
 
@@ -37,7 +36,7 @@ CPI_DEV void putI(double* H, int r0, int c0, double s) {
 }
 
 template <int MODEL>
-__global__ void __launch_bounds__(FTHREADS, CPI_K3_MINB) k_factor_eval(const FactorParams p) {
+__global__ void __launch_bounds__(FTHREADS, K3_MIN_BLOCKS) k_factor_eval(const FactorParams p) {
     extern __shared__ double tile[];
     const int tid = threadIdx.x;
     const int64_t f0 = (int64_t)blockIdx.x * FPB;

@@ -52,13 +52,9 @@ template <class T> CPI_DEV void gather_cols(const T* V, int nx, int pv, T* X1, T
 
 // ---- per-model layout --------------------------------------------------------------------------------------------------
 // RK4 stage values handed from the (theta|v)-column group to the p-column group through LANE-PRIVATE shared memory
-// slots, [entry][thread]: TV, GV, AV, VV (model 2: + CV) for the four stages.
+// slots, [entry][thread]: TV, GV (model 2: + CV) for the four stages.
 template <int MODEL> struct TriL {
-#ifndef CPI_TRI_UNFUSED12
     static constexpr int NSL = (MODEL == 1 ? 6 : 9) * 4 + (MODEL == 1 ? 0 : 9);   // TV, GV (+ CV) for the four stages; model 2: + TG(start) columns 1, 2 and TT(start) 11, 21, 22
-#else
-    static constexpr int NSL = (MODEL == 1 ? 12 : 15) * 4;      // + AV, VV in the split cascade
-#endif
     // front state parked in lane-private smem during the covariance step: bw, ba, alpha, beta, then
     //   model 1: J_q, J_a, J_b, H_a, H_b (own columns)      model 2: g_k and the own columns of the 7 non-trivial Discrete_J_b blocks
     static constexpr int NFS = (MODEL == 1) ? 23 : 32;
@@ -69,36 +65,21 @@ template <int MODEL, class T> struct TriSmem {
     static constexpr int NT = TriNT<MODEL, T>::NT;
     static constexpr int WPB = TRI_WPW * NT / 32;                     // window slots per CTA
     static constexpr size_t off_fs = (size_t)TriL<MODEL>::NSL * NT * sizeof(T);
-#ifdef CPI_TRI_PSMEM
-    static constexpr size_t off_sc = off_fs + (size_t)33 * NT * 8;
-#else
     static constexpr size_t off_sc = off_fs + (size_t)TriL<MODEL>::NFS * NT * 8;
-#endif
     // scalar sets: one slot per window + one dummy slot per warp for the two idle lanes
     static constexpr size_t off_buf = (off_sc + (size_t)(WPB + NT / 32) * TriSC<MODEL>::STRIDE * 8 + 127) / 128 * 128;
     static constexpr size_t off_bar = off_buf + (size_t)WPB * TRI_BUF_STRIDE;
     static constexpr size_t bytes = off_bar + (size_t)WPB * 8 * TRI_NBUF;
 };
-#ifndef CPI_TRI_PSMEM
-static_assert(TriSmem<1, double>::bytes <= 28160 - 1024 && TriSmem<1, float>::bytes <= 28160 - 1024 && TriSmem<2, float>::bytes <= 28160 - 1024,
+static_assert(TriSmem<1, double>::bytes <= 28160 - 1024 && TriSmem<1, float>::bytes <= 28160 - 1024 && TriSmem<2, double>::bytes <= 28160 - 1024 &&
+              TriSmem<2, float>::bytes <= 28160 - 1024,
               "8 CTAs per SM need <= 220 KB / 8 of shared memory each (incl. 1 KB the system reserves per CTA)");
-static_assert(TriSmem<2, double>::bytes <= 32182 - 1024, "model 2 fp64 (split cascade: 7 CTAs per SM)");
-#endif
 
 #define SLT(e) sl[(e) * NT]
-#ifdef CPI_TRI_PSMEM        // experiment: covariance state parked in lane-private smem between groups, front state in registers
-#define FST(e) fsr[e]
-#define PST(e) ps[(e) * NT]   /* ps is double* in this variant */
-#else
 #define FST(e) fs[(e) * NT]
-#endif
 #define CN(s) ((s) < 2 ? hdt : dt)                       /* x_{s+2} = x_1 + CN(s) k_{s+1}:  dt/2, dt/2, dt   (CpiV1.h:312, 323, 344) */
 #define KSUM(ks, k, s) ((s) == 0 ? (k) : ((s) == 3 ? (ks) + (k) : fma(T(2), (k), (ks))))   /* ((k1 + 2 k2) + 2 k3) + k4  (CpiV1.h:352) */
-#ifdef CPI_TRI_NOFENCE
-#define CPI_FENCE()
-#else
 #define CPI_FENCE() asm volatile("" ::: "memory")
-#endif
 
 // -(R^T u): element i = -(column i of R) . u      (R row-major 3x3)
 template <class T> CPI_DEV void negRt(const T* R, const T* u, T* o) {
@@ -116,22 +97,12 @@ template <class T> struct TriP {
 // One RK4 step of the covariance (model 1: CpiV1.h:272-353).  w, ah: estimated readings; R, Rm, R1: old / mid / new
 // rotation (row-major, lane frame); pgg, paa: the scalar diagonal blocks P_bg,bg and P_ba,ba at the start of the step.
 template <int MODEL, int NT, class T>
-CPI_DEV void tri_cov_step(TriP<T>& P, T* sl, double* ps, const T* w, const T* ah, const T* gt, const T* R, const T* Rm, const T* R1, T pgg, T paa, T dt, T dt6,
+CPI_DEV void tri_cov_step(TriP<T>& P, T* sl, const T* w, const T* ah, const T* gt, const T* R, const T* Rm, const T* R1, T pgg, T paa, T dt, T dt6,
                           T q_w, T q_wb, T q_a, T q_ab, int nx, int pv) {
     const T hdt = dt * T(0.5);
-#ifndef CPI_TRI_UNFUSED12
     constexpr int NS = (MODEL == 1) ? 6 : 9;              // slot entries per stage: TV, GV (+ CV)
     constexpr int SL_CV = 6;
-#ifdef CPI_TRI_M2_NOPARK
-    constexpr bool PARK = false;
-#else
     constexpr bool PARK = MODEL == 2 && sizeof(T) == 8;   // model 2 fp64: halves the register spills (ptxas: 200 -> 116 B of spill stores per sample)
-#endif
-#else
-    constexpr bool PARK = false;
-    constexpr int NS = (MODEL == 1) ? 12 : 15;            // slot entries per stage: TV, GV, AV, VV (+ CV)
-    constexpr int SL_CV = 12;
-#endif
     // Model 2 (CpiV2.h:326-443): the clone rows c of P_big are re-initialised from the theta rows at every step (B_k), so within a
     // step  P_cg = TG(start), P_cc = TT(start), P_ca = 0  are constant and only three transient blocks evolve:
     //     TC = P_theta,c  (starts as TT):  TC' = -W TC - TG(start)^T            [needs nothing cross-lane; TV and CV need all of it]
@@ -139,10 +110,6 @@ CPI_DEV void tri_cov_step(TriP<T>& P, T* sl, double* ps, const T* w, const T* ah
     //     CP = P_c,p      (starts as TP):  CP' = CV                            [recomputed from CV's stage values]
     // and the v rows gain  C_s P_c,J  with  C_s = -R_s^T [g_tau x]  (CpiV2.h:335).
     {   // ---- group 1a: TG, TT, GV, TV, stage by stage (self-contained: needs only w, the rotations and a_hat)
-#ifdef CPI_TRI_PSMEM
-#pragma unroll
-        for (int e = 0; e < 3; e++) { P.TG[e] = PST(e); P.TT[e] = PST(3 + e); P.GV[e] = PST(6 + e); P.TV[e] = PST(9 + e); }
-#endif
         T xTG[3], xTT[3], xGV[3], xTV[3], xTC[3], xCV[3];
         T sTG[3], sTT[3], sGV[3], sTV[3];
         T G1s[3], G2s[3], tts[3];                             // model 2: TG(start) columns 1, 2 and TT(start) entries 11, 21, 22
@@ -239,13 +206,8 @@ CPI_DEV void tri_cov_step(TriP<T>& P, T* sl, double* ps, const T* w, const T* ah
             P.TG[e] = fma((double)dt6, (double)sTG[e], P.TG[e]); P.TT[e] = fma((double)dt6, (double)sTT[e], P.TT[e]);
             P.GV[e] = fma((double)dt6, (double)sGV[e], P.GV[e]); P.TV[e] = fma((double)dt6, (double)sTV[e], P.TV[e]);
         }
-#ifdef CPI_TRI_PSMEM
-#pragma unroll
-        for (int e = 0; e < 3; e++) { PST(e) = P.TG[e]; PST(3 + e) = P.TT[e]; PST(6 + e) = P.GV[e]; PST(9 + e) = P.TV[e]; }
-#endif
     }
     CPI_FENCE();
-#ifndef CPI_TRI_UNFUSED12      /* default: groups 1b and 2 fused (measured +6..8 % over the split cascade, which stays for A/B runs) */
     {   // ---- groups 1b + 2 fused: AV, VV, TP, GP, AP, VP, PP in ONE stage loop (AV / VV never go through the slots)
         T xAV[3], xVV[3], sAV[3], sVV[3], oAV[3], oVV[3];
         T xTP[3], xGP[3], xAP[3], xVP[3], oTP[3], oGP[3], oAP[3], oVP[3];
@@ -327,126 +289,6 @@ CPI_DEV void tri_cov_step(TriP<T>& P, T* sl, double* ps, const T* w, const T* ah
     CPI_FENCE();
 }
 
-#else
-    {   // ---- group 1b: AV, VV (need TV's stage values)
-        T xAV[3], xVV[3], sAV[3], sVV[3], oAV[3], oVV[3];
-#ifdef CPI_TRI_PSMEM
-#pragma unroll
-        for (int e = 0; e < 3; e++) { P.AV[e] = PST(12 + e); P.VV[e] = PST(15 + e); }
-#endif
-#pragma unroll
-        for (int e = 0; e < 3; e++) { oAV[e] = (T)P.AV[e]; oVV[e] = (T)P.VV[e]; xAV[e] = oAV[e]; xVV[e] = oVV[e]; }
-#pragma unroll
-        for (int s = 0; s < 4; s++) {
-            const T* Rs = (s == 0) ? R : (s == 3 ? R1 : Rm);
-            const T rc[3] = {Rs[0], Rs[3], Rs[6]};
-            T tv[3];
-#pragma unroll
-            for (int e = 0; e < 3; e++) { tv[e] = SLT(s * NS + e); SLT(s * NS + 6 + e) = xAV[e]; SLT(s * NS + 9 + e) = xVV[e]; }
-            const T pa_s = (s == 0) ? paa : fma(q_ab, (s == 3 ? dt : hdt), paa);
-            T kAV[3], kVV[3];
-            // AV:  paa_s B_s[0,:]^T = -paa_s (column 0 of R_s)
-#pragma unroll
-            for (int e = 0; e < 3; e++) kAV[e] = -(pa_s * rc[e]);
-            // VV:  M + M^T + q_a I,  M[:,0] = A_s TV_0 + B_s AV_0 = -R_s^T (a x TV_0 + AV_0)
-            {
-                T u[3], m0[3];
-                cross(ah, tv, u);
-#pragma unroll
-                for (int e = 0; e < 3; e++) u[e] += xAV[e];
-                if (MODEL == 2) {                             // + C_s CV_0 = -R_s^T (g_tau x CV_0)
-                    T cv[3], u2[3];
-#pragma unroll
-                    for (int e = 0; e < 3; e++) cv[e] = SLT(s * NS + SL_CV + e);
-                    cross(gt, cv, u2);
-#pragma unroll
-                    for (int e = 0; e < 3; e++) u[e] += u2[e];
-                }
-                negRt(Rs, u, m0);
-                const T m01 = shf(m0[2], nx), m02 = shf(m0[1], pv);   // M[0,1], M[0,2]
-                kVV[0] = m0[0] + m0[0] + q_a; kVV[1] = m0[1] + m01; kVV[2] = m0[2] + m02;
-            }
-#pragma unroll
-            for (int e = 0; e < 3; e++) {
-                sAV[e] = KSUM(sAV[e], kAV[e], s); sVV[e] = KSUM(sVV[e], kVV[e], s);
-                if (s < 3) { xAV[e] = fma(kAV[e], CN(s), oAV[e]); xVV[e] = fma(kVV[e], CN(s), oVV[e]); }
-            }
-        }
-#pragma unroll
-        for (int e = 0; e < 3; e++) { P.AV[e] = fma((double)dt6, (double)sAV[e], P.AV[e]); P.VV[e] = fma((double)dt6, (double)sVV[e], P.VV[e]); }
-#ifdef CPI_TRI_PSMEM
-#pragma unroll
-        for (int e = 0; e < 3; e++) { PST(12 + e) = P.AV[e]; PST(15 + e) = P.VV[e]; }
-#endif
-    }
-    CPI_FENCE();
-    {   // ---- group 2: the p-column blocks TP, GP, AP, VP, PP
-        T xTP[3], xGP[3], xAP[3], xVP[3], oTP[3], oGP[3], oAP[3], oVP[3];
-        T sTP[3], sGP[3], sAP[3], sVP[3], sPP[3];
-#ifdef CPI_TRI_PSMEM
-#pragma unroll
-        for (int e = 0; e < 3; e++) { P.TP[e] = PST(18 + e); P.GP[e] = PST(21 + e); P.AP[e] = PST(24 + e); P.VP[e] = PST(27 + e); P.PP[e] = PST(30 + e); }
-#endif
-#pragma unroll
-        for (int e = 0; e < 3; e++) { oTP[e] = (T)P.TP[e]; oGP[e] = (T)P.GP[e]; oAP[e] = (T)P.AP[e]; oVP[e] = (T)P.VP[e]; }
-#pragma unroll
-        for (int e = 0; e < 3; e++) { xTP[e] = oTP[e]; xGP[e] = oGP[e]; xAP[e] = oAP[e]; xVP[e] = oVP[e]; }
-#pragma unroll
-        for (int s = 0; s < 4; s++) {
-            const T* Rs = (s == 0) ? R : (s == 3 ? R1 : Rm);
-            T tv[3], gv[3], av[3], vv[3];
-#pragma unroll
-            for (int e = 0; e < 3; e++) { tv[e] = SLT(s * NS + e); gv[e] = SLT(s * NS + 3 + e); av[e] = SLT(s * NS + 6 + e); vv[e] = SLT(s * NS + 9 + e); }
-            T kTP[3], kVP[3], kPP[3];
-            // TP:  -W TP - GP + TV
-            cross(xTP, w, kTP);
-#pragma unroll
-            for (int e = 0; e < 3; e++) kTP[e] = (kTP[e] - xGP[e]) + tv[e];
-            // VP:  A_s TP_0 + B_s AP_0 + VV_0
-            {
-                T u[3], m0[3];
-                cross(ah, xTP, u);
-#pragma unroll
-                for (int e = 0; e < 3; e++) u[e] += xAP[e];
-                if (MODEL == 2) {                             // + C_s CP_0,  CP_s = TP(start) + CN(s-1) CV_{s-1}
-                    T cp[3], u2[3];
-#pragma unroll
-                    for (int e = 0; e < 3; e++) cp[e] = (s == 0) ? oTP[e] : fma((T)SLT((s - 1) * NS + SL_CV + e), CN(s - 1), oTP[e]);
-                    cross(gt, cp, u2);
-#pragma unroll
-                    for (int e = 0; e < 3; e++) u[e] += u2[e];
-                }
-                (void)m0;
-#pragma unroll
-                for (int e = 0; e < 3; e++) kVP[e] = fma(-Rs[6 + e], u[2], fma(-Rs[3 + e], u[1], fma(-Rs[e], u[0], vv[e])));   // VV_0 - (column e of R_s) . u
-            }
-            // PP:  VP + VP^T
-            kPP[0] = xVP[0] + xVP[0]; kPP[1] = xVP[1] + shf(xVP[2], nx); kPP[2] = xVP[2] + shf(xVP[1], pv);
-#pragma unroll
-            for (int e = 0; e < 3; e++) {
-                sTP[e] = KSUM(sTP[e], kTP[e], s); sGP[e] = KSUM(sGP[e], gv[e], s); sAP[e] = KSUM(sAP[e], av[e], s);
-                sVP[e] = KSUM(sVP[e], kVP[e], s); sPP[e] = KSUM(sPP[e], kPP[e], s);
-                if (s < 3) {
-                    xTP[e] = fma(kTP[e], CN(s), oTP[e]); xGP[e] = fma(gv[e], CN(s), oGP[e]); xAP[e] = fma(av[e], CN(s), oAP[e]);
-                    xVP[e] = fma(kVP[e], CN(s), oVP[e]);
-                }
-            }
-        }
-#pragma unroll
-        for (int e = 0; e < 3; e++) {
-            P.TP[e] = fma((double)dt6, (double)sTP[e], P.TP[e]); P.GP[e] = fma((double)dt6, (double)sGP[e], P.GP[e]);
-            P.AP[e] = fma((double)dt6, (double)sAP[e], P.AP[e]); P.VP[e] = fma((double)dt6, (double)sVP[e], P.VP[e]);
-            P.PP[e] = fma((double)dt6, (double)sPP[e], P.PP[e]);
-        }
-#ifdef CPI_TRI_PSMEM
-#pragma unroll
-        for (int e = 0; e < 3; e++) { PST(18 + e) = P.TP[e]; PST(21 + e) = P.GP[e]; PST(24 + e) = P.AP[e]; PST(27 + e) = P.VP[e]; PST(30 + e) = P.PP[e]; }
-#endif
-    }
-    CPI_FENCE();
-}
-
-#endif
 // D v  with  D = I - a [w x] + b [w x]^2 :   v - a (w x v) + b (w x (w x v));  second result with (a2, b2) on the same cross products
 CPI_DEV void rot_col2(double a, double b, double a2, double b2, const double* w, const double* v, double* o, double* o2) {
     double t[3], u[3];
@@ -479,11 +321,7 @@ constexpr bool kLoadOnly = false, kCovOnly = false;
 enum : int { SC_A1 = 0, SC_B1, SC_A2, SC_B2, SC_F1, SC_F2, SC_F3, SC_F4, SC_DT6, SC_D1, SC_D2, SC_D3, SC_D4, SC_CA, SC_CB, SC_N };
 
 template <int MODEL, class T>
-#ifdef CPI_TRI_MAXNREG          // experiment switch: cap the registers per thread instead of taking all 255
-__global__ void __maxnreg__(CPI_TRI_MAXNREG) k_preintegrate_tri(const PreintParams p) {
-#else
 __global__ void __launch_bounds__((TriNT<MODEL, T>::NT), 1) k_preintegrate_tri(const PreintParams p) {
-#endif
     using SM_ = TriSmem<MODEL, T>;
     constexpr int NT = SM_::NT;
     constexpr int CH = 8 / (int)sizeof(T) * 2;            // samples per TMA chunk: 2 (fp64) or 4 (fp32) = 112 B in one aligned 128-B fetch
@@ -501,13 +339,7 @@ __global__ void __launch_bounds__((TriNT<MODEL, T>::NT), 1) k_preintegrate_tri(c
     if (wid * TRI_WPW >= p.wpb || (int64_t)blockIdx.x * p.wpb + wid * TRI_WPW >= p.n_windows) return;   // whole warp idle (warp-uniform)
 
     T* sl = reinterpret_cast<T*>(smem_raw) + threadIdx.x;
-#ifdef CPI_TRI_PSMEM
-    double* ps = reinterpret_cast<double*>(smem_raw + SM_::off_fs) + threadIdx.x;
-    double fsr[TriL<MODEL>::NFS];
-#else
     double* fs = reinterpret_cast<double*>(smem_raw + SM_::off_fs) + threadIdx.x;
-    double* ps = nullptr;
-#endif
     // per-window scalar sets of the current 3 samples (the two idle lanes of a warp get a dummy slot of their own)
     double* sc = reinterpret_cast<double*>(smem_raw + SM_::off_sc) + (size_t)(lane_ok ? wslot : SM_::WPB + wid) * TriSC<MODEL>::STRIDE;
     const T* buf = reinterpret_cast<const T*>(smem_raw + SM_::off_buf + (size_t)wslot * TRI_BUF_STRIDE);
@@ -582,10 +414,6 @@ __global__ void __launch_bounds__((TriNT<MODEL, T>::NT), 1) k_preintegrate_tri(c
     TriP<T> P;
 #pragma unroll
     for (int e = 0; e < 3; e++) P.TG[e] = P.TT[e] = P.GV[e] = P.TV[e] = P.AV[e] = P.VV[e] = P.TP[e] = P.GP[e] = P.AP[e] = P.VP[e] = P.PP[e] = 0.0;
-#ifdef CPI_TRI_PSMEM
-#pragma unroll
-    for (int e = 0; e < 33; e++) PST(e) = 0.0;
-#endif
 
     // ---- continuation: resume from the state a previous call left in a record (the batched form of calling feed_IMU again on an existing
     // CpiV1 / CpiV2 object, CpiBase.h:86 -- every field of the object is in the record; model 2's clone rows are re-initialised at every
@@ -613,11 +441,7 @@ __global__ void __launch_bounds__((TriNT<MODEL, T>::NT), 1) k_preintegrate_tri(c
             }
             auto blk = [&](int I, int J) { return (double)Pm[(3 * I + r) + 15 * (3 * J + c)]; };
             P.TT[k] = blk(0, 0); P.VV[k] = blk(2, 2);
-#ifndef CPI_TRI_UNFUSED12
             P.PP[k] = 0.5 * blk(4, 4);                           // PP is carried as Q with PP = Q + Q^T: the symmetric half is a valid Q
-#else
-            P.PP[k] = blk(4, 4);
-#endif
             P.TG[k] = blk(0, 1); P.GV[k] = blk(1, 2); P.TV[k] = blk(0, 2); P.AV[k] = blk(3, 2);
             P.TP[k] = blk(0, 4); P.GP[k] = blk(1, 4); P.AP[k] = blk(3, 4); P.VP[k] = blk(2, 4);
         }
@@ -876,7 +700,7 @@ __global__ void __launch_bounds__((TriNT<MODEL, T>::NT), 1) k_preintegrate_tri(c
                 for (int e = 0; e < 3; e++) { w_[e] = (T)wh[e]; a_[e] = (T)ah[e]; g_[e] = (T)g_tau[e]; }
 #pragma unroll
                 for (int e = 0; e < 9; e++) { R_[e] = (T)R[e]; Rm_[e] = (T)Rm[e]; R1_[e] = (T)R1[e]; }
-                tri_cov_step<MODEL, NT, T>(P, sl, ps, w_, a_, g_, R_, Rm_, R1_, (T)pgg, (T)paa, (T)dt, (T)dt6, (T)p.q_w, (T)p.q_wb, (T)p.q_a, (T)p.q_ab, nx, pv);
+                tri_cov_step<MODEL, NT, T>(P, sl, w_, a_, g_, R_, Rm_, R1_, (T)pgg, (T)paa, (T)dt, (T)dt6, (T)p.q_w, (T)p.q_wb, (T)p.q_a, (T)p.q_ab, nx, pv);
                 pgg += dt6 * (p.q_wb + 2.0 * p.q_wb + 2.0 * p.q_wb + p.q_wb);
                 paa += dt6 * (p.q_ab + 2.0 * p.q_ab + 2.0 * p.q_ab + p.q_ab);
             }
@@ -900,21 +724,10 @@ __global__ void __launch_bounds__((TriNT<MODEL, T>::NT), 1) k_preintegrate_tri(c
     // ---- write the record (column-major 3x3 / 15x15, include/cpi_b200.h).  Lane c writes original column c (rows c, c+1, c+2).
     // symmetric diagonal blocks: average the two independently rounded copies of each off-diagonal entry (the reference
     // symmetrises every step, CpiV1.h:353)
-#ifdef CPI_TRI_PSMEM
-#pragma unroll
-    for (int e = 0; e < 3; e++) {
-        P.TG[e] = PST(e); P.TT[e] = PST(3 + e); P.GV[e] = PST(6 + e); P.TV[e] = PST(9 + e); P.AV[e] = PST(12 + e); P.VV[e] = PST(15 + e);
-        P.TP[e] = PST(18 + e); P.GP[e] = PST(21 + e); P.AP[e] = PST(24 + e); P.VP[e] = PST(27 + e); P.PP[e] = PST(30 + e);
-    }
-#endif
     double sTT[3], sVV[3], sPP[3];
     sTT[0] = P.TT[0]; sTT[1] = 0.5 * (P.TT[1] + shf(P.TT[2], nx)); sTT[2] = 0.5 * (P.TT[2] + shf(P.TT[1], pv));
     sVV[0] = P.VV[0]; sVV[1] = 0.5 * (P.VV[1] + shf(P.VV[2], nx)); sVV[2] = 0.5 * (P.VV[2] + shf(P.VV[1], pv));
-#ifndef CPI_TRI_UNFUSED12
     sPP[0] = P.PP[0] + P.PP[0]; sPP[1] = P.PP[1] + shf(P.PP[2], nx); sPP[2] = P.PP[2] + shf(P.PP[1], pv);     // PP = Q + Q^T (exactly symmetric: a + b == b + a)
-#else
-    sPP[0] = P.PP[0]; sPP[1] = 0.5 * (P.PP[1] + shf(P.PP[2], nx)); sPP[2] = 0.5 * (P.PP[2] + shf(P.PP[1], pv));
-#endif
     if (!active) return;
     constexpr int RD = (MODEL == 1) ? CPI_REC_V1_DOUBLES : CPI_REC_V2_DOUBLES;
     T* rec = reinterpret_cast<T*>(p.out) + win * (int64_t)RD;
@@ -955,7 +768,6 @@ __global__ void __launch_bounds__((TriNT<MODEL, T>::NT), 1) k_preintegrate_tri(c
 
 #undef SLT
 #undef FST
-#undef PST
 #undef CN
 #undef KSUM
 

@@ -46,6 +46,8 @@ def test_argument_validation_without_gpu():
     rc = lib.cpi_preintegrate_batch(1, 64, -5, None, 1, None, None, None, 0, None, None)
     assert rc == -1
     assert lib.cpi_preintegrate_batch(1, 64, 0, None, 1, None, None, None, 0, None, None) == 0      # empty batch is a no-op
+    rc = lib.cpi_preintegrate_batch(1, 64, 2**31 - 1, None, 1, None, None, None, 0, None, None)
+    assert rc == -1 and b"too many windows" in lib.cpi_last_error()
     import numpy as np
     bad = np.array([0, 5, 3, 9], dtype=np.int64); buf = np.zeros(64)
     P = lambda a: ctypes.c_void_p(a.ctypes.data)
