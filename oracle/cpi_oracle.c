@@ -818,6 +818,401 @@ int oracle_scan_records(int64_t n_groups, const int64_t* offsets, int64_t unifor
     return group_job(3, n_groups, offsets, uniform, records, lin, out, nthreads);
 }
 
+/* ------------------------------------------------------------------ the solver side of a chain (DESIGN.md 3e, 3f) -- */
+/* Not reference routines: dense, literal statements of the chain marginalisation (K8), the prior move (k_prior_at), the SPD
+ * block-tridiagonal solve and the LM model decrease, so that they check the kernels' lane algebra instead of repeating it.
+ * 15x15 blocks are column-major [225] as in include/cpi_b200.h; symmetric inputs are read from their lower triangle, as the kernels
+ * read them.  The chain layouts are those of the C ABI: CSR state offsets, or chains of `uniform` states when offsets is NULL;
+ * chain c's factors are stored back to back from index offsets[c] - c. */
+enum { B15 = 225 };
+
+static void sym_lower(real* dst, const double* src) {
+    for (int j = 0; j < 15; j++) for (int i = j; i < 15; i++) E(dst, 15, i, j) = E(dst, 15, j, i) = src[i + 15 * j];
+}
+
+/* A = L L^T in place (L lower, the upper triangle zeroed).  Returns 0 at the first pivot that is not positive. */
+static int chol15(real* A) {
+    for (int j = 0; j < 15; j++) {
+        real d = E(A, 15, j, j);
+        for (int k = 0; k < j; k++) d -= E(A, 15, j, k) * E(A, 15, j, k);
+        if (!(d > 0)) return 0;
+        d = sqrt(d);
+        E(A, 15, j, j) = d;
+        for (int i = j + 1; i < 15; i++) {
+            real s = E(A, 15, i, j);
+            for (int k = 0; k < j; k++) s -= E(A, 15, i, k) * E(A, 15, j, k);
+            E(A, 15, i, j) = s / d;
+        }
+        for (int i = 0; i < j; i++) E(A, 15, i, j) = 0;
+    }
+    return 1;
+}
+/* B (15 x n) <- L^-1 B */
+static void fwd_n(const real* L, real* B, int n) {
+    for (int c = 0; c < n; c++) for (int i = 0; i < 15; i++) {
+        real s = E(B, 15, i, c);
+        for (int k = 0; k < i; k++) s -= E(L, 15, i, k) * E(B, 15, k, c);
+        E(B, 15, i, c) = s / E(L, 15, i, i);
+    }
+}
+/* v <- L^-T v */
+static void bwd_1(const real* L, real* v) {
+    for (int i = 14; i >= 0; i--) {
+        real s = v[i];
+        for (int k = i + 1; k < 15; k++) s -= E(L, 15, k, i) * v[k];
+        v[i] = s / E(L, 15, i, i);
+    }
+}
+/* v <- L^-T v column by column, as warp_bwd15 (chol15.cuh): x_i = v_i / L_ii, then v_j -= L_ij x_i for j < i */
+static void bwd_col(const real* L, real* v) {
+    for (int i = 14; i >= 0; i--) {
+        v[i] = v[i] / E(L, 15, i, i);
+        for (int j = 0; j < i; j++) v[j] -= E(L, 15, i, j) * v[i];
+    }
+}
+static void fill_nan(double* p, int64_t n) { for (int64_t i = 0; i < n; i++) p[i] = NAN; }
+
+/* K8 for one chain: states lo .. hi-1, factors from fo.  Lam, eta, f start at the prior (0 without one); for k < m:
+ *   M = Lam + G11_k = L L^T,  [Z z] = L^-1 [G12_k  eta + g1_k],  Lam <- G22_k - Z^T Z,  eta <- g2_k - Z^T z,  f <- f + f_k - z^T z.
+ * m out of [0, hi - lo) or a pivot that is not positive: NaN.  m = 0: the prior's bits.  sc (may be NULL) [242]: the size of the
+ * terms that cancel into the result, |G22| + |Z|^T |Z| and |g2| + |Z|^T |z| of the last step, |f_prior| + sum |f_k| + sum z^T z, and the
+ * last step's z^T z. */
+static void marg_chain(int64_t c, int64_t lo, int64_t hi, int64_t m, const double* G11, const double* G12, const double* G22, const double* g1,
+                       const double* g2, const double* fk, const double* pi, const double* pr, const double* pf, double* oi, double* orr,
+                       double* of, double* sc) {
+    if (!(m >= 0 && m < hi - lo)) {
+        fill_nan(oi, B15); fill_nan(orr, 15); fill_nan(of, 1); if (sc) fill_nan(sc, 242);
+        return;
+    }
+    if (m == 0) {
+        for (int t = 0; t < B15; t++) oi[t] = pi ? pi[c * B15 + t] : 0.0;
+        for (int t = 0; t < 15; t++) orr[t] = pr ? pr[c * 15 + t] : 0.0;
+        *of = pf ? pf[c] : 0.0;
+        if (sc) { for (int t = 0; t < B15; t++) sc[t] = fabs(oi[t]); for (int t = 0; t < 15; t++) sc[B15 + t] = fabs(orr[t]); sc[240] = fabs(*of); sc[241] = 0; }
+        return;
+    }
+    real Lam[B15], eta[15], F, M[B15], Z[15 * 16], A[B15], fs;
+    if (pi) sym_lower(Lam, pi + c * B15); else mat_zero(Lam, B15);
+    for (int t = 0; t < 15; t++) eta[t] = pr ? pr[c * 15 + t] : 0.0;
+    F = pf ? pf[c] : 0.0;
+    fs = fabs(F);
+    const int64_t f0 = lo - c;
+    for (int64_t k = 0; k < m; k++) {
+        const int64_t fi = f0 + k;
+        sym_lower(A, G11 + fi * B15);
+        for (int t = 0; t < B15; t++) M[t] = Lam[t] + A[t];
+        if (!chol15(M)) {
+            fill_nan(oi, B15); fill_nan(orr, 15); fill_nan(of, 1); if (sc) fill_nan(sc, 242);
+            return;
+        }
+        load(Z, G12 + fi * B15, B15);
+        for (int r = 0; r < 15; r++) Z[B15 + r] = eta[r] + g1[fi * 15 + r];
+        fwd_n(M, Z, 16);
+        sym_lower(A, G22 + fi * B15);
+        real zz = 0;
+        for (int q = 0; q < 15; q++) zz += Z[B15 + q] * Z[B15 + q];
+        for (int j = 0; j < 15; j++) {
+            for (int i = 0; i < 15; i++) {
+                real s = 0;
+                for (int q = 0; q < 15; q++) s += E(Z, 15, q, i) * E(Z, 15, q, j);
+                E(Lam, 15, i, j) = E(A, 15, i, j) - s;
+            }
+            real s = 0;
+            for (int q = 0; q < 15; q++) s += E(Z, 15, q, j) * Z[B15 + q];
+            eta[j] = (real)g2[fi * 15 + j] - s;
+        }
+        F = F + (real)fk[fi] - zz;
+        fs += fabs((real)fk[fi]) + zz;
+        if (sc && k == m - 1) {
+            for (int j = 0; j < 15; j++) {
+                for (int i = 0; i < 15; i++) {
+                    real s = fabs(E(A, 15, i, j));
+                    for (int q = 0; q < 15; q++) s += fabs(E(Z, 15, q, i)) * fabs(E(Z, 15, q, j));
+                    sc[i + 15 * j] = (double)s;
+                }
+                real s = fabs((real)g2[fi * 15 + j]);
+                for (int q = 0; q < 15; q++) s += fabs(E(Z, 15, q, j)) * fabs(Z[B15 + q]);
+                sc[B15 + j] = (double)s;
+            }
+            sc[241] = (double)zz;
+        }
+    }
+    store(oi, Lam, B15); store(orr, eta, 15); *of = (double)F;
+    if (sc) sc[240] = (double)fs;
+}
+
+/* The sequential block Cholesky of one chain's rows lo .. hi-1 of A = tridiag(E^T, D, E), x_lo -> x_{hi-1}, then back:
+ *   M_k = D_k - U_{k-1}^T U_{k-1} = L_k L_k^T,  U_k = L_k^-1 E_k,  y_k = L_k^-1 (b_k - U_{k-1}^T y_{k-1});  x_k = L_k^-T (y_k - U_k x_{k+1}).
+ * A pivot that is not positive: NaN for the chain. */
+static void seq_chain(int64_t lo, int64_t hi, const double* D, const double* Eb, const double* b, double* x) {
+    const int64_t n = hi - lo;
+    real* L = (real*)malloc((size_t)n * 2 * B15 * sizeof(real));
+    real* U = L + n * B15;
+    real* y = (real*)malloc((size_t)n * 15 * sizeof(real));
+    int ok = 1;
+    for (int64_t k = 0; k < n && ok; k++) {
+        real* Lk = L + k * B15;
+        sym_lower(Lk, D + (lo + k) * B15);
+        for (int r = 0; r < 15; r++) y[k * 15 + r] = b[(lo + k) * 15 + r];
+        if (k > 0) {
+            const real* Up = U + (k - 1) * B15;
+            for (int j = 0; j < 15; j++) {
+                for (int i = 0; i < 15; i++) {
+                    real s = 0;
+                    for (int q = 0; q < 15; q++) s += E(Up, 15, q, i) * E(Up, 15, q, j);
+                    E(Lk, 15, i, j) -= s;
+                }
+                real s = 0;
+                for (int q = 0; q < 15; q++) s += E(Up, 15, q, j) * y[(k - 1) * 15 + q];
+                y[k * 15 + j] -= s;
+            }
+        }
+        ok = chol15(Lk);
+        if (!ok) break;
+        fwd_n(Lk, y + k * 15, 1);
+        if (k + 1 < n) { load(U + k * B15, Eb + (lo + k) * B15, B15); fwd_n(Lk, U + k * B15, 15); }
+    }
+    if (!ok) {
+        fill_nan(x + lo * 15, n * 15);
+    } else {
+        for (int64_t k = n - 1; k >= 0; k--) {
+            real v[15];
+            for (int r = 0; r < 15; r++) v[r] = y[k * 15 + r];
+            if (k + 1 < n) {
+                const real* Uk = U + k * B15;
+                for (int r = 0; r < 15; r++) { real s = 0; for (int q = 0; q < 15; q++) s += E(Uk, 15, r, q) * y[(k + 1) * 15 + q]; v[r] -= s; }
+            }
+            bwd_1(L + k * B15, v);
+            for (int r = 0; r < 15; r++) y[k * 15 + r] = v[r];        /* y now holds x_k */
+        }
+        store(x + lo * 15, y, n * 15);
+    }
+    free(L); free(y);
+}
+
+/* The block cyclic reduction of the whole system (rows 0 .. m-1, couplings as given), level by level in the order of solve.cu:
+ * odd node i: D_i = Lc Lc^T, Za = Lc^-1 E_{i-1}^T, Zb = Lc^-1 E_i (0 for the last node), zb = Lc^-1 b_i; even node j -> node j/2 of the
+ * next level: D' = D_j - Zb_{j-1}^T Zb_{j-1} - Za_{j+1}^T Za_{j+1}, b' = b_j - Zb_{j-1}^T zb_{j-1} - Za_{j+1}^T zb_{j+1},
+ * E' = -Za_{j+1}^T Zb_{j+1}; one node: x = D^-1 b; back: Lc^T x_i = zb - Za x_{i-1} - Zb x_{i+1}.  Blocks held full (D symmetric);
+ * products are subtracted one at a time in the kernels' order, and L^-T runs column by column as warp_bwd15 does. */
+static void bcr_level(int64_t m, const real* D, const real* Eb, const real* b, real* x) {
+    if (m == 1) {
+        real L[B15], v[15];
+        memcpy(L, D, sizeof L);
+        if (!chol15(L)) { for (int r = 0; r < 15; r++) x[r] = NAN; return; }
+        memcpy(v, b, sizeof v);
+        fwd_n(L, v, 1); bwd_col(L, v);
+        memcpy(x, v, sizeof v);
+        return;
+    }
+    const int64_t odd = m / 2, even = (m + 1) / 2;
+    real* Lc = (real*)malloc((size_t)(odd * (3 * B15 + 15) + even * (2 * B15 + 30)) * sizeof(real));
+    real *Za = Lc + odd * B15, *Zb = Za + odd * B15, *zb = Zb + odd * B15;
+    real *Dn = zb + odd * 15, *En = Dn + even * B15, *bn = En + even * B15, *xn = bn + even * 15;
+    for (int64_t t = 0; t < odd; t++) {
+        const int64_t i = 2 * t + 1;
+        real* L = Lc + t * B15;
+        memcpy(L, D + i * B15, B15 * sizeof(real));
+        int ok = chol15(L);
+        transpose(15, 15, Eb + (i - 1) * B15, Za + t * B15);
+        if (i + 1 < m) memcpy(Zb + t * B15, Eb + i * B15, B15 * sizeof(real)); else mat_zero(Zb + t * B15, B15);
+        memcpy(zb + t * 15, b + i * 15, 15 * sizeof(real));
+        if (!ok) for (int e = 0; e < B15; e++) L[e] = NAN;
+        fwd_n(L, Za + t * B15, 15); fwd_n(L, Zb + t * B15, 15); fwd_n(L, zb + t * 15, 1);
+    }
+    for (int64_t u = 0; u < even; u++) {
+        const int64_t j = 2 * u;
+        real *Dj = Dn + u * B15, *bj = bn + u * 15, *Ej = En + u * B15;
+        memcpy(Dj, D + j * B15, B15 * sizeof(real));
+        memcpy(bj, b + j * 15, 15 * sizeof(real));
+        mat_zero(Ej, B15);
+        const real *ZbL = j >= 1 ? Zb + ((j - 2) / 2) * B15 : 0, *zbL = j >= 1 ? zb + ((j - 2) / 2) * 15 : 0;
+        const real *ZaR = j + 1 < m ? Za + (j / 2) * B15 : 0, *ZbR = j + 1 < m ? Zb + (j / 2) * B15 : 0, *zbR = j + 1 < m ? zb + (j / 2) * 15 : 0;
+        for (int c2 = 0; c2 < 15; c2++) {                       /* the products subtracted one by one, interleaved, as k_bcr_reduce */
+            for (int r = 0; r < 15; r++) {
+                real d = E(Dj, 15, r, c2), e = 0;
+                for (int q = 0; q < 15; q++) {
+                    if (ZbL) d -= E(ZbL, 15, q, r) * E(ZbL, 15, q, c2);
+                    if (ZaR) d -= E(ZaR, 15, q, r) * E(ZaR, 15, q, c2);
+                    if (ZaR && j + 2 < m) e -= E(ZaR, 15, q, r) * E(ZbR, 15, q, c2);
+                }
+                E(Dj, 15, r, c2) = d;
+                E(Ej, 15, r, c2) = e;
+            }
+            real v = bj[c2];
+            for (int q = 0; q < 15; q++) {
+                if (ZbL) v -= E(ZbL, 15, q, c2) * zbL[q];
+                if (ZaR) v -= E(ZaR, 15, q, c2) * zbR[q];
+            }
+            bj[c2] = v;
+        }
+    }
+    bcr_level(even, Dn, En, bn, xn);
+    for (int64_t u = 0; u < even; u++) memcpy(x + 2 * u * 15, xn + u * 15, 15 * sizeof(real));
+    for (int64_t t = 0; t < odd; t++) {
+        const int64_t i = 2 * t + 1;
+        real v[15];
+        for (int r = 0; r < 15; r++) {
+            real s = zb[t * 15 + r];
+            for (int q = 0; q < 15; q++) {
+                s -= E(Za + t * B15, 15, r, q) * x[(i - 1) * 15 + q];
+                if (i + 1 < m) s -= E(Zb + t * B15, 15, r, q) * x[(i + 1) * 15 + q];
+            }
+            v[r] = s;
+        }
+        bwd_col(Lc + t * B15, v);
+        memcpy(x + i * 15, v, sizeof v);
+    }
+    free(Lc);
+}
+
+/* the LM model decrease of one chain (k_lm_terms + k_lm_decide's sums): out[5] = (m, the size of its terms, cur, new, moved)
+ *   m = sum_k delta_k^T (2 rhs_k - (H delta)_k),  H = tridiag(E^T, D - diag(damp), E) of the chain,  size = sum_k |delta_k|^T (2 |rhs_k| + |H| |delta|),
+ *   cur / new = the chain's factor costs + the prior's, moved = 1 if any delta != 0. */
+static void lm_chain(int64_t c, int64_t lo, int64_t hi, const double* rhs, const double* D, const double* Eb, const double* damp, const double* delta,
+                     const double* f_cur, const double* pf_cur, const double* f_new, const double* pf_new, double* out) {
+    real m = 0, sz = 0, cur = pf_cur ? pf_cur[c] : 0.0, nw = pf_new ? pf_new[c] : 0.0;
+    int moved = 0;
+    for (int64_t k = lo; k < hi; k++) {
+        for (int r = 0; r < 15; r++) {
+            real hd = 0, ha = 0;
+            for (int q = 0; q < 15; q++) {
+                real h = D[k * B15 + r + 15 * q] - (q == r ? (real)damp[k * 15 + r] : 0);
+                hd += h * delta[k * 15 + q]; ha += fabs(h) * fabs((real)delta[k * 15 + q]);
+                if (k > lo) { real e = Eb[(k - 1) * B15 + q + 15 * r]; hd += e * delta[(k - 1) * 15 + q]; ha += fabs(e) * fabs((real)delta[(k - 1) * 15 + q]); }
+                if (k + 1 < hi) { real e = Eb[k * B15 + r + 15 * q]; hd += e * delta[(k + 1) * 15 + q]; ha += fabs(e) * fabs((real)delta[(k + 1) * 15 + q]); }
+            }
+            const real d = delta[k * 15 + r];
+            m += d * (2 * (real)rhs[k * 15 + r] - hd);
+            sz += fabs(d) * (2 * fabs((real)rhs[k * 15 + r]) + ha);
+            moved |= delta[k * 15 + r] != 0.0;
+        }
+        if (k + 1 < hi) { cur += f_cur[k - c]; nw += f_new[k - c]; }
+    }
+    out[0] = (double)m; out[1] = (double)sz; out[2] = (double)cur; out[3] = (double)nw; out[4] = moved;
+}
+
+typedef struct {
+    int kind, t, nt; int64_t n;                  /* kind 0: marginalise, 1: sequential solve, 2: LM terms */
+    const int64_t *offsets, *n_marg; int64_t uniform, marg_uniform;
+    const double *G11, *G12, *G22, *g1, *g2, *f, *pi, *pr, *pf;
+    const double *D, *E, *b, *damp, *delta, *f_cur, *pf_cur, *f_new, *pf_new;
+    double *oi, *orr, *of, *sc, *x;
+} cjob_t;
+
+static void* cworker(void* arg) {
+    cjob_t* j = (cjob_t*)arg;
+    for (int64_t c = j->t; c < j->n; c += j->nt) {             /* interleaved: chain lengths vary by orders of magnitude */
+        const int64_t lo = j->offsets ? j->offsets[c] : c * j->uniform, hi = j->offsets ? j->offsets[c + 1] : lo + j->uniform;
+        if (j->kind == 0)
+            marg_chain(c, lo, hi, j->n_marg ? j->n_marg[c] : j->marg_uniform, j->G11, j->G12, j->G22, j->g1, j->g2, j->f, j->pi, j->pr, j->pf,
+                       j->oi + c * B15, j->orr + c * 15, j->of + c, j->sc ? j->sc + c * 242 : 0);
+        else if (j->kind == 1)
+            seq_chain(lo, hi, j->D, j->E, j->b, j->x);
+        else
+            lm_chain(c, lo, hi, j->b, j->D, j->E, j->damp, j->delta, j->f_cur, j->pf_cur, j->f_new, j->pf_new, j->x + c * 5);
+    }
+    return 0;
+}
+
+static void crun(cjob_t* proto, int nthreads) {
+    if (nthreads < 1) nthreads = 1;
+    if (nthreads > 256) nthreads = 256;
+    cjob_t jobs[256]; pthread_t th[256];
+    for (int t = 0; t < nthreads; t++) { jobs[t] = *proto; jobs[t].t = t; jobs[t].nt = nthreads; }
+    if (nthreads == 1) { cworker(&jobs[0]); return; }
+    for (int t = 0; t < nthreads; t++) pthread_create(&th[t], 0, cworker, &jobs[t]);
+    for (int t = 0; t < nthreads; t++) pthread_join(th[t], 0);
+}
+
+int oracle_chain_marginalize(int64_t n_chains, const int64_t* offsets, int64_t uniform, const int64_t* n_marg, int64_t marg_uniform,
+                             const double* G11, const double* G12, const double* G22, const double* g1, const double* g2, const double* f,
+                             const double* prior_info, const double* prior_rhs, const double* prior_f, double* out_info, double* out_rhs,
+                             double* out_f, double* scale, int nthreads) {
+    if (n_chains < 0 || (!offsets && uniform < 1)) return -1;
+    cjob_t j; memset(&j, 0, sizeof j);
+    j.kind = 0; j.n = n_chains; j.offsets = offsets; j.uniform = uniform; j.n_marg = n_marg; j.marg_uniform = marg_uniform;
+    j.G11 = G11; j.G12 = G12; j.G22 = G22; j.g1 = g1; j.g2 = g2; j.f = f; j.pi = prior_info; j.pr = prior_rhs; j.pf = prior_f;
+    j.oi = out_info; j.orr = out_rhs; j.of = out_f; j.sc = scale;
+    crun(&j, nthreads);
+    return 0;
+}
+
+int oracle_chain_solve(int64_t n_chains, const int64_t* offsets, int64_t uniform, const double* D, const double* E, const double* b, double* x,
+                       int order, int nthreads) {
+    if (n_chains < 0 || (!offsets && uniform < 1) || (order != 0 && order != 1)) return -1;
+    const int64_t n = offsets ? offsets[n_chains] : n_chains * uniform;
+    if (n == 0) return 0;
+    if (order == 0) {
+        cjob_t j; memset(&j, 0, sizeof j);
+        j.kind = 1; j.n = n_chains; j.offsets = offsets; j.uniform = uniform; j.D = D; j.E = E; j.b = b; j.x = x;
+        crun(&j, nthreads);
+        return 0;
+    }
+    real* Dl = (real*)malloc((size_t)n * (2 * B15 + 30) * sizeof(real));
+    real *El = Dl + n * B15, *bl = El + n * B15, *xl = bl + n * 15;
+    for (int64_t k = 0; k < n; k++) {
+        sym_lower(Dl + k * B15, D + k * B15);
+        if (k + 1 < n) load(El + k * B15, E + k * B15, B15); else mat_zero(El + k * B15, B15);
+        load(bl + k * 15, b + k * 15, 15);
+    }
+    bcr_level(n, Dl, El, bl, xl);
+    store(x, xl, n * 15);
+    free(Dl);
+    return 0;
+}
+
+int oracle_lm_terms(int64_t n_chains, const int64_t* offsets, int64_t uniform, const double* rhs, const double* D, const double* E,
+                    const double* damp, const double* delta, const double* f_cur, const double* pf_cur, const double* f_new,
+                    const double* pf_new, double* out, int nthreads) {
+    if (n_chains < 0 || (!offsets && uniform < 1)) return -1;
+    cjob_t j; memset(&j, 0, sizeof j);
+    j.kind = 2; j.n = n_chains; j.offsets = offsets; j.uniform = uniform; j.b = rhs; j.D = D; j.E = E; j.damp = damp; j.delta = delta;
+    j.f_cur = f_cur; j.pf_cur = pf_cur; j.f_new = f_new; j.pf_new = pf_new; j.x = out;
+    crun(&j, nthreads);
+    return 0;
+}
+
+/* local(x_lin, x): the delta with x = retract(x_lin, delta): the rotation vector of dq = q_x (x) q_lin^-1 (quat_multiply: w >= 0,
+ * normalised), 2 atan2(|v|, w) v / |v|, exactly 0 when the two quaternions have the same bits and 2 v where |v| = 0; the other 12
+ * entries are differences.  The `same` test is on the double inputs, so both builds take the same branch. */
+static void local_state(const double* xl_in, const double* x_in, real* d) {
+    real xl[CPI_STATE_DOUBLES], x[CPI_STATE_DOUBLES], qi[4], dq[4];
+    load(xl, xl_in, CPI_STATE_DOUBLES); load(x, x_in, CPI_STATE_DOUBLES);
+    quat_inv(xl, qi);
+    quat_multiply(x, qi, dq);
+    const real s = norm3(dq);
+    const int same = x_in[0] == xl_in[0] && x_in[1] == xl_in[1] && x_in[2] == xl_in[2] && x_in[3] == xl_in[3];
+    const real k = same ? 0 : (s > 0 ? 2 * atan2(s, dq[3]) / s : 2);
+    for (int j = 0; j < 3; j++) d[j] = k * dq[j];
+    for (int j = 0; j < 12; j++) d[3 + j] = x[4 + j] - xl[4 + j];
+}
+
+int oracle_local(int64_t n, const double* lin, const double* x, double* delta) {
+    for (int64_t i = 0; i < n; i++) {
+        real d[15];
+        local_state(lin + i * CPI_STATE_DOUBLES, x + i * CPI_STATE_DOUBLES, d);
+        store(delta + i * 15, d, 15);
+    }
+    return 0;
+}
+
+/* k_prior_at: delta = local(lin, x), rhs' = rhs - info delta, f' = f - 2 rhs^T delta + delta^T info delta (info read in full) */
+int oracle_prior_at(int64_t n, const double* info, const double* rhs, const double* f, const double* lin, const double* x, double* rhs_out,
+                    double* f_out) {
+    for (int64_t i = 0; i < n; i++) {
+        real d[15], u[15], fo = f ? f[i] : 0.0;
+        local_state(lin + i * CPI_STATE_DOUBLES, x + i * CPI_STATE_DOUBLES, d);
+        for (int r = 0; r < 15; r++) { real s = 0; for (int q = 0; q < 15; q++) s += info[i * B15 + r + 15 * q] * d[q]; u[r] = s; }
+        for (int r = 0; r < 15; r++) {
+            fo += d[r] * (u[r] - 2 * (real)rhs[i * 15 + r]);
+            rhs_out[i * 15 + r] = (double)((real)rhs[i * 15 + r] - u[r]);
+        }
+        if (f_out) f_out[i] = (double)fo;
+    }
+    return 0;
+}
+
 /* ------------------------------------------------------------------ batch drivers -------------------------------- */
 typedef struct {
     int kind, model, flags, t, nt; int64_t n;

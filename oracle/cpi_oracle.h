@@ -29,6 +29,26 @@ int oracle_merge_records(int64_t n_groups, const int64_t* offsets, int64_t unifo
 int oracle_scan_records(int64_t n_groups, const int64_t* offsets, int64_t uniform, const double* records, const double* lin,
                         double* out, int nthreads);
 
+/* The solver side of a chain (DESIGN.md 3e, 3f), dense.  Chain layouts as the C ABI (CSR state offsets, or chains of `uniform`
+ * states when offsets is NULL).  chain_marginalize: K8's recurrence with a plain 15x15 Cholesky, NaN rule and m = 0 copy as
+ * cpi_imu_chain_marginalize; scale (may be NULL) [n_chains, 242]: per chain the size of the terms that cancel into info (225), rhs
+ * (15) and f (1), and the last step's z^T z.  chain_solve: x = A^-1 b of the SPD block-tridiagonal system, order 0 a sequential block
+ * Cholesky per chain, order 1 the block cyclic reduction of the whole system in the order of solve.cu.  lm_terms: out [n_chains, 5] =
+ * (model decrease, the size of its terms, current cost, candidate cost, delta != 0).  local / prior_at: the inverse of retract and
+ * cpi_imu_prior_at. */
+int oracle_chain_marginalize(int64_t n_chains, const int64_t* offsets, int64_t uniform, const int64_t* n_marg, int64_t marg_uniform,
+                             const double* G11, const double* G12, const double* G22, const double* g1, const double* g2, const double* f,
+                             const double* prior_info, const double* prior_rhs, const double* prior_f, double* out_info, double* out_rhs,
+                             double* out_f, double* scale, int nthreads);
+int oracle_chain_solve(int64_t n_chains, const int64_t* offsets, int64_t uniform, const double* D, const double* E, const double* b, double* x,
+                       int order, int nthreads);
+int oracle_lm_terms(int64_t n_chains, const int64_t* offsets, int64_t uniform, const double* rhs, const double* D, const double* E,
+                    const double* damp, const double* delta, const double* f_cur, const double* pf_cur, const double* f_new,
+                    const double* pf_new, double* out, int nthreads);
+int oracle_local(int64_t n, const double* lin, const double* x, double* delta);
+int oracle_prior_at(int64_t n, const double* info, const double* rhs, const double* f, const double* lin, const double* x, double* rhs_out,
+                    double* f_out);
+
 /* quat_ops.h helpers (col-major 3x3) */
 void oracle_rot_2_quat(const double* R, double* q);
 void oracle_quat_2_Rot(const double* q, double* R);

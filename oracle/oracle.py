@@ -204,6 +204,74 @@ class Oracle(_Base):
         """Every prefix of the left fold of every group (layout as cpi_scan_records_host); rows outside every group are zero."""
         return self._fold("oracle_scan_records", records, lin, group_offsets, group, nthreads, True)
 
+    # ---- the solver side of a chain (K8, k_prior_at, the block-tridiagonal solve, the LM model decrease).  Layouts as
+    # include/cpi_b200.h: chain_offsets [n_chains+1] int64, or chains of `uniform` states with n_chains given.
+    @staticmethod
+    def _chains(chain_offsets, uniform, n_chains):
+        if chain_offsets is not None:
+            offs = np.ascontiguousarray(chain_offsets, dtype=np.int64)
+            return offs.shape[0] - 1, offs, 0, int(offs[-1])
+        assert uniform is not None and uniform >= 1 and n_chains is not None
+        return int(n_chains), None, int(uniform), int(n_chains) * int(uniform)
+
+    def chain_marginalize(self, G11, G12, G22, g1, g2, f, n_marg, prior=None, chain_offsets=None, uniform=None, n_chains=None, nthreads=1):
+        """K8's recurrence per chain: returns (info [C,225], rhs [C,15], f [C], scale [C,242]) -- scale: the size of the terms that cancel
+        into info and rhs in the last step, of f over all steps, and the last step's z^T z.  n_marg: int or [C] int64."""
+        fn = self._rec_fn("oracle_chain_marginalize", [ctypes.c_int64, _PI, ctypes.c_int64, _PI, ctypes.c_int64] + [_P] * 12 + [_P, ctypes.c_int])
+        C, offs, u, _ = self._chains(chain_offsets, uniform, n_chains)
+        blk = [np.ascontiguousarray(a, dtype=np.float64) for a in (G11, G12, G22, g1, g2, f)]
+        nm, nmu = (None, int(n_marg)) if np.isscalar(n_marg) else (np.ascontiguousarray(n_marg, dtype=np.int64), 0)
+        pr = [None] * 3 if prior is None else [np.ascontiguousarray(a, dtype=np.float64) for a in prior]
+        oi, orr, of, sc = np.zeros((C, 225)), np.zeros((C, 15)), np.zeros(C), np.zeros((C, 242))
+        dp = lambda a: None if a is None else _d(a)
+        assert fn(C, _i(offs), u, _i(nm), nmu, *[_d(a) for a in blk], *[dp(a) for a in pr], _d(oi), _d(orr), _d(of), _d(sc), int(nthreads)) == 0
+        return oi, orr, of, sc
+
+    def chain_solve(self, D, E, b, order, chain_offsets=None, uniform=None, n_chains=None, nthreads=1):
+        """x [N,15] of tridiag(E^T, D, E) x = b: order 0 sequential block Cholesky per chain, 1 the block cyclic reduction of solve.cu."""
+        fn = self._rec_fn("oracle_chain_solve", [ctypes.c_int64, _PI, ctypes.c_int64, _P, _P, _P, _P, ctypes.c_int, ctypes.c_int])
+        C, offs, u, N = self._chains(chain_offsets, uniform, n_chains)
+        D = np.ascontiguousarray(D, dtype=np.float64).reshape(N, 225)
+        E = np.ascontiguousarray(E, dtype=np.float64).reshape(-1, 225)
+        if E.shape[0] < max(N - 1, 1):
+            E = np.concatenate([E, np.zeros((max(N - 1, 1) - E.shape[0], 225))])
+        b = np.ascontiguousarray(b, dtype=np.float64).reshape(N, 15)
+        x = np.zeros((N, 15))
+        assert fn(C, _i(offs), u, _d(D), _d(E), _d(b), _d(x), int(order), int(nthreads)) == 0
+        return x
+
+    def lm_terms(self, rhs, D, E, damp, delta, f_cur, f_new, pf_cur=None, pf_new=None, chain_offsets=None, uniform=None, n_chains=None, nthreads=1):
+        """Per chain [C,5]: (model decrease m, sum |delta|^T (2|rhs| + |H||delta|), current cost, candidate cost, delta != 0)."""
+        fn = self._rec_fn("oracle_lm_terms", [ctypes.c_int64, _PI, ctypes.c_int64] + [_P] * 10 + [ctypes.c_int])
+        C, offs, u, N = self._chains(chain_offsets, uniform, n_chains)
+        a = [np.ascontiguousarray(x, dtype=np.float64) for x in (rhs, D, E, damp, delta, f_cur)]
+        pc = None if pf_cur is None else np.ascontiguousarray(pf_cur, dtype=np.float64)
+        fnw = np.ascontiguousarray(f_new, dtype=np.float64)
+        pn = None if pf_new is None else np.ascontiguousarray(pf_new, dtype=np.float64)
+        dp = lambda x: None if x is None else _d(x)
+        out = np.zeros((C, 5))
+        assert fn(C, _i(offs), u, *[_d(x) for x in a], dp(pc), _d(fnw), dp(pn), _d(out), int(nthreads)) == 0
+        return out
+
+    def local(self, lin, x):
+        """local(x_lin, x) [n,15], the inverse of retract."""
+        fn = self._rec_fn("oracle_local", [ctypes.c_int64, _P, _P, _P])
+        lin = np.ascontiguousarray(lin, dtype=np.float64).reshape(-1, 16)
+        x = np.ascontiguousarray(x, dtype=np.float64).reshape(-1, 16)
+        d = np.zeros((lin.shape[0], 15))
+        assert fn(lin.shape[0], _d(lin), _d(x), _d(d)) == 0
+        return d
+
+    def prior_at(self, info, rhs, f, lin, x):
+        """cpi_imu_prior_at: (rhs' [n,15], f' [n])."""
+        fn = self._rec_fn("oracle_prior_at", [ctypes.c_int64] + [_P] * 7)
+        info = np.ascontiguousarray(info, dtype=np.float64).reshape(-1, 225)
+        n = info.shape[0]
+        a = [np.ascontiguousarray(v, dtype=np.float64) for v in (rhs, f, lin, x)]
+        ro, fo = np.zeros((n, 15)), np.zeros(n)
+        assert fn(n, _d(info), *[_d(v) for v in a], _d(ro), _d(fo)) == 0
+        return ro, fo
+
 
 class OracleLD(Oracle):
     """The same restatement computed in long double (oracle/liboracle_ld.so): double in, double out, about 1e-19 working
