@@ -42,6 +42,7 @@ SYMBOLS = {
     "cpi_imu_chains_solve": (c_int, [c_i64, c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "cpi_imu_chains_lm_workspace": (c_i64, [c_i64]),
     "cpi_imu_chains_lm_update": (c_int, [c_i64, c_vp, c_i64, c_i64, c_vp] + [c_vp] * 19),
+    "cpi_imu_state_priors_fold": (c_int, [c_i64, c_vp, c_i64] + [c_vp] * 13),
     "cpi_predict_state_batch": (c_int, [c_int, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "cpi_propagate_batch": (c_int, [c_int, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "cpi_propagate_batch_host": (c_int, [c_int, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),

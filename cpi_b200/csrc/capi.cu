@@ -612,6 +612,26 @@ int cpi_imu_prior_at(int64_t n, const double* info, const double* rhs, const dou
     return CPI_OK;
 }
 
+int cpi_imu_state_priors_fold(int64_t n_chains, const int64_t* chain_offsets, int64_t chain_uniform, const int64_t* sp_offsets,
+                              const double* sp_info, const double* sp_rhs, const double* sp_f, double* G11, double* G22, double* g1,
+                              double* g2, double* f, double* prior_info, double* prior_rhs, double* prior_f, void* stream) {
+    int rc = chain_layout_check(n_chains, chain_offsets, chain_uniform);
+    if (rc || n_chains == 0) return rc;
+    if (!sp_offsets) return fail(CPI_EINVAL, "null pointer argument (sp_offsets)");
+    if ((sp_info == nullptr) != (sp_rhs == nullptr)) return fail(CPI_EINVAL, "sp_info and sp_rhs must both be given or both be null");
+    if (!sp_info && !sp_f) return fail(CPI_EINVAL, "null pointer argument (sp_f: the f-only fold needs the priors' constants)");
+    if (!chain_offsets && chain_uniform == 1) {                    // every state is a chain of its own: everything lands on the chain priors
+        if (sp_info && (!prior_info || !prior_rhs)) return fail(CPI_EINVAL, "null pointer argument (prior_info / prior_rhs: single-state chains)");
+        if (sp_f && !prior_f) return fail(CPI_EINVAL, "null pointer argument (prior_f: single-state chains)");
+    }
+    DevInfo d;
+    if ((rc = device_info(d))) return rc;
+    CU(cpi::state_priors_fold_launch(n_chains, chain_offsets, chain_uniform, sp_offsets, sp_info, sp_rhs, sp_f, G11, G22, g1, g2, f, prior_info,
+                                     prior_rhs, prior_f, d.sms, (cudaStream_t)stream));
+    g_launches += 1;
+    return CPI_OK;
+}
+
 int64_t cpi_imu_chain_solve_workspace(int64_t n_states) { return n_states < 0 ? (int64_t)CPI_EINVAL : cpi::chain_solve_workspace_bytes(n_states); }
 
 int cpi_imu_chain_solve(int64_t n_states, const double* D, const double* E, const double* rhs, double* x, void* workspace, void* stream) {

@@ -94,6 +94,10 @@ cudaError_t lm_update_launch(int64_t n_chains, const int64_t* offs, int64_t unif
                              const double* pf_cur, const double* f_new, const double* pf_new, const double* rhs, const double* D, const double* E,
                              const double* damp, const double* delta, const double* states_new, double* states, double* lam, double* cost,
                              int32_t* status, int32_t* iterations, int32_t* tries, int32_t* any_running, double* ws, cudaStream_t st);
+// state_priors.cu: priors on any state folded into the factor blocks / chain priors (sp_info, sp_rhs NULL: the f-only fold)
+cudaError_t state_priors_fold_launch(int64_t n_chains, const int64_t* offs, int64_t uniform, const int64_t* sp_offsets, const double* sp_info,
+                                     const double* sp_rhs, const double* sp_f, double* G11, double* G22, double* g1, double* g2, double* f,
+                                     double* prior_info, double* prior_rhs, double* prior_f, int sms, cudaStream_t st);
 cudaError_t retract_launch(int64_t n, const double* states, const double* xi, double* out, cudaStream_t st);
 
 }  // namespace cpi

@@ -225,17 +225,98 @@ def chains_assemble(G11, G12, G22, g1, g2, chain_offsets, lam=0.0, prior_info=No
     return D, E[:N - 1], rhs
 
 
-def chain_marginalize(G11, G12, G22, g1, g2, f, chain_offsets, n_marg, prior=None, n_chains=None, stream=None):
+def _state_priors(state_priors, N, dev, offs=None, S=0):
+    """Validated state priors (state_idx [M] int64, info [M,225], rhs [M,15] | None, f [M] | None, lin [M,16]) on N states: returns
+    (idx, info, rhs (zeros if None), f or None, lin, single) with single whether a chain of one state carries a prior, or None for
+    state_priors None or M = 0.  Checks shapes and dtypes, then 0 <= state_idx < N (the one host read), then the device."""
+    import torch
+
+    if state_priors is None:
+        return None
+    if not isinstance(state_priors, (tuple, list)) or len(state_priors) != 5:
+        raise ValueError("state_priors is (state_idx [M], info [M,225], rhs [M,15] or None, f [M] or None, lin [M,16])")
+    idx, info, rhs, f, lin = state_priors
+    if not isinstance(idx, torch.Tensor) or idx.dtype != torch.int64 or idx.dim() != 1:
+        raise ValueError("state_priors: state_idx must be a 1-d int64 tensor")
+    M = idx.numel()
+    for name, t, k in (("info", info, 225), ("rhs", rhs, 15), ("f", f, 1), ("lin", lin, 16)):
+        if t is None and name in ("rhs", "f"):
+            continue
+        if not isinstance(t, torch.Tensor) or t.dtype != torch.float64:
+            raise ValueError(f"state_priors: {name} must be a float64 tensor")
+        if t.numel() != k * M or t.dim() < 1 or t.shape[0] != M:
+            raise ValueError(f"state_priors: {name} needs {k} doubles for each of the {M} priors")
+    if M:
+        flags = [((idx < 0) | (idx >= N)).any()]
+        if offs is not None and idx.device == offs.device:         # a chain of one state carrying a prior: the chain prior is its target
+            c = (torch.searchsorted(offs, idx.clamp(0, max(N - 1, 0)), right=True) - 1).clamp(0, offs.numel() - 2)
+            flags.append(((offs[c + 1] - offs[c]) == 1).any())
+        flags = torch.stack(flags).tolist()
+        if flags[0]:
+            raise IndexError(f"state_priors: state_idx out of range [0, {N})")
+    if not idx.is_cuda or idx.device != dev:
+        raise ValueError(f"state_priors: state_idx must be a CUDA tensor on {dev}")
+    _check_f64(dev, state_prior_info=info, state_prior_rhs=rhs, state_prior_f=f, state_prior_lin=lin)
+    if M == 0:
+        return None
+    single = bool(flags[1]) if offs is not None else S == 1
+    rhs = torch.zeros((M, 15), dtype=torch.float64, device=dev) if rhs is None else rhs
+    return idx, info.reshape(M, 225), rhs.reshape(M, 15), None if f is None else f.reshape(M), lin.reshape(M, 16), single
+
+
+def _state_prior_csr(key, N):
+    """(order, sp_offsets [N+1]): the stable sort of the priors by key and the CSR of the keys below N (the priors of state k are
+    order[sp_offsets[k] .. sp_offsets[k+1]-1])."""
+    import torch
+
+    key_s, order = torch.sort(key, stable=True)
+    return order, torch.searchsorted(key_s, torch.arange(N + 1, dtype=torch.int64, device=key.device))
+
+
+def state_priors_fold(chain_offsets, sp_offsets, sp_info, sp_rhs, sp_f, G11=None, G22=None, g1=None, g2=None, f=None, prior_info=None,
+                      prior_rhs=None, prior_f=None, n_chains=None, stream=None):
+    """Add already-moved state priors IN PLACE into the factor blocks and chain priors (cpi_imu_state_priors_fold): a prior on state k
+    of chain c goes to G11 / g1 / f of factor k - c, on a chain's last state to G22 / g2 / f of factor k - 1 - c, on a chain's only state
+    to the chain prior.  sp_offsets: device int64 [N+1] CSR over the states (priors sorted by state, added in that order); sp_info
+    [M,225] / sp_rhs [M,15]: both or None (None: the f-only fold of sp_f [M]); a target that is None receives nothing.  Chain layout as
+    chains_assemble (the state count N is sp_offsets' length - 1)."""
+    import torch
+
+    dev = sp_offsets.device
+    if not sp_offsets.is_cuda or sp_offsets.dtype != torch.int64 or sp_offsets.dim() != 1 or sp_offsets.numel() < 1:
+        raise ValueError("sp_offsets must be a 1-d int64 CUDA tensor of n_states + 1 entries")
+    _check_f64(dev, sp_info=sp_info, sp_rhs=sp_rhs, sp_f=sp_f, G11=G11, G22=G22, g1=g1, g2=g2, f=f, prior_info=prior_info,
+               prior_rhs=prior_rhs, prior_f=prior_f)
+    N = sp_offsets.numel() - 1
+    C, offs, S = _chain_layout(chain_offsets, dev, n_states=N, n_chains=n_chains)
+    for t in (G11, G22, g1, g2, f, prior_info, prior_rhs, prior_f):
+        if t is not None and not t.is_contiguous():
+            raise ValueError("the fold writes in place: its targets must be contiguous")
+    c = lambda t: None if t is None else t.contiguous()
+    with torch.cuda.device(dev):
+        st = stream if stream is not None else torch.cuda.current_stream(dev)
+        capi.check(capi.load().cpi_imu_state_priors_fold(C, _tptr(offs), S, _tptr(sp_offsets.contiguous()), _tptr(c(sp_info)), _tptr(c(sp_rhs)),
+                                                         _tptr(c(sp_f)), _tptr(G11), _tptr(G22), _tptr(g1), _tptr(g2), _tptr(f), _tptr(prior_info),
+                                                         _tptr(prior_rhs), _tptr(prior_f), ctypes.c_void_p(st.cuda_stream)))
+
+
+def chain_marginalize(G11, G12, G22, g1, g2, f, chain_offsets, n_marg, prior=None, n_chains=None, stream=None, state_priors=None):
     """Eliminate the first n_marg states of every chain into a dense prior on the first state it keeps (cpi_imu_chain_marginalize,
     kernel K8): the Schur complement a fixed-lag smoother keeps of the states that leave its window, at the linearisation point of the
     blocks, undamped.  Blocks as factor_hessian returns them (chain layout as chains_assemble); n_marg: int or device int64 [n_chains]
     (0 <= n_marg < states of the chain); prior: (info [n_chains,225], rhs [n_chains,15], f [n_chains]) on every chain's first state, or
-    None.  Returns the prior on state offsets[c] + n_marg[c]: (info [n_chains,225] exactly symmetric, rhs [n_chains,15], f [n_chains])."""
+    None.  state_priors: as chains_lm_step, taken as given at the blocks' linearisation point; only those on eliminated states
+    (state_idx < offsets[c] + n_marg[c]) are folded, into copies of G11 / g1 / f, so a prior on a kept state is left to the caller.
+    Returns the prior on state offsets[c] + n_marg[c]: (info [n_chains,225] exactly symmetric, rhs [n_chains,15], f [n_chains])."""
     import torch
 
     dev = G11.device
-    _check_f64(dev, G11=G11, G12=G12, G22=G22, g1=g1, g2=g2, f=f)
     nf = G11.numel() // 225
+    sp = None
+    if state_priors is not None:
+        C, offs, S = _chain_layout(chain_offsets, dev, n_factors=nf, n_chains=n_chains)
+        sp = _state_priors(state_priors, nf + C, dev)
+    _check_f64(dev, G11=G11, G12=G12, G22=G22, g1=g1, g2=g2, f=f)
     C, offs, S = _chain_layout(chain_offsets, dev, n_factors=nf, n_chains=n_chains)
     if any(t.numel() != k * nf for t, k in ((G11, 225), (G12, 225), (G22, 225), (g1, 15), (g2, 15), (f, 1))):
         raise ValueError("G11 / G12 / G22 need 225 doubles, g1 / g2 15 and f 1 per factor")
@@ -252,6 +333,19 @@ def chain_marginalize(G11, G12, G22, g1, g2, f, chain_offsets, n_marg, prior=Non
         nm, nmu = n_marg.contiguous(), 0
     else:
         nm, nmu = None, int(n_marg)
+    if sp is not None:                                               # eliminated states are never last: their priors land in G11 / g1 / f
+        idx, s_info, s_rhs, s_f, _, _ = sp
+        if offs is not None:
+            c = (torch.searchsorted(offs, idx, right=True) - 1).clamp(0, C - 1)
+            head = offs[c]
+        else:
+            c = idx // S
+            head = c * S
+        head = head + (nm[c] if nm is not None else nmu)
+        order, sp_off = _state_prior_csr(torch.where(idx < head, idx, idx + nf + C), nf + C)
+        G11, g1, f = G11.contiguous().clone(), g1.contiguous().clone(), f.contiguous().clone()
+        state_priors_fold(offs if offs is not None else S, sp_off, s_info[order], s_rhs[order], None if s_f is None else s_f[order],
+                          G11=G11, g1=g1, f=f, n_chains=C, stream=stream)
     info = torch.empty((C, 225), dtype=torch.float64, device=dev)
     rhs = torch.empty((C, 15), dtype=torch.float64, device=dev)
     fo = torch.empty((C,), dtype=torch.float64, device=dev)
@@ -285,14 +379,16 @@ def prior_at(info, rhs, f, lin_states, states, stream=None):
     return rhs_out, f_out
 
 
-def chains_lm_step(model, states, records, lin, chain_offsets, prior=None, lam=1e-5, diagonal_damping=True, stream=None):
+def chains_lm_step(model, states, records, lin, chain_offsets, prior=None, lam=1e-5, diagonal_damping=True, stream=None, state_priors=None):
     """One damped Gauss-Newton step of many independent IMU-only chains at once (a fixed-lag smoother's windows), on the device:
     evaluateError -> information blocks -> prior_at (every chain's prior moved to its current first state) -> chains_assemble ->
     ONE block-cyclic-reduction solve over all chains -> retract.  states [N,16]; records / lin: the N - n_chains factors, chain c's
     stored back to back from index offsets[c] - c; chain_offsets as chains_assemble (device int64 [n_chains+1], or states per chain);
     prior: (info [n_chains,225], rhs [n_chains,15], f [n_chains], lin_states [n_chains,16]) or None.  lin_states = None: the prior is
     linearised at the chains' current first states, so it is used as given without prior_at (rhs and f may then be None: zero).
-    Returns (new_states, delta [N,15], cost per chain before the step [n_chains] = sum of e^T P^-1 e + the moved prior's f')."""
+    state_priors: priors on any states, (state_idx [M] int64, info [M,225], rhs [M,15] or None, f [M] or None, lin [M,16]) or None
+    (include/cpi_b200.h, DESIGN.md section 3g): moved to the states by prior_at and folded into the blocks (state_priors_fold).
+    Returns (new_states, delta [N,15], cost per chain before the step [n_chains] = sum of e^T P^-1 e + the moved priors' f')."""
     import torch
 
     dev = states.device
@@ -301,6 +397,7 @@ def chains_lm_step(model, states, records, lin, chain_offsets, prior=None, lam=1
     nf = N - C
     if records.numel() != REC_DOUBLES[model] * nf:
         raise ValueError(f"{C} chains over {N} states hold {nf} factors: one record each")
+    sp = _state_priors(state_priors, N, dev, offs, S)
     idx_i = idx_j = chain_of = None
     if C > 1:                                                        # one chain: the eval kernel's own chain indexing
         ar = torch.arange(nf, dtype=torch.int64, device=dev)
@@ -318,6 +415,18 @@ def chains_lm_step(model, states, records, lin, chain_offsets, prior=None, lam=1
         if lin0 is not None:
             first = states.reshape(N, 16)[offs[:-1]] if offs is not None else states.reshape(N, 16)[::S]
             pr, pf = prior_at(pi, pr, pf, lin0, first, stream=stream)
+    if sp is not None:
+        idx, s_info, s_rhs, s_f, s_lin, single = sp
+        order, sp_off = _state_prior_csr(idx, N)
+        s_info, s_lin, idx = s_info[order], s_lin[order], idx[order]
+        r_m, f_m = prior_at(s_info, s_rhs[order], None if s_f is None else s_f[order], s_lin, states.reshape(N, 16).index_select(0, idx),
+                            stream=stream)
+        if single:                                                   # the chain prior receives priors: fold into copies (zeros without one)
+            z = lambda t, *shape: torch.zeros(shape, dtype=torch.float64, device=dev) if t is None else t.contiguous().clone()
+            pi, pr, pf = z(pi, C, 225), z(pr, C, 15), z(pf, C)
+        state_priors_fold(offs if offs is not None else S, sp_off, s_info, r_m, f_m, G11=G11, G22=G22, g1=g1, g2=g2, f=f,
+                          prior_info=pi if single else None, prior_rhs=pr if single else None, prior_f=pf if single else None, n_chains=C,
+                          stream=stream)
     D, E, rhs = chains_assemble(G11, G12, G22, g1, g2, chain_offsets, lam, pi, pr, diagonal_damping=diagonal_damping, n_chains=C, stream=stream)
     dx = chain_solve(D, E, rhs, stream=stream)
     # per-chain cost: one chain sums like chain_lm_step always has; many chains scatter-add their factors' f
@@ -424,21 +533,27 @@ def chains_solve(D, E, rhs, chain_offsets, n_chains=None, workspace=None, stream
 
 
 def chains_lm(model, states, records, lin, chain_offsets, prior=None, lam=1e-5, diagonal_damping=True, params=None, max_rounds=200, check_every=8,
-              stream=None):
+              stream=None, state_priors=None):
     """Levenberg-Marquardt of many independent IMU-only chains at once, to convergence, on the device (GTSAM's
     LevenbergMarquardtOptimizer rule per chain: include/cpi_b200.h, DESIGN.md section 3f).  Arguments as chains_lm_step; lam: the
     initial lambda of every chain; params: capi.LMParams (None: GTSAM's defaults).  A prior without a linearisation point is taken as
     linearised at the initial first states.  Per round: eval -> information blocks -> prior_at -> chains_assemble_lm (lambda per chain)
     -> chains_solve (chains isolated) -> retract -> factor_cost + prior_at at the candidate -> cpi_imu_chains_lm_update.  No host
     synchronisation inside the loop except one 4-byte "any chain running" read every check_every rounds (0: max_rounds rounds, fully
-    asynchronous).  Returns (states [N,16], cost [C] at them, lam [C], status [C] int32 (capi.LM_*), iterations [C] (accepted steps),
-    tries [C] (rounds the chain ran)), all int32 counters."""
+    asynchronous).  state_priors as chains_lm_step: every round moves them to the current states after the information blocks and
+    folds them in (state_priors_fold), and folds their f' at the candidate into its cost.  Returns (states [N,16], cost [C] at them,
+    lam [C], status [C] int32 (capi.LM_*), iterations [C] (accepted steps), tries [C] (rounds the chain ran)), all int32 counters."""
     import torch
 
     lib = capi.load()
     dev = states.device
-    _check_f64(dev, states=states, records=records, lin=lin)
     N = states.numel() // 16
+    if state_priors is not None:
+        C, offs, S = _chain_layout(chain_offsets, dev, n_states=N)
+        sp = _state_priors(state_priors, N, dev, offs, S)
+    else:
+        sp = None
+    _check_f64(dev, states=states, records=records, lin=lin)
     C, offs, S = _chain_layout(chain_offsets, dev, n_states=N)
     nf = N - C
     if records.numel() != REC_DOUBLES[model] * nf or lin.numel() != 13 * nf:
@@ -468,6 +583,18 @@ def chains_lm(model, states, records, lin, chain_offsets, prior=None, lam=1e-5, 
         pr = torch.zeros((C, 15), **f64) if pr is None else pr.contiguous()
         pf = torch.zeros(C, **f64) if pf is None else pf.contiguous()
         lin0 = X.index_select(0, first) if lin0 is None else lin0.contiguous()
+    use_prior, single, s_lin = prior is not None, False, None
+    if sp is not None:
+        s_idx, s_info, s_rhs, s_f, s_lin, single = sp
+        order, sp_off = _state_prior_csr(s_idx, N)
+        s_idx, s_info, s_rhs, s_lin = s_idx[order], s_info[order].contiguous(), s_rhs[order].contiguous(), s_lin[order].contiguous()
+        s_f = None if s_f is None else s_f[order].contiguous()
+        M = s_idx.numel()
+        s_x, s_r, s_fc, s_fn = torch.empty((M, 16), **f64), torch.empty((M, 15), **f64), torch.empty(M, **f64), torch.empty(M, **f64)
+        if single and not use_prior:                                 # a chain of one state carries priors: a zero chain prior receives them
+            pi, pr, pf, lin0 = torch.zeros((C, 225), **f64), torch.zeros((C, 15), **f64), torch.zeros(C, **f64), X.index_select(0, first)
+            use_prior = True
+    pi_r = torch.empty((C, 225), **f64) if single else None          # the chain prior's info with the round's priors folded in
     lam_t = torch.full((C,), float(lam), **f64)
     cost = torch.zeros(C, **f64)
     status, iters, tries = torch.zeros(C, **i32), torch.zeros(C, **i32), torch.zeros(C, **i32)
@@ -493,22 +620,34 @@ def chains_lm(model, states, records, lin, chain_offsets, prior=None, lam=1e-5, 
                     capi.check(lib.cpi_imu_factor_eval_batch(model, nf, p(X), p(idx_i), p(idx_j), p(records), p(lin), p(e), p(H1), p(H2), sp))
                     capi.check(lib.cpi_imu_factor_hessian_batch(model, nf, p(records), p(e), p(H1), p(H2), p(G11), p(G12), p(G22), p(g1), p(g2),
                                                                 p(f_cur), sp))
-                if prior is not None:
+                if use_prior:
                     torch.index_select(X, 0, first, out=x0)
                     capi.check(lib.cpi_imu_prior_at(C, p(pi), p(pr), p(pf), p(lin0), p(x0), p(pr_c), p(pf_c), sp))
+                if s_lin is not None:                                # the state priors at X, folded into this round's blocks
+                    torch.index_select(X, 0, s_idx, out=s_x)
+                    capi.check(lib.cpi_imu_prior_at(M, p(s_info), p(s_rhs), p(s_f), p(s_lin), p(s_x), p(s_r), p(s_fc), sp))
+                    if single:
+                        pi_r.copy_(pi)
+                    capi.check(lib.cpi_imu_state_priors_fold(C, p(offs), S, p(sp_off), p(s_info), p(s_r), p(s_fc), p(G11), p(G22), p(g1), p(g2),
+                                                             p(f_cur), p(pi_r), p(pr_c if single else None), p(pf_c if single else None), sp))
                 capi.check(lib.cpi_imu_chains_assemble_lm(C, p(offs), S, p(G11), p(G12), p(G22), p(g1), p(g2), p(lam_t), int(bool(diagonal_damping)),
-                                                          p(pi), p(pr_c if prior is not None else None), p(D), p(E), p(rhs), p(damp), sp))
+                                                          p(pi_r if single else pi), p(pr_c if use_prior else None), p(D), p(E), p(rhs), p(damp), sp))
                 capi.check(lib.cpi_imu_chains_solve(C, p(offs), S, N, p(D), p(E), p(rhs), p(dx), p(ws_solve), sp))
                 capi.check(lib.cpi_retract_batch(N, p(X), p(dx), p(Xn), sp))
                 if nf:
                     capi.check(lib.cpi_imu_factor_cost_batch(model, nf, p(Xn), p(idx_i), p(idx_j), p(records), p(lin), p(f_new), sp))
-                if prior is not None:
+                if use_prior:
                     torch.index_select(Xn, 0, first, out=x0)
                     capi.check(lib.cpi_imu_prior_at(C, p(pi), p(pr), p(pf), p(lin0), p(x0), p(pr_n), p(pf_n), sp))
+                if s_lin is not None:                                # their f' at the candidate, into its cost
+                    torch.index_select(Xn, 0, s_idx, out=s_x)
+                    capi.check(lib.cpi_imu_prior_at(M, p(s_info), p(s_rhs), p(s_f), p(s_lin), p(s_x), p(s_r), p(s_fn), sp))
+                    capi.check(lib.cpi_imu_state_priors_fold(C, p(offs), S, p(sp_off), None, None, p(s_fn), None, None, None, None, p(f_new), None,
+                                                             None, p(pf_n if single else None), sp))
                 if check:
                     flag.zero_()
-                capi.check(lib.cpi_imu_chains_lm_update(C, p(offs), S, N, ctypes.byref(params), p(f_cur), p(pf_c if prior is not None else None),
-                                                        p(f_new), p(pf_n if prior is not None else None), p(rhs), p(D), p(E), p(damp), p(dx), p(Xn),
+                capi.check(lib.cpi_imu_chains_lm_update(C, p(offs), S, N, ctypes.byref(params), p(f_cur), p(pf_c if use_prior else None),
+                                                        p(f_new), p(pf_n if use_prior else None), p(rhs), p(D), p(E), p(damp), p(dx), p(Xn),
                                                         p(X), p(lam_t), p(cost), p(status), p(iters), p(tries), p(flag if check else None),
                                                         p(ws_lm), sp))
                 if check and int(flag.item()) == 0:

@@ -256,7 +256,8 @@ int cpi_imu_factor_whiten_batch(int model, int64_t n_factors, const double* reco
  *       lambda I (diagonal_damping = 0, GTSAM's default) or lambda * clamp(diag D[k], 1e-6, 1e32) (diagonal_damping = 1, Marquardt).
  *       NOTE: an IMU-only chain anchored by one prior is numerically singular in fp64 beyond a few hundred keyframes with
  *       undamped / lambda-I normal equations (the drift modes carry ~1e-16 of the largest eigenvalue) -- for ANY elimination order;
- *       diagonal damping (or the camera factors of the real graph) restores a well-posed system (DESIGN.md section 5).
+ *       diagonal damping (or the camera factors of the real graph) restores a well-posed system (DESIGN.md section 5); so do priors
+ *       on later states (position fixes: cpi_imu_state_priors_fold, DESIGN.md section 3g).
  *   cpi_imu_chain_solve      x = (that SPD block-tridiagonal matrix)^-1 rhs by block cyclic reduction (Cholesky on the 15x15 pivots):
  *       ~2 log2(n) + 1 kernel launches instead of an n-step sequential block recurrence.  `workspace`: device buffer of
  *       cpi_imu_chain_solve_workspace(n_states) bytes.  The step is then applied with cpi_retract_batch.
@@ -377,6 +378,40 @@ int cpi_imu_chains_lm_update(int64_t n_chains, const int64_t* chain_offsets, int
                              const double* prior_f_new, const double* rhs, const double* D, const double* E, const double* damp,
                              const double* delta, const double* states_new, double* states, double* lambda, double* cost,
                              int32_t* status, int32_t* iterations, int32_t* tries, int32_t* any_running, void* workspace, void* stream);
+
+/*
+ * Priors on any state of many chains (DESIGN.md section 3g): GTSAM's PriorFactor / the reference's JPLNavStatePrior on any keyframe --
+ * absolute position or attitude fixes, zero-velocity updates, anchors every N keyframes.  fp64, DEVICE pointers, asynchronous on
+ * `stream`, no allocation.  PARITY UNPINNED (the convention is the library's own); tests/test_state_priors.py holds the numpy statement.
+ *
+ * A state prior i is (s_i, info_i[225] column-major, rhs_i[15], f_i, lin_i[16]) in the convention of the chain prior above: s_i indexes
+ * the concatenated states of the chain layout, cost = 1/2 (f - 2 rhs^T delta + delta^T info delta) with delta = local(lin_i, x_{s_i}).
+ * It is moved to the current states by cpi_imu_prior_at (n = the number of state priors), Jacobian of local taken as the identity.
+ * A measurement x_bar with information W is (info = W, rhs = 0, f = 0, lin = x_bar): cost delta^T W delta.  A partial measurement
+ * (position only, velocity only) uses a PSD W that is zero outside its blocks.  Limits:
+ *   - lin_i must be a finite state with a unit quaternion even where W is zero: delta is formed in full, and 0 * NaN poisons.
+ *   - With the identity Jacobian, a strong ATTITUDE prior with a large residual converges to a point off the true optimum by second
+ *     order in that residual.  Position, velocity and bias priors are exact (local is a difference there).
+ *
+ *   cpi_imu_state_priors_fold   adds the moved priors (sp_info, sp_rhs = rhs', sp_f = f') IN PLACE into blocks the assembly, the
+ *       solves, K8 and the LM decision already read.  For a prior on state k of chain c (states o[c] .. o[c+1]-1):
+ *           k not the chain's last state                 -> G11, g1, f of the factor to its right (index k - c)
+ *           k the last state of a chain of >= 2 states   -> G22, g2, f of the factor to its left  (index k - 1 - c)
+ *           k the only state of its chain                -> the chain prior prior_info, prior_rhs, prior_f of chain c
+ *       Each 15x15 block and rhs segment receives the priors of one state; the f of a chain's last factor receives those of its
+ *       two states (the left state's first, one warp adding both).  The priors are sorted by state: sp_offsets (device int64
+ *       [n_states+1], CSR) gives state k the priors sp_offsets[k] .. sp_offsets[k+1]-1, added one after the other in that order
+ *       (no atomics: the same bits on every run).  Folded before the assembly, a prior sits in diag(D) before the damping, where
+ *       Marquardt's diagonal damping and the model decrease of cpi_imu_chains_lm_update see it.  K8 eliminates states that are never
+ *       the last of their chain, so the priors of eliminated states land in exactly the G11 blocks it consumes.
+ *       sp_info / sp_rhs: both or neither; neither is the f-only fold (sp_f into f / prior_f only: the candidate's cost in LM).
+ *       sp_f may be NULL.  A NULL target receives nothing: pass it only where no prior can land (for example G22 / g2 when no prior
+ *       sits on a chain's last state); with chain_uniform = 1 the chain-prior targets are required.  The chain is found by binary
+ *       search on a device-resident layout, which is never read on the host.
+ */
+int cpi_imu_state_priors_fold(int64_t n_chains, const int64_t* chain_offsets, int64_t chain_uniform, const int64_t* sp_offsets,
+                              const double* sp_info, const double* sp_rhs, const double* sp_f, double* G11, double* G22, double* g1,
+                              double* g2, double* f, double* prior_info, double* prior_rhs, double* prior_f, void* stream);
 
 /* ---- callers either side of the factor ("next" rows) ----------------------------------------------------------------- */
 
