@@ -43,6 +43,7 @@ SYMBOLS = {
     "cpi_imu_chains_lm_workspace": (c_i64, [c_i64]),
     "cpi_imu_chains_lm_update": (c_int, [c_i64, c_vp, c_i64, c_i64, c_vp] + [c_vp] * 19),
     "cpi_imu_state_priors_fold": (c_int, [c_i64, c_vp, c_i64] + [c_vp] * 13),
+    "cpi_imu_state_priors_robust": (c_int, [c_i64] + [c_vp] * 9),
     "cpi_predict_state_batch": (c_int, [c_int, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "cpi_propagate_batch": (c_int, [c_int, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "cpi_propagate_batch_host": (c_int, [c_int, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
@@ -71,6 +72,8 @@ SYMBOLS = {
 REC_DOUBLES = {1: 290, 2: 308}
 # Levenberg-Marquardt chain status (CPI_LM_*)
 LM_RUNNING, LM_CONVERGED, LM_MAX_ITERATIONS, LM_LAMBDA_EXHAUSTED, LM_NONFINITE = 0, 1, 2, 3, 4
+# robust losses on state priors (CPI_LOSS_*)
+LOSS_GAUSSIAN, LOSS_HUBER, LOSS_CAUCHY = 0, 1, 2
 
 
 class LMParams(ctypes.Structure):

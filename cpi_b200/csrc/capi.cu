@@ -632,6 +632,22 @@ int cpi_imu_state_priors_fold(int64_t n_chains, const int64_t* chain_offsets, in
     return CPI_OK;
 }
 
+int cpi_imu_state_priors_robust(int64_t n, const int32_t* loss, const double* loss_k, const double* info, const double* rhs, const double* f,
+                                double* info_out, double* rhs_out, double* f_out, void* stream) {
+    if (n < 0) return fail(CPI_EINVAL, "negative count");
+    if (n == 0) return CPI_OK;
+    if (n > ((int64_t)1 << 31)) return fail(CPI_EINVAL, "too many priors (%lld; at most 2^31 per call)", (long long)n);
+    if (!loss || !loss_k || !f || !f_out) return fail(CPI_EINVAL, "null pointer argument (loss / loss_k / f / f_out)");
+    if ((info_out == nullptr) != (rhs_out == nullptr)) return fail(CPI_EINVAL, "info_out and rhs_out must both be given or both be null");
+    if (info_out && (!info || !rhs)) return fail(CPI_EINVAL, "null pointer argument (info / rhs: the full pass reads them)");
+    DevInfo d;
+    int rc = device_info(d);
+    if (rc) return rc;
+    CU(cpi::state_priors_robust_launch(n, loss, loss_k, info, rhs, f, info_out, rhs_out, f_out, (cudaStream_t)stream));
+    g_launches += 1;
+    return CPI_OK;
+}
+
 int64_t cpi_imu_chain_solve_workspace(int64_t n_states) { return n_states < 0 ? (int64_t)CPI_EINVAL : cpi::chain_solve_workspace_bytes(n_states); }
 
 int cpi_imu_chain_solve(int64_t n_states, const double* D, const double* E, const double* rhs, double* x, void* workspace, void* stream) {

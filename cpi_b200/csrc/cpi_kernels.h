@@ -98,6 +98,9 @@ cudaError_t lm_update_launch(int64_t n_chains, const int64_t* offs, int64_t unif
 cudaError_t state_priors_fold_launch(int64_t n_chains, const int64_t* offs, int64_t uniform, const int64_t* sp_offsets, const double* sp_info,
                                      const double* sp_rhs, const double* sp_f, double* G11, double* G22, double* g1, double* g2, double* f,
                                      double* prior_info, double* prior_rhs, double* prior_f, int sms, cudaStream_t st);
+// state_priors.cu: robust (Huber / Cauchy) reweighting of moved measurement priors (info_out, rhs_out NULL: the f-only pass)
+cudaError_t state_priors_robust_launch(int64_t n, const int32_t* loss, const double* loss_k, const double* info, const double* rhs,
+                                       const double* f, double* info_out, double* rhs_out, double* f_out, cudaStream_t st);
 cudaError_t retract_launch(int64_t n, const double* states, const double* xi, double* out, cudaStream_t st);
 
 }  // namespace cpi

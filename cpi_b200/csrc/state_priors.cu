@@ -9,7 +9,14 @@
 //                       range sp_offsets[k] .. sp_offsets[k+1]-1 and are added one after the other in that order: additions only, no
 //                       atomics, the same bits on every run.  Each 15x15 block and rhs segment receives the priors of exactly one
 //                       state; the f of a chain's last factor receives those of its two states, added by one warp, the left state's first.
-// GTSAM is not part of the reference tree: PARITY UNPINNED -- the numpy statement of tests/test_state_priors.py is the reference.
+//   k_state_prior_robust  reweights moved MEASUREMENT priors (rhs = 0, f = 0 before prior_at, so f' = s = delta^T W delta) by a robust
+//                       loss (DESIGN.md section 3h): (info, rhs', f') -> (w info, w rhs', c(s)) with c = 2 rho(sqrt s) and the IRLS
+//                       weight w = dc/ds of GTSAM's noiseModel::Robust (Huber, Cauchy).  One warp per prior (grid-stride), one lane
+//                       computes s, w and c and broadcasts them, the lanes scale the 225 + 15 entries.  A weight of exactly 1 copies.
+// GTSAM is not part of the reference tree: PARITY UNPINNED -- the numpy statement of tests/test_state_priors.py is the reference (and
+// that of tests/test_robust_priors.py for the losses).
+#include <math_constants.h>
+
 #include <algorithm>
 
 #include "cpi_common.cuh"
@@ -77,6 +84,57 @@ cudaError_t state_priors_fold_launch(int64_t n_chains, const int64_t* offs, int6
     if (grid < 1) return cudaSuccess;
     k_state_prior_fold<<<(int)grid, 128, 0, st>>>(n_chains, offs, uniform, sp_offsets, sp_info, sp_rhs, sp_f, G11, G22, g1, g2, f, prior_info,
                                                   prior_rhs, prior_f);
+    return cudaGetLastError();
+}
+
+// cost c(s) and IRLS weight w(s) = dc/ds of a whitened squared residual s under loss `code` with threshold k (standard deviations).
+// A Huber inlier (s <= k^2) is the Gaussian prior itself: w = 1, c = s.  An unknown code, or k outside 0 < k^2 < inf, gives NaN.
+CPI_DEV void robust_loss(int code, double k, double s, double& w, double& c) {
+    if (code == CPI_LOSS_GAUSSIAN) { w = 1.0; c = s; return; }
+    const double k2 = k * k;
+    if (!(k > 0.0 && k2 > 0.0 && k2 < CUDART_INF) || (code != CPI_LOSS_HUBER && code != CPI_LOSS_CAUCHY)) {
+        w = c = CUDART_NAN;
+        return;
+    }
+    if (code == CPI_LOSS_HUBER) {
+        if (s <= k2) { w = 1.0; c = s; return; }
+        const double r = sqrt(s);
+        w = k / r;
+        c = 2.0 * k * r - k2;
+    } else {
+        const double u = s / k2;
+        w = 1.0 / (1.0 + u);
+        c = k2 * log1p(u);
+    }
+}
+
+__global__ void __launch_bounds__(128) k_state_prior_robust(int64_t n, const int32_t* loss, const double* loss_k, const double* info,
+                                                            const double* rhs, const double* f, double* info_out, double* rhs_out, double* f_out) {
+    const int wib = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int64_t i = (int64_t)blockIdx.x * 4 + wib; i < n; i += (int64_t)gridDim.x * 4) {
+        double w = 0.0, c = 0.0;
+        if (lane == 0) robust_loss(loss[i], loss_k[i], f[i], w, c);
+        w = __shfl_sync(0xffffffffu, w, 0);
+        c = __shfl_sync(0xffffffffu, c, 0);
+        if (info_out) {                                            // rhs_out may alias rhs: each lane reads its entry before writing it
+            for (int t = lane; t < 225; t += 32) {
+                const double v = info[i * 225 + t];
+                info_out[i * 225 + t] = w == 1.0 ? v : w * v;
+            }
+            if (lane < 15) {
+                const double v = rhs[i * 15 + lane];
+                rhs_out[i * 15 + lane] = w == 1.0 ? v : w * v;
+            }
+        }
+        if (lane == 0) f_out[i] = c;                               // f_out may alias f: lane 0 read f[i] above
+    }
+}
+
+cudaError_t state_priors_robust_launch(int64_t n, const int32_t* loss, const double* loss_k, const double* info, const double* rhs,
+                                       const double* f, double* info_out, double* rhs_out, double* f_out, cudaStream_t st) {
+    const int64_t grid = std::min<int64_t>((n + 3) / 4, 0x7fffffff);
+    if (grid < 1) return cudaSuccess;
+    k_state_prior_robust<<<(int)grid, 128, 0, st>>>(n, loss, loss_k, info, rhs, f, info_out, rhs_out, f_out);
     return cudaGetLastError();
 }
 

@@ -15,7 +15,7 @@ import ctypes
 import numpy as np
 
 from . import capi
-from .capi import REC, REC_DOUBLES
+from .capi import LOSS_CAUCHY, LOSS_GAUSSIAN, REC, REC_DOUBLES
 
 
 def _ptr(a):
@@ -225,13 +225,35 @@ def chains_assemble(G11, G12, G22, g1, g2, chain_offsets, lam=0.0, prior_info=No
     return D, E[:N - 1], rhs
 
 
-def _state_priors(state_priors, N, dev, offs=None, S=0):
+def _loss_flags(code, k, rhs, f, measurement):
+    """The value checks of state_prior_loss as 0-d bool tensors, for the entry's one host read: a code outside {0, 1, 2}, a robust
+    prior whose k does not satisfy 0 < k^2 < inf, and (measurement) a robust prior with a nonzero rhs or f."""
+    import torch
+
+    robust = code != LOSS_GAUSSIAN
+    k2 = k * k
+    flags = [((code < LOSS_GAUSSIAN) | (code > LOSS_CAUCHY)).any(), (robust & ~((k > 0) & (k2 > 0) & torch.isfinite(k2))).any()]
+    if measurement:
+        nz = torch.zeros_like(robust)
+        if rhs is not None:
+            nz = nz | (rhs.reshape(code.numel(), 15) != 0).any(dim=1)
+        if f is not None:
+            nz = nz | (f.reshape(code.numel()) != 0)
+        flags.append((robust & nz).any())
+    return flags
+
+
+def _state_priors(state_priors, N, dev, offs=None, S=0, loss=None, measurement=True):
     """Validated state priors (state_idx [M] int64, info [M,225], rhs [M,15] | None, f [M] | None, lin [M,16]) on N states: returns
-    (idx, info, rhs (zeros if None), f or None, lin, single) with single whether a chain of one state carries a prior, or None for
-    state_priors None or M = 0.  Checks shapes and dtypes, then 0 <= state_idx < N (the one host read), then the device."""
+    (idx, info, rhs (zeros if None), f or None, lin, single, loss) with single whether a chain of one state carries a prior, or None
+    for state_priors None or M = 0.  loss: state_prior_loss, (code [M] int32, k [M] float64) or None, returned as given.  Checks
+    shapes and dtypes, then 0 <= state_idx < N and the loss values (the one host read), then the device.  measurement: a robust prior
+    must have rhs and f None or zero (chain_marginalize takes them moved, and skips that check)."""
     import torch
 
     if state_priors is None:
+        if loss is not None:
+            raise ValueError("state_prior_loss needs state_priors")
         return None
     if not isinstance(state_priors, (tuple, list)) or len(state_priors) != 5:
         raise ValueError("state_priors is (state_idx [M], info [M,225], rhs [M,15] or None, f [M] or None, lin [M,16])")
@@ -246,14 +268,35 @@ def _state_priors(state_priors, N, dev, offs=None, S=0):
             raise ValueError(f"state_priors: {name} must be a float64 tensor")
         if t.numel() != k * M or t.dim() < 1 or t.shape[0] != M:
             raise ValueError(f"state_priors: {name} needs {k} doubles for each of the {M} priors")
+    if loss is not None:
+        if not isinstance(loss, (tuple, list)) or len(loss) != 2:
+            raise ValueError("state_prior_loss is (loss [M] int32, loss_k [M] float64)")
+        code, lk = loss
+        if not isinstance(code, torch.Tensor) or code.dtype != torch.int32 or code.dim() != 1 or code.numel() != M:
+            raise ValueError(f"state_prior_loss: loss must be a 1-d int32 tensor with one code for each of the {M} priors")
+        if not isinstance(lk, torch.Tensor) or lk.dtype != torch.float64 or lk.dim() != 1 or lk.numel() != M:
+            raise ValueError(f"state_prior_loss: loss_k must be a 1-d float64 tensor with one threshold for each of the {M} priors")
+        if code.device != idx.device or lk.device != idx.device:
+            raise ValueError("state_prior_loss: loss and loss_k must be on the device of state_idx")
     if M:
         flags = [((idx < 0) | (idx >= N)).any()]
         if offs is not None and idx.device == offs.device:         # a chain of one state carrying a prior: the chain prior is its target
             c = (torch.searchsorted(offs, idx.clamp(0, max(N - 1, 0)), right=True) - 1).clamp(0, offs.numel() - 2)
             flags.append(((offs[c + 1] - offs[c]) == 1).any())
+        else:
+            flags.append(torch.zeros((), dtype=torch.bool, device=idx.device))
+        if loss is not None:
+            flags += _loss_flags(code, lk, rhs, f, measurement)
         flags = torch.stack(flags).tolist()
         if flags[0]:
             raise IndexError(f"state_priors: state_idx out of range [0, {N})")
+        if loss is not None:
+            if flags[2]:
+                raise ValueError("state_prior_loss: loss codes are 0 (Gaussian), 1 (Huber) and 2 (Cauchy)")
+            if flags[3]:
+                raise ValueError("state_prior_loss: a Huber or Cauchy prior needs a threshold k with 0 < k^2 < inf")
+            if measurement and flags[4]:
+                raise ValueError("state_prior_loss: a Huber or Cauchy prior must be a measurement prior (rhs and f None or zero)")
     if not idx.is_cuda or idx.device != dev:
         raise ValueError(f"state_priors: state_idx must be a CUDA tensor on {dev}")
     _check_f64(dev, state_prior_info=info, state_prior_rhs=rhs, state_prior_f=f, state_prior_lin=lin)
@@ -261,7 +304,8 @@ def _state_priors(state_priors, N, dev, offs=None, S=0):
         return None
     single = bool(flags[1]) if offs is not None else S == 1
     rhs = torch.zeros((M, 15), dtype=torch.float64, device=dev) if rhs is None else rhs
-    return idx, info.reshape(M, 225), rhs.reshape(M, 15), None if f is None else f.reshape(M), lin.reshape(M, 16), single
+    return (idx, info.reshape(M, 225), rhs.reshape(M, 15), None if f is None else f.reshape(M), lin.reshape(M, 16), single,
+            None if loss is None else (code.contiguous(), lk.contiguous()))
 
 
 def _state_prior_csr(key, N):
@@ -300,22 +344,62 @@ def state_priors_fold(chain_offsets, sp_offsets, sp_info, sp_rhs, sp_f, G11=None
                                                          _tptr(prior_rhs), _tptr(prior_f), ctypes.c_void_p(st.cuda_stream)))
 
 
-def chain_marginalize(G11, G12, G22, g1, g2, f, chain_offsets, n_marg, prior=None, n_chains=None, stream=None, state_priors=None):
+def state_priors_robust(loss, loss_k, info, rhs, f, info_out=None, rhs_out=None, f_out=None, stream=None):
+    """Robust (Huber / Cauchy) reweighting of moved measurement priors (cpi_imu_state_priors_robust; include/cpi_b200.h, DESIGN.md
+    section 3h): with s = f, (info, rhs, f) -> (w(s) info, w(s) rhs, c(s)) per prior.  loss: device int32 [M] (capi.LOSS_*); loss_k:
+    float64 [M] (thresholds in standard deviations); info [M,225] / rhs [M,15]: both or None (None: the f-only pass); f [M] the moved
+    f' = s.  Outputs are allocated where None (rhs_out may be rhs, f_out may be f).  Returns (info_out, rhs_out, f_out), the first two
+    None for the f-only pass."""
+    import torch
+
+    dev = f.device
+    _check_f64(dev, loss_k=loss_k, info=info, rhs=rhs, f=f, info_out=info_out, rhs_out=rhs_out, f_out=f_out)
+    M = f.numel()
+    if not loss.is_cuda or loss.device != dev or loss.dtype != torch.int32 or loss.numel() != M or loss_k.numel() != M:
+        raise ValueError(f"loss must be an int32 CUDA tensor on {dev} and loss_k float64, one entry per prior")
+    if (info is None) != (rhs is None):
+        raise ValueError("info and rhs must both be given or both be None")
+    if info is not None and (info.numel() != 225 * M or rhs.numel() != 15 * M):
+        raise ValueError("info needs 225 doubles and rhs 15 per prior")
+    for t in (info_out, rhs_out, f_out):
+        if t is not None and not t.is_contiguous():
+            raise ValueError("the outputs must be contiguous")
+    if info is not None:
+        info_out = torch.empty((M, 225), dtype=torch.float64, device=dev) if info_out is None else info_out
+        rhs_out = torch.empty((M, 15), dtype=torch.float64, device=dev) if rhs_out is None else rhs_out
+    else:
+        info_out = rhs_out = None
+    f_out = torch.empty(M, dtype=torch.float64, device=dev) if f_out is None else f_out
+    c = lambda t: None if t is None else t.contiguous()
+    with torch.cuda.device(dev):
+        st = stream if stream is not None else torch.cuda.current_stream(dev)
+        capi.check(capi.load().cpi_imu_state_priors_robust(M, _tptr(loss.contiguous()), _tptr(loss_k.contiguous()), _tptr(c(info)), _tptr(c(rhs)),
+                                                           _tptr(f.contiguous()), _tptr(info_out), _tptr(rhs_out), _tptr(f_out),
+                                                           ctypes.c_void_p(st.cuda_stream)))
+    return info_out, rhs_out, f_out
+
+
+def chain_marginalize(G11, G12, G22, g1, g2, f, chain_offsets, n_marg, prior=None, n_chains=None, stream=None, state_priors=None,
+                      state_prior_loss=None):
     """Eliminate the first n_marg states of every chain into a dense prior on the first state it keeps (cpi_imu_chain_marginalize,
     kernel K8): the Schur complement a fixed-lag smoother keeps of the states that leave its window, at the linearisation point of the
     blocks, undamped.  Blocks as factor_hessian returns them (chain layout as chains_assemble); n_marg: int or device int64 [n_chains]
     (0 <= n_marg < states of the chain); prior: (info [n_chains,225], rhs [n_chains,15], f [n_chains]) on every chain's first state, or
     None.  state_priors: as chains_lm_step, taken as given at the blocks' linearisation point; only those on eliminated states
     (state_idx < offsets[c] + n_marg[c]) are folded, into copies of G11 / g1 / f, so a prior on a kept state is left to the caller.
+    state_prior_loss: as chains_lm_step; a robust prior is given moved, (W, rhs', f') with f' = s, and enters with its weight frozen
+    at the blocks' linearisation point (state_priors_robust before the fold; f must then be given).
     Returns the prior on state offsets[c] + n_marg[c]: (info [n_chains,225] exactly symmetric, rhs [n_chains,15], f [n_chains])."""
     import torch
 
     dev = G11.device
     nf = G11.numel() // 225
     sp = None
-    if state_priors is not None:
+    if state_priors is not None or state_prior_loss is not None:
         C, offs, S = _chain_layout(chain_offsets, dev, n_factors=nf, n_chains=n_chains)
-        sp = _state_priors(state_priors, nf + C, dev)
+        if state_prior_loss is not None and state_priors is not None and len(state_priors) == 5 and state_priors[3] is None:
+            raise ValueError("state_prior_loss: chain_marginalize takes the priors moved, and a robust prior's f' is its s: f must be given")
+        sp = _state_priors(state_priors, nf + C, dev, loss=state_prior_loss, measurement=False)
     _check_f64(dev, G11=G11, G12=G12, G22=G22, g1=g1, g2=g2, f=f)
     C, offs, S = _chain_layout(chain_offsets, dev, n_factors=nf, n_chains=n_chains)
     if any(t.numel() != k * nf for t, k in ((G11, 225), (G12, 225), (G22, 225), (g1, 15), (g2, 15), (f, 1))):
@@ -334,7 +418,7 @@ def chain_marginalize(G11, G12, G22, g1, g2, f, chain_offsets, n_marg, prior=Non
     else:
         nm, nmu = None, int(n_marg)
     if sp is not None:                                               # eliminated states are never last: their priors land in G11 / g1 / f
-        idx, s_info, s_rhs, s_f, _, _ = sp
+        idx, s_info, s_rhs, s_f, _, _, s_loss = sp
         if offs is not None:
             c = (torch.searchsorted(offs, idx, right=True) - 1).clamp(0, C - 1)
             head = offs[c]
@@ -343,9 +427,11 @@ def chain_marginalize(G11, G12, G22, g1, g2, f, chain_offsets, n_marg, prior=Non
             head = c * S
         head = head + (nm[c] if nm is not None else nmu)
         order, sp_off = _state_prior_csr(torch.where(idx < head, idx, idx + nf + C), nf + C)
+        s_info, s_rhs, s_f = s_info[order], s_rhs[order], None if s_f is None else s_f[order]
+        if s_loss is not None:                                       # the weights frozen at the blocks' point (s = the given f')
+            s_info, s_rhs, s_f = state_priors_robust(s_loss[0][order], s_loss[1][order], s_info, s_rhs, s_f, stream=stream)
         G11, g1, f = G11.contiguous().clone(), g1.contiguous().clone(), f.contiguous().clone()
-        state_priors_fold(offs if offs is not None else S, sp_off, s_info[order], s_rhs[order], None if s_f is None else s_f[order],
-                          G11=G11, g1=g1, f=f, n_chains=C, stream=stream)
+        state_priors_fold(offs if offs is not None else S, sp_off, s_info, s_rhs, s_f, G11=G11, g1=g1, f=f, n_chains=C, stream=stream)
     info = torch.empty((C, 225), dtype=torch.float64, device=dev)
     rhs = torch.empty((C, 15), dtype=torch.float64, device=dev)
     fo = torch.empty((C,), dtype=torch.float64, device=dev)
@@ -379,7 +465,8 @@ def prior_at(info, rhs, f, lin_states, states, stream=None):
     return rhs_out, f_out
 
 
-def chains_lm_step(model, states, records, lin, chain_offsets, prior=None, lam=1e-5, diagonal_damping=True, stream=None, state_priors=None):
+def chains_lm_step(model, states, records, lin, chain_offsets, prior=None, lam=1e-5, diagonal_damping=True, stream=None, state_priors=None,
+                   state_prior_loss=None):
     """One damped Gauss-Newton step of many independent IMU-only chains at once (a fixed-lag smoother's windows), on the device:
     evaluateError -> information blocks -> prior_at (every chain's prior moved to its current first state) -> chains_assemble ->
     ONE block-cyclic-reduction solve over all chains -> retract.  states [N,16]; records / lin: the N - n_chains factors, chain c's
@@ -388,6 +475,9 @@ def chains_lm_step(model, states, records, lin, chain_offsets, prior=None, lam=1
     linearised at the chains' current first states, so it is used as given without prior_at (rhs and f may then be None: zero).
     state_priors: priors on any states, (state_idx [M] int64, info [M,225], rhs [M,15] or None, f [M] or None, lin [M,16]) or None
     (include/cpi_b200.h, DESIGN.md section 3g): moved to the states by prior_at and folded into the blocks (state_priors_fold).
+    state_prior_loss: (loss [M] int32 capi.LOSS_*, loss_k [M] float64) aligned with state_priors, or None (DESIGN.md section 3h): a
+    Huber or Cauchy prior (a measurement prior: rhs and f None or zero) is reweighted at the states (state_priors_robust) before the
+    fold and costs c(s).
     Returns (new_states, delta [N,15], cost per chain before the step [n_chains] = sum of e^T P^-1 e + the moved priors' f')."""
     import torch
 
@@ -397,7 +487,7 @@ def chains_lm_step(model, states, records, lin, chain_offsets, prior=None, lam=1
     nf = N - C
     if records.numel() != REC_DOUBLES[model] * nf:
         raise ValueError(f"{C} chains over {N} states hold {nf} factors: one record each")
-    sp = _state_priors(state_priors, N, dev, offs, S)
+    sp = _state_priors(state_priors, N, dev, offs, S, loss=state_prior_loss)
     idx_i = idx_j = chain_of = None
     if C > 1:                                                        # one chain: the eval kernel's own chain indexing
         ar = torch.arange(nf, dtype=torch.int64, device=dev)
@@ -416,11 +506,13 @@ def chains_lm_step(model, states, records, lin, chain_offsets, prior=None, lam=1
             first = states.reshape(N, 16)[offs[:-1]] if offs is not None else states.reshape(N, 16)[::S]
             pr, pf = prior_at(pi, pr, pf, lin0, first, stream=stream)
     if sp is not None:
-        idx, s_info, s_rhs, s_f, s_lin, single = sp
+        idx, s_info, s_rhs, s_f, s_lin, single, s_loss = sp
         order, sp_off = _state_prior_csr(idx, N)
         s_info, s_lin, idx = s_info[order], s_lin[order], idx[order]
         r_m, f_m = prior_at(s_info, s_rhs[order], None if s_f is None else s_f[order], s_lin, states.reshape(N, 16).index_select(0, idx),
                             stream=stream)
+        if s_loss is not None:                                       # reweighted at the states: (w W, w rhs', c(s))
+            s_info, _, _ = state_priors_robust(s_loss[0][order], s_loss[1][order], s_info, r_m, f_m, rhs_out=r_m, f_out=f_m, stream=stream)
         if single:                                                   # the chain prior receives priors: fold into copies (zeros without one)
             z = lambda t, *shape: torch.zeros(shape, dtype=torch.float64, device=dev) if t is None else t.contiguous().clone()
             pi, pr, pf = z(pi, C, 225), z(pr, C, 15), z(pf, C)
@@ -533,7 +625,7 @@ def chains_solve(D, E, rhs, chain_offsets, n_chains=None, workspace=None, stream
 
 
 def chains_lm(model, states, records, lin, chain_offsets, prior=None, lam=1e-5, diagonal_damping=True, params=None, max_rounds=200, check_every=8,
-              stream=None, state_priors=None):
+              stream=None, state_priors=None, state_prior_loss=None):
     """Levenberg-Marquardt of many independent IMU-only chains at once, to convergence, on the device (GTSAM's
     LevenbergMarquardtOptimizer rule per chain: include/cpi_b200.h, DESIGN.md section 3f).  Arguments as chains_lm_step; lam: the
     initial lambda of every chain; params: capi.LMParams (None: GTSAM's defaults).  A prior without a linearisation point is taken as
@@ -541,16 +633,18 @@ def chains_lm(model, states, records, lin, chain_offsets, prior=None, lam=1e-5, 
     -> chains_solve (chains isolated) -> retract -> factor_cost + prior_at at the candidate -> cpi_imu_chains_lm_update.  No host
     synchronisation inside the loop except one 4-byte "any chain running" read every check_every rounds (0: max_rounds rounds, fully
     asynchronous).  state_priors as chains_lm_step: every round moves them to the current states after the information blocks and
-    folds them in (state_priors_fold), and folds their f' at the candidate into its cost.  Returns (states [N,16], cost [C] at them,
+    folds them in (state_priors_fold), and folds their f' at the candidate into its cost.  state_prior_loss as chains_lm_step: the
+    robust priors are reweighted at every round's states before the fold (the weighted info goes to a buffer of the call; the given
+    info is constant), and their cost c(s) at the candidate goes into its cost.  Returns (states [N,16], cost [C] at them,
     lam [C], status [C] int32 (capi.LM_*), iterations [C] (accepted steps), tries [C] (rounds the chain ran)), all int32 counters."""
     import torch
 
     lib = capi.load()
     dev = states.device
     N = states.numel() // 16
-    if state_priors is not None:
+    if state_priors is not None or state_prior_loss is not None:
         C, offs, S = _chain_layout(chain_offsets, dev, n_states=N)
-        sp = _state_priors(state_priors, N, dev, offs, S)
+        sp = _state_priors(state_priors, N, dev, offs, S, loss=state_prior_loss)
     else:
         sp = None
     _check_f64(dev, states=states, records=records, lin=lin)
@@ -583,14 +677,18 @@ def chains_lm(model, states, records, lin, chain_offsets, prior=None, lam=1e-5, 
         pr = torch.zeros((C, 15), **f64) if pr is None else pr.contiguous()
         pf = torch.zeros(C, **f64) if pf is None else pf.contiguous()
         lin0 = X.index_select(0, first) if lin0 is None else lin0.contiguous()
-    use_prior, single, s_lin = prior is not None, False, None
+    use_prior, single, s_lin, s_loss = prior is not None, False, None, None
     if sp is not None:
-        s_idx, s_info, s_rhs, s_f, s_lin, single = sp
+        s_idx, s_info, s_rhs, s_f, s_lin, single, s_loss = sp
         order, sp_off = _state_prior_csr(s_idx, N)
         s_idx, s_info, s_rhs, s_lin = s_idx[order], s_info[order].contiguous(), s_rhs[order].contiguous(), s_lin[order].contiguous()
         s_f = None if s_f is None else s_f[order].contiguous()
         M = s_idx.numel()
         s_x, s_r, s_fc, s_fn = torch.empty((M, 16), **f64), torch.empty((M, 15), **f64), torch.empty(M, **f64), torch.empty(M, **f64)
+        s_iw = s_info                                                # the info the fold reads: the round's weighted copy under a loss
+        if s_loss is not None:
+            s_code, s_k = s_loss[0][order].contiguous(), s_loss[1][order].contiguous()
+            s_iw = torch.empty((M, 225), **f64)
         if single and not use_prior:                                 # a chain of one state carries priors: a zero chain prior receives them
             pi, pr, pf, lin0 = torch.zeros((C, 225), **f64), torch.zeros((C, 15), **f64), torch.zeros(C, **f64), X.index_select(0, first)
             use_prior = True
@@ -626,9 +724,11 @@ def chains_lm(model, states, records, lin, chain_offsets, prior=None, lam=1e-5, 
                 if s_lin is not None:                                # the state priors at X, folded into this round's blocks
                     torch.index_select(X, 0, s_idx, out=s_x)
                     capi.check(lib.cpi_imu_prior_at(M, p(s_info), p(s_rhs), p(s_f), p(s_lin), p(s_x), p(s_r), p(s_fc), sp))
+                    if s_loss is not None:                           # reweighted at X: (w W, w rhs', c(s))
+                        capi.check(lib.cpi_imu_state_priors_robust(M, p(s_code), p(s_k), p(s_info), p(s_r), p(s_fc), p(s_iw), p(s_r), p(s_fc), sp))
                     if single:
                         pi_r.copy_(pi)
-                    capi.check(lib.cpi_imu_state_priors_fold(C, p(offs), S, p(sp_off), p(s_info), p(s_r), p(s_fc), p(G11), p(G22), p(g1), p(g2),
+                    capi.check(lib.cpi_imu_state_priors_fold(C, p(offs), S, p(sp_off), p(s_iw), p(s_r), p(s_fc), p(G11), p(G22), p(g1), p(g2),
                                                              p(f_cur), p(pi_r), p(pr_c if single else None), p(pf_c if single else None), sp))
                 capi.check(lib.cpi_imu_chains_assemble_lm(C, p(offs), S, p(G11), p(G12), p(G22), p(g1), p(g2), p(lam_t), int(bool(diagonal_damping)),
                                                           p(pi_r if single else pi), p(pr_c if use_prior else None), p(D), p(E), p(rhs), p(damp), sp))
@@ -642,6 +742,8 @@ def chains_lm(model, states, records, lin, chain_offsets, prior=None, lam=1e-5, 
                 if s_lin is not None:                                # their f' at the candidate, into its cost
                     torch.index_select(Xn, 0, s_idx, out=s_x)
                     capi.check(lib.cpi_imu_prior_at(M, p(s_info), p(s_rhs), p(s_f), p(s_lin), p(s_x), p(s_r), p(s_fn), sp))
+                    if s_loss is not None:                           # c(s) at the candidate
+                        capi.check(lib.cpi_imu_state_priors_robust(M, p(s_code), p(s_k), None, None, p(s_fn), None, None, p(s_fn), sp))
                     capi.check(lib.cpi_imu_state_priors_fold(C, p(offs), S, p(sp_off), None, None, p(s_fn), None, None, None, None, p(f_new), None,
                                                              None, p(pf_n if single else None), sp))
                 if check:

@@ -413,6 +413,36 @@ int cpi_imu_state_priors_fold(int64_t n_chains, const int64_t* chain_offsets, in
                               const double* sp_info, const double* sp_rhs, const double* sp_f, double* G11, double* G22, double* g1,
                               double* g2, double* f, double* prior_info, double* prior_rhs, double* prior_f, void* stream);
 
+/*
+ * Robust losses on state priors (DESIGN.md section 3h): GTSAM's noiseModel::Robust (Huber, Cauchy) around a prior's noise model, so
+ * that an outlying fix (GNSS multipath, a false zero-velocity detection, a bad anchor) pulls with a bounded or vanishing weight
+ * instead of quadratically.  fp64, DEVICE pointers, asynchronous on `stream`, no allocation.  PARITY UNPINNED; tests/test_robust_priors.py
+ * holds the numpy statement.
+ *
+ * A robust prior must be a MEASUREMENT prior (rhs = 0, f = 0): after cpi_imu_prior_at its f' is s = delta^T W delta, the whitened
+ * squared residual.  A prior with a nonzero rhs or f (a marginal prior, for example) has no residual to robustify.  With the library's
+ * cost convention (a Gaussian prior costs s, twice GTSAM's error) a robust prior costs c(s) = 2 rho(sqrt s), rho GTSAM's mEstimator
+ * residual, and enters the linear system with the IRLS weight w(s) = dc/ds (what noiseModel::Robust::WhitenSystem applies):
+ *     CPI_LOSS_GAUSSIAN   c = s                                            w = 1
+ *     CPI_LOSS_HUBER, k   c = s if s <= k^2, else 2 k sqrt(s) - k^2        w = 1 if s <= k^2, else k / sqrt(s)
+ *     CPI_LOSS_CAUCHY, k  c = k^2 log1p(s / k^2)                           w = 1 / (1 + s / k^2)
+ * k is in whitened units (standard deviations); it must satisfy 0 < k^2 < inf, and is ignored for CPI_LOSS_GAUSSIAN.  A Gaussian prior
+ * and a Huber inlier are copied bit for bit.  An unknown code or an invalid k gives NaN weight and cost for that prior (its chain
+ * then ends CPI_LM_NONFINITE in LM; no other prior is touched).
+ *
+ *   cpi_imu_state_priors_robust   (info, rhs, f) -> (w info, w rhs, c(s)) with s = f, per prior: info / rhs / f as cpi_imu_prior_at
+ *       leaves them (rhs', f').  loss: int32 [n], loss_k: double [n].  info_out / rhs_out: both or neither; neither is the f-only pass
+ *       (the candidate's cost in LM).  rhs_out may alias rhs and f_out may alias f; info_out receives the weighted info, so the
+ *       caller's info stays constant.  One warp per prior, no atomics: the same bits on every run.  Then cpi_imu_state_priors_fold
+ *       adds the weighted priors unchanged.  In LM the weight is recomputed at the states of every round; in marginalisation it is
+ *       frozen at the blocks' linearisation point, as GTSAM linearises a robust factor it marginalises.
+ */
+#define CPI_LOSS_GAUSSIAN        0
+#define CPI_LOSS_HUBER           1
+#define CPI_LOSS_CAUCHY          2
+int cpi_imu_state_priors_robust(int64_t n, const int32_t* loss, const double* loss_k, const double* info, const double* rhs, const double* f,
+                                double* info_out, double* rhs_out, double* f_out, void* stream);
+
 /* ---- callers either side of the factor ("next" rows) ----------------------------------------------------------------- */
 
 /* x_{k+1} prediction from x_k and a record: getpredictedstate_v1/_v2 (GraphSolver_IMU.cpp:263-307).
