@@ -37,6 +37,7 @@ SYMBOLS = {
     "cpi_imu_chain_marginalize": (c_int, [c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "cpi_imu_prior_at": (c_int, [c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "cpi_imu_factor_cost_batch": (c_int, [c_int, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "cpi_imu_chains_cost_sum": (c_int, [c_i64, c_vp, c_i64, c_vp, c_vp, c_vp]),
     "cpi_imu_chains_assemble_lm": (c_int, [c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "cpi_imu_chains_solve_workspace": (c_i64, [c_i64, c_i64]),
     "cpi_imu_chains_solve": (c_int, [c_i64, c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),

@@ -496,6 +496,16 @@ int cpi_imu_factor_cost_batch(int model, int64_t n_factors, const double* states
     return CPI_OK;
 }
 
+int cpi_imu_chains_cost_sum(int64_t n_chains, const int64_t* chain_offsets, int64_t chain_uniform, const double* f, double* cost, void* stream) {
+    if (n_chains < 0) return fail(CPI_EINVAL, "negative count");
+    if (n_chains == 0) return CPI_OK;
+    if (!chain_offsets && chain_uniform < 1) return fail(CPI_EINVAL, "chain_uniform must be >= 1 without chain_offsets");
+    if (!f || !cost) return fail(CPI_EINVAL, "null pointer argument");
+    CU(cpi::chains_cost_sum_launch(n_chains, chain_offsets, chain_offsets ? 0 : chain_uniform, f, cost, (cudaStream_t)stream));
+    g_launches += 1;
+    return CPI_OK;
+}
+
 int cpi_imu_chains_assemble_lm(int64_t n_chains, const int64_t* chain_offsets, int64_t chain_uniform, const double* G11, const double* G12,
                                const double* G22, const double* g1, const double* g2, const double* lambda, int diagonal_damping,
                                const double* prior_info, const double* prior_rhs, double* D, double* E, double* rhs, double* damp, void* stream) {

@@ -89,6 +89,7 @@ cudaError_t prior_at_launch(int64_t n, const double* info, const double* rhs, co
 // lm.cu: the factor cost (K9) and the per-chain Levenberg-Marquardt decision
 cudaError_t factor_cost_launch(int model, int64_t n, const double* states, const int64_t* idx_i, const int64_t* idx_j, const double* records,
                                const double* lin, double* f, cudaStream_t st);
+cudaError_t chains_cost_sum_launch(int64_t n_chains, const int64_t* offs, int64_t uniform, const double* f, double* cost, cudaStream_t st);
 int64_t lm_workspace_bytes(int64_t n_states);
 cudaError_t lm_update_launch(int64_t n_chains, const int64_t* offs, int64_t uniform, int64_t n_states, const cpi_lm_params& p, const double* f_cur,
                              const double* pf_cur, const double* f_new, const double* pf_new, const double* rhs, const double* D, const double* E,

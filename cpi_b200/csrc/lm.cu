@@ -207,6 +207,20 @@ __global__ void __launch_bounds__(128) k_lm_decide(int64_t n_chains, const int64
         for (int64_t t = lo * CPI_STATE_DOUBLES + threadIdx.x; t < hi * CPI_STATE_DOUBLES; t += blockDim.x) states[t] = states_new[t];
 }
 
+// cost[c] = the sum of f over chain c's factors (factor index offs[c] - c .. offs[c + 1] - c - 1, or (S - 1) per chain): one warp per
+// chain, each lane sums its strided share in index order, then a fixed shuffle tree -- no atomics, the same bits on every run.
+__global__ void __launch_bounds__(128) k_chains_cost_sum(int64_t n_chains, const int64_t* offs, int64_t uniform, const double* f, double* cost) {
+    const int lane = threadIdx.x & 31;
+    const int64_t c = (int64_t)blockIdx.x * 4 + (threadIdx.x >> 5);
+    if (c >= n_chains) return;
+    const int64_t lo = offs ? offs[c] - c : c * (uniform - 1), hi = offs ? offs[c + 1] - c - 1 : lo + uniform - 1;
+    double s = 0.0;
+    for (int64_t j = lo + lane; j < hi; j += 32) s += f[j];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (lane == 0) cost[c] = s;
+}
+
 // ---- launchers ----------------------------------------------------------------------------------------------------------------------
 cudaError_t factor_cost_launch(int model, int64_t n, const double* states, const int64_t* idx_i, const int64_t* idx_j, const double* records,
                                const double* lin, double* f, cudaStream_t st) {
@@ -214,6 +228,12 @@ cudaError_t factor_cost_launch(int model, int64_t n, const double* states, const
     const int grid = (int)((n + 3) / 4);
     if (model == 1) k_factor_cost<1><<<grid, 128, 0, st>>>(n, states, idx_i, idx_j, records, lin, f);
     else k_factor_cost<2><<<grid, 128, 0, st>>>(n, states, idx_i, idx_j, records, lin, f);
+    return cudaGetLastError();
+}
+
+cudaError_t chains_cost_sum_launch(int64_t n_chains, const int64_t* offs, int64_t uniform, const double* f, double* cost, cudaStream_t st) {
+    if (n_chains == 0) return cudaSuccess;
+    k_chains_cost_sum<<<(int)((n_chains + 3) / 4), 128, 0, st>>>(n_chains, offs, uniform, f, cost);
     return cudaGetLastError();
 }
 

@@ -521,8 +521,16 @@ def chains_lm_step(model, states, records, lin, chain_offsets, prior=None, lam=1
                           stream=stream)
     D, E, rhs = chains_assemble(G11, G12, G22, g1, g2, chain_offsets, lam, pi, pr, diagonal_damping=diagonal_damping, n_chains=C, stream=stream)
     dx = chain_solve(D, E, rhs, stream=stream)
-    # per-chain cost: one chain sums like chain_lm_step always has; many chains scatter-add their factors' f
-    cost = f.sum().reshape(1) if C == 1 else torch.zeros(C, dtype=torch.float64, device=dev).index_add_(0, chain_of, f)
+    # per-chain cost: one chain sums like chain_lm_step always has; many chains sum their factors' f in a fixed order
+    # (cpi_imu_chains_cost_sum: an atomic scatter-add would give different bits from run to run)
+    if C == 1:
+        cost = f.sum().reshape(1)
+    else:
+        cost = torch.empty(C, dtype=torch.float64, device=dev)
+        with torch.cuda.device(dev):
+            st = stream if stream is not None else torch.cuda.current_stream(dev)
+            capi.check(capi.load().cpi_imu_chains_cost_sum(C, _tptr(offs), S, _tptr(f), _tptr(cost),
+                                                           ctypes.c_void_p(st.cuda_stream)))
     if pf is not None:
         cost = cost + pf
     return retract(states, dx, stream=stream), dx, cost

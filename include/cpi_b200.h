@@ -337,6 +337,8 @@ int cpi_imu_chains_assemble(int64_t n_chains, const int64_t* chain_offsets, int6
  *   cpi_imu_factor_cost_batch    (K9) f = e^T P_meas^-1 e of n factors at the states (indexing as cpi_imu_factor_eval_batch): the
  *       residual of evaluateError and one Cholesky + forward substitution, no e / H written; bitwise cpi_imu_factor_hessian_batch's f.
  *       A factor whose P_meas is not positive definite gets NaN.
+ *   cpi_imu_chains_cost_sum      cost[c] = the sum of f (device double[n_states - n_chains], one per factor, chains back to back) over
+ *       chain c's factors, in a fixed order (no atomics: the same bits on every run).  Layout as cpi_imu_chains_assemble.
  *   cpi_imu_chains_assemble_lm   cpi_imu_chains_assemble with lambda[n_chains] (device) per chain; damp (device double[n_states*15],
  *       may be NULL) receives the diagonal the damping added.
  *   cpi_imu_chains_solve         the block cyclic reduction of cpi_imu_chain_solve over n_states = the layout's state count, with every
@@ -365,6 +367,7 @@ typedef struct cpi_lm_params {
 } cpi_lm_params;
 int cpi_imu_factor_cost_batch(int model, int64_t n_factors, const double* states, const int64_t* idx_i, const int64_t* idx_j,
                               const double* records, const double* lin, double* f, void* stream);
+int cpi_imu_chains_cost_sum(int64_t n_chains, const int64_t* chain_offsets, int64_t chain_uniform, const double* f, double* cost, void* stream);
 int cpi_imu_chains_assemble_lm(int64_t n_chains, const int64_t* chain_offsets, int64_t chain_uniform,
                                const double* G11, const double* G12, const double* G22, const double* g1, const double* g2,
                                const double* lambda, int diagonal_damping, const double* prior_info, const double* prior_rhs,

@@ -357,6 +357,31 @@ def test_first_round_is_chains_lm_step(cuda, oracle, model):
 
 
 @pytest.mark.gpu
+@pytest.mark.parametrize("ragged", [True, False])
+def test_chains_lm_step_cost_is_a_fixed_order_sum(cuda, oracle, ragged):
+    """chains_lm_step's cost per chain is the sum of its factors' f (K9 at the same states) to rounding, summed in a fixed order: the
+    same bits on every call (an atomic scatter-add differs from run to run in the last bits).  Single-state chains cost 0."""
+    from cpi_b200 import factor
+    torch = cuda
+    sizes = [1, 4, 9, 2, 30, 17, 64, 65, 1, 100] if ragged else [33] * 8
+    X, rec, L, offs, _, _ = make_problem(oracle, 1, sizes, 11)
+    a = (_dev(torch, X), _dev(torch, rec), _dev(torch, L))
+    layout = _dev(torch, offs) if ragged else 33
+    costs = [factor.chains_lm_step(1, *a, layout)[2].cpu().numpy() for _ in range(8)]
+    assert all(np.array_equal(c, costs[0]) for c in costs), "the per-chain cost changes from call to call"
+    C = len(sizes)
+    chain = np.repeat(np.arange(C), np.asarray(sizes) - 1)
+    ii = np.arange(len(chain)) + chain
+    f = factor.factor_cost(1, a[0], a[1], a[2], _dev(torch, ii), _dev(torch, ii + 1)).cpu().numpy()
+    assert np.all(np.isfinite(f))
+    for c in range(C):
+        fc = f[chain == c]
+        want = float(np.sum(fc.astype(np.longdouble)))
+        assert abs(costs[0][c] - want) <= 1e-15 * max(len(fc), 1) * np.sum(np.abs(fc)), (c, costs[0][c], want)
+    assert np.all(costs[0][np.asarray(sizes) == 1] == 0.0)
+
+
+@pytest.mark.gpu
 @pytest.mark.parametrize("model", [1, 2])
 def test_lm_matches_numpy(cuda, oracle, model):
     """About 40 ragged chains of 1-60 states, with and without priors, small and large perturbations: every chain's accept / reject

@@ -243,11 +243,11 @@ def test_fp32_storage_variant(cuda, oracle, model, flags):
     from parity import fp32_errors
     worst = fp32_errors(got, ref)
     print(model, flags, {k: f"{v:.1e}" for k, v in worst.items()})
-    # the imu_avg / analytic modes run on the round-1 lane-per-window kernels (float tile, float state): their P gate is the round-1 one
+    # the imu_avg / analytic modes run on the round-1 lane-per-window kernels (float covariance tile): their P gate is the round-1 one.
+    # Their Jacobian state is fp64 (rounded on output), so the Jacobians keep the 1.5e-7 of the other modes.
     legacy = bool(flags)
     for k, gate in FP32_GATES[model].items():
         g = gate if not (legacy and k in ("P", "P_block")) else 2e-4
-        g = g if not (legacy and model == 2 and k in ("J_q", "J_a", "J_b", "H_a", "H_b", "O_a", "O_b")) else 5e-6
         assert worst[k] <= g, (k, worst[k], g)
     P = g64[:, 65:290].reshape(n, 15, 15)
     assert np.array_equal(P, P.transpose(0, 2, 1)) and np.all(P[:, 0:6, 9:12] == 0)

@@ -8,9 +8,9 @@ fp64 computation is on that window (ill-conditioned windows: the small_w band, t
 K, and otherwise within K * floor of the truth.
 
 CPU tests: the extended oracle is pinned to the golden records and to the fp64 oracle; the gate passes the fp64 oracle's own
-records and fails each of three injected subtle errors.  GPU tests: the stress batch (tests/stress.py) through the device entry
-point, the host entry point, a continuation cut at ring / trio boundaries, and imu_avg on the round-1 kernels, models 1 and 2,
-fp64 and fp32.  Constants calibrated on one H100 80GB HBM3 (700 W power limit); DESIGN.md section 5 lists the measured worst ratios."""
+records (default and analytic mode) and fails each of four injected subtle errors.  GPU tests: the stress batch (tests/stress.py)
+through the device entry point, the host entry point, a continuation cut at ring / trio boundaries, imu_avg on the round-1
+kernels and model 2 with analytic Jacobians (with and without imu_avg, device and host entry), models 1 and 2, fp64 and fp32.  Constants calibrated on one H100 80GB HBM3 (700 W power limit); DESIGN.md section 5 lists the measured worst ratios."""
 import os
 import subprocess
 
@@ -18,7 +18,7 @@ import numpy as np
 import pytest
 
 import stress
-from parity import compare_records, conditioned_gate, field_errors, imu_avg_inputs, window_band
+from parity import REC, compare_records, conditioned_gate, field_errors, imu_avg_inputs, window_band
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SIGMAS = np.array([0.005, 4e-6, 0.01, 0.0002])
@@ -35,7 +35,12 @@ K64, FLOOR64 = 8.0, 1e-15
 K32 = 8.0
 U32 = 2.0 ** -24
 COND32 = 2.0 ** 29
-FP32_ALLOW = dict(device=(U32, 1e-6, 2e-11), host=(U32, 1e-6, 2e-11), cont=(4 * U32, 1e-6, 2e-11), avg=(4e-6, 2e-5, 5e-8))
+# Model 2 with analytic Jacobians runs on the round-1 kernels too, but keeps R, alpha, beta and the Jacobian state in fp64 (only
+# the P tile and its stage slots are float): the output rounding on means and Jacobians, the round-1 allowance on P.
+FP32_ALLOW = dict(device=(U32, 1e-6, 2e-11), host=(U32, 1e-6, 2e-11), cont=(4 * U32, 1e-6, 2e-11), avg=(4e-6, 2e-5, 5e-8),
+                  ana=(U32, 2e-5, 5e-8), ana_avg=(U32, 2e-5, 5e-8))
+# (model 2) flags of each path; "ana" / "ana_avg" are model 2 with CPI_FLAG_ANALYTIC_JACOBIANS (state_transition_jacobians = False)
+PATH_FLAGS = dict(device=0, host=0, cont=0, avg=1, ana=2, ana_avg=3)
 
 
 @pytest.fixture(scope="session")
@@ -191,6 +196,35 @@ def test_gate_fails_a_J_a_column_perturbation_in_a_band_window(stress_cpu):
     assert any(b.startswith("J_a") for b in bad), bad
 
 
+@pytest.fixture(scope="module")
+def stress_cpu_ana(oracle, oracle_ld):
+    """Model 2 with analytic Jacobians on the stress batch without the long windows, with both oracles."""
+    S, off, L, tags = stress.make_batch(n_long=0)
+    a = oracle.preintegrate(2, S, L, SIGMAS, 2, offsets=off, nthreads=_threads())
+    b = oracle_ld.preintegrate(2, S, L, SIGMAS, 2, offsets=off, nthreads=_threads())
+    return S, off, L, tags, a, b
+
+
+@pytest.mark.parametrize("field", ["O_a", "O_b"])
+def test_gate_fails_one_analytic_O_element_rounded_to_fp32(stress_cpu_ana, field):
+    """Analytic mode: the fp64 oracle passes the gate; one element of O_a or O_b rounded to fp32, where the rounding is below the
+    north-star 1e-9 of the field (compare_records passes it), fails it."""
+    S, off, L, tags, o64, truth = stress_cpu_ana
+    _, _, bad = gate(2, np.float64, "device", o64, o64, truth, np.diff(off))
+    assert not bad, bad
+    a, b = REC[field]
+    O = o64[:, a:b]
+    d = np.abs(O.astype(np.float32).astype(np.float64) - O) / np.maximum(np.linalg.norm(O, axis=1, keepdims=True), 1e-300)
+    d[d >= 5e-10] = 0.0                                              # keep it under the north-star gate
+    i, j = np.unravel_index(int(np.argmax(d)), d.shape)
+    assert d[i, j] > 1e-12
+    rec = o64.copy()
+    rec[i, a + j] = np.float32(rec[i, a + j])
+    compare_records(rec[i:i + 1], o64[i:i + 1], 2, in_band=window_band(S, off, L)[i:i + 1])
+    _, _, bad = gate(2, np.float64, "device", rec, o64, truth, np.diff(off))
+    assert any(x.startswith(field) for x in bad), bad
+
+
 # ---------------------------------------------------------------------------------------------------------- GPU
 
 @pytest.fixture(scope="module")
@@ -211,40 +245,49 @@ def _oracles(oracle, oracle_ld, model, dtype, flags, S, off, L):
     return _truth_cache[key]
 
 
-def _run_path(torch, preint, model, path, Sx, Lx, off):
+def _run_path(torch, preint, model, path, Sx, Lx, off, flags=0):
     d = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()
-    if path == "device":
-        out = preint.preintegrate(model, d(Sx), d(Lx), SIGMAS, 0, offsets=d(off))
-    elif path == "host":
-        return preint.preintegrate_host(model, Sx, Lx, SIGMAS, 0, offsets=off)
-    elif path == "cont":
+    if flags & 1:
+        Sx, off = imu_avg_inputs(Sx, off)
+    if path == "host":
+        return preint.preintegrate_host(model, Sx, Lx, SIGMAS, flags, offsets=off)
+    if path == "cont":
         SA, oa, SB, ob = stress.split_for_continuation(Sx, off)
-        out = preint.preintegrate(model, d(SA), d(Lx), SIGMAS, 0, offsets=d(oa))
-        out = preint.preintegrate(model, d(SB), d(Lx), SIGMAS, 0, offsets=d(ob), continue_records=out)
+        out = preint.preintegrate(model, d(SA), d(Lx), SIGMAS, flags, offsets=d(oa))
+        out = preint.preintegrate(model, d(SB), d(Lx), SIGMAS, flags, offsets=d(ob), continue_records=out)
     else:
-        Sa, oa = imu_avg_inputs(Sx, off)
-        out = preint.preintegrate(model, d(Sa), d(Lx), SIGMAS, preint.FLAG_IMU_AVG, offsets=d(oa))
+        out = preint.preintegrate(model, d(Sx), d(Lx), SIGMAS, flags, offsets=d(off))
     torch.cuda.synchronize()
     return out.cpu().numpy()
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("path", ["device", "host", "cont", "avg"])
+@pytest.mark.parametrize("path", ["device", "host", "cont", "avg", "ana", "ana_avg"])
 @pytest.mark.parametrize("dtype", [np.float64, np.float32])
 @pytest.mark.parametrize("model", [1, 2])
 def test_kernels_against_extended_oracle(cuda, oracle, oracle_ld, stress_batch, model, dtype, path):
     """Every stress regime through one entry point, held to the conditioned gate.  fp32: inputs rounded to float, both oracles
-    run on the rounded inputs."""
+    run on the rounded inputs.  ana / ana_avg (model 2 with analytic Jacobians, without and with imu_avg): the device and the host
+    entry, which give the same bits; model 1 is always analytic, so there the flag is dropped and the record is the one without it,
+    bit for bit."""
     from cpi_b200 import preint
     S, off, L, tags = stress_batch
-    got = _run_path(cuda, preint, model, path, S.astype(dtype), L.astype(dtype), off)
+    Sx, Lx = S.astype(dtype), L.astype(dtype)
+    flags = PATH_FLAGS[path] if model == 2 or not path.startswith("ana") else PATH_FLAGS[path] & 1
+    entry = "host" if path == "host" else ("cont" if path == "cont" else "device")
+    got = _run_path(cuda, preint, model, entry, Sx, Lx, off, flags)
+    if path.startswith("ana"):
+        host = _run_path(cuda, preint, model, "host", Sx, Lx, off, PATH_FLAGS[path])
+        assert np.array_equal(host, got), "host and device entry differ"
+        dev = _run_path(cuda, preint, model, "device", Sx, Lx, off, PATH_FLAGS[path])
+        assert np.array_equal(dev, got), "the analytic flag changes the record"
     assert got.dtype == dtype
     P = got[:, 65:290].reshape(-1, 15, 15)
     assert np.array_equal(P, P.transpose(0, 2, 1)), "P is not exactly symmetric"
-    flags = 1 if path == "avg" else 0
     o64, truth = _oracles(oracle, oracle_ld, model, dtype, flags, S, off, L)
     steps = np.maximum(np.diff(off), 1)
-    ratio, worst, bad = gate(model, dtype, path, got, o64, truth, steps)
+    gpath = path if model == 2 or not path.startswith("ana") else ("avg" if flags & 1 else "device")
+    ratio, worst, bad = gate(model, dtype, gpath, got, o64, truth, steps)
     report(f"m{model} {np.dtype(dtype).name} {path}", ratio, tags)
     if dtype == np.float32:
         eP = np.max(np.stack([e for k, e in field_errors(got, truth, model).items() if k.startswith("P_")]), axis=0)

@@ -360,11 +360,7 @@ def test_no_loss_gaussian_codes_and_huber_inliers_are_bitwise_the_plain_calls(cu
         for l in losses:
             got = fn(1, *a, prior=dev_prior(torch, pri), state_priors=_sp_dev(torch, *sp), state_prior_loss=dl(l))
             what = (fn.__name__, None if l is None else int(l[0][0]))
-            if fn is factor.chains_lm_step:                            # its per-chain cost is an index_add_: the order of the sum varies
-                assert torch.equal(ref[0], got[0]) and torch.equal(ref[1], got[1]), what
-                assert np.all(_ulps(got[2].cpu().numpy(), ref[2].cpu().numpy()) <= 64), what
-            else:
-                assert all(torch.equal(u, v) for u, v in zip(ref, got)), what
+            assert all(torch.equal(u, v) for u, v in zip(ref, got)), what
     nm = _dev(torch, np.array([0, 2, 5, 1, 29, 3]))
     e, H1, H2 = factor.factor_eval(1, a[0], a[1], a[2], *_chain_idx(torch, offs))
     G = factor.factor_hessian(1, a[1], e, H1, H2)
