@@ -45,7 +45,10 @@ SYMBOLS = {
     "cpi_imu_chains_lm_update": (c_int, [c_i64, c_vp, c_i64, c_i64, c_vp] + [c_vp] * 19),
     "cpi_imu_state_priors_fold": (c_int, [c_i64, c_vp, c_i64] + [c_vp] * 13),
     "cpi_imu_state_priors_robust": (c_int, [c_i64] + [c_vp] * 9),
-    "cpi_predict_state_batch": (c_int, [c_int, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "cpi_imu_records_relinearize_workspace": (c_i64, [c_int, c_i64, c_i64]),
+    "cpi_imu_records_relinearize": (c_int, [c_int, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_int, ctypes.c_double, ctypes.c_double,
+                                            ctypes.c_double, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "cpi_predict_state_batch":(c_int, [c_int, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "cpi_propagate_batch": (c_int, [c_int, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "cpi_propagate_batch_host": (c_int, [c_int, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "cpi_retract_batch": (c_int, [c_i64, c_vp, c_vp, c_vp, c_vp]),

@@ -164,6 +164,55 @@ int cpi_preintegrate_batch_continue(int model, int dtype, int64_t n_windows, con
     return preintegrate_dev(model, dtype, n_windows, sample_offsets, ns_uniform, samples, lin, sigmas, flags, records, stream, 0, records);
 }
 
+int64_t cpi_imu_records_relinearize_workspace(int model, int64_t n_factors, int64_t n_entries) {
+    if (model != 1 && model != 2) return fail(CPI_EINVAL, "model must be 1 or 2 (got %d)", model);
+    if (n_factors < 0 || n_entries < 0) return fail(CPI_EINVAL, "negative count");
+    if (n_factors >= 2147483647 || n_entries > ((int64_t)1 << 56)) return fail(CPI_EINVAL, "count out of range");
+    return cpi::relin_workspace_bytes(cpi_record_doubles(model), n_factors, n_entries);
+}
+
+int cpi_imu_records_relinearize(int model, int64_t n_factors, const double* states, const int64_t* idx_i, const int64_t* sample_offsets,
+                                int64_t ns_uniform, const double* samples, const double* sigmas, int flags, double tol_bw, double tol_ba,
+                                double tol_theta, double* lin, double* records, int32_t* relinearized, int64_t* n_relinearized,
+                                void* workspace, void* stream) {
+    if (n_relinearized) *n_relinearized = 0;
+    if (model != 1 && model != 2) return fail(CPI_EINVAL, "model must be 1 or 2 (got %d)", model);
+    if (n_factors < 0 || (!sample_offsets && ns_uniform < 0)) return fail(CPI_EINVAL, "negative count");
+    if (n_factors >= 2147483647) return fail(CPI_EINVAL, "too many factors (%lld; at most 2^31 - 2 per call)", (long long)n_factors);
+    const double tols[3] = {tol_bw, tol_ba, tol_theta};
+    const char* names[3] = {"tol_bw", "tol_ba", "tol_theta"};
+    for (int t = 0; t < 3; t++)
+        if (!(tols[t] >= 0.0)) return fail(CPI_EINVAL, "%s must be >= 0 (+inf disables the test; got %g)", names[t], tols[t]);
+    if (n_factors == 0) return CPI_OK;
+    if (!states || !lin || !records || !sigmas) return fail(CPI_EINVAL, "null pointer argument (states / lin / records / sigmas)");
+    if (!workspace) return fail(CPI_EINVAL, "null pointer argument (workspace: cpi_imu_records_relinearize_workspace bytes)");
+    if ((uintptr_t)workspace & 15) return fail(CPI_EINVAL, "workspace must be 16-byte aligned");
+    const int64_t ent_uniform = ns_uniform + ((flags & CPI_FLAG_IMU_AVG) ? 1 : 0);
+    if (!samples && !sample_offsets && ent_uniform > 0) return fail(CPI_EINVAL, "samples is null");
+    DevInfo d;
+    int rc = device_info(d);
+    if (rc) return rc;
+    const int rd = cpi_record_doubles(model);
+    cudaStream_t st = (cudaStream_t)stream;
+    const cpi::RelinWorkspace w = cpi::relin_workspace(workspace, rd, n_factors);
+    CU(cpi::relin_select_launch(model, n_factors, states, idx_i, sample_offsets, ent_uniform, lin, tol_bw * tol_bw, tol_ba * tol_ba,
+                                tol_theta * tol_theta, relinearized, w, st));
+    g_launches += 3;
+    // the call's one host synchronisation: the re-preintegration's grid depends on the count, and so does the caller's next step
+    long long tot[2] = {0, 0};
+    CU(cudaMemcpyAsync(tot, w.pre + cpi::relin_total_offset(n_factors), sizeof tot, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    if (n_relinearized) *n_relinearized = tot[0];
+    if (tot[0] == 0) return CPI_OK;
+    CU(cpi::relin_gather_launch(tot[0], sample_offsets, ent_uniform, samples, w, d.sms, st));
+    g_launches += 1;
+    rc = preintegrate_dev(model, 64, tot[0], w.coff, 0, w.csamp, w.clin, sigmas, flags, w.crec, stream, 0);
+    if (rc) return rc;
+    CU(cpi::relin_scatter_launch(tot[0], rd, w, records, lin, d.sms, st));
+    g_launches += 1;
+    return CPI_OK;
+}
+
 int cpi_preintegrate_batch_host(int model, int dtype, int64_t n_windows, const int64_t* sample_offsets, int64_t ns_uniform,
                                 const void* samples, const void* lin, const double* sigmas, int flags, void* out_records) {
     if (model != 1 && model != 2) return fail(CPI_EINVAL, "model must be 1 or 2 (got %d)", model);

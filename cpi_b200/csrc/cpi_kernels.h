@@ -103,5 +103,25 @@ cudaError_t state_priors_fold_launch(int64_t n_chains, const int64_t* offs, int6
 cudaError_t state_priors_robust_launch(int64_t n, const int32_t* loss, const double* loss_k, const double* info, const double* rhs,
                                        const double* f, double* info_out, double* rhs_out, double* f_out, cudaStream_t st);
 cudaError_t retract_launch(int64_t n, const double* states, const double* xi, double* out, cudaStream_t st);
+// relinearize.cu: selection, stable compaction, gather and scatter around the K1/K2 launch of cpi_imu_records_relinearize
+struct RelinWorkspace {
+    double* crec;             // compact records [n][rd]
+    double* clin;             // compact linearisation points [n][13]
+    int64_t* idx;             // the selected factors, in factor order
+    int64_t* coff;            // compact CSR sample offsets [n + 1]
+    int32_t* flag;            // per factor 0/1
+    long long* blk;           // per CTA of the selection: {selected, entries}
+    long long* pre;           // their exclusive prefixes, then the grand totals {selected, entries} the host reads
+    double* csamp;            // compact samples (16-byte aligned), last
+    int64_t head_bytes;       // bytes before csamp
+};
+RelinWorkspace relin_workspace(void* ws, int rd, int64_t n);
+int64_t relin_workspace_bytes(int rd, int64_t n, int64_t n_entries);
+int64_t relin_total_offset(int64_t n);   // index into `pre` of the grand totals
+cudaError_t relin_select_launch(int model, int64_t n, const double* states, const int64_t* idx_i, const int64_t* offs, int64_t ent_uniform,
+                                const double* lin, double tw2, double ta2, double tt2, int32_t* mask, const RelinWorkspace& w, cudaStream_t st);
+cudaError_t relin_gather_launch(int64_t n_sel, const int64_t* offs, int64_t ent_uniform, const double* samples, const RelinWorkspace& w,
+                                int sms, cudaStream_t st);
+cudaError_t relin_scatter_launch(int64_t n_sel, int rd, const RelinWorkspace& w, double* records, double* lin, int sms, cudaStream_t st);
 
 }  // namespace cpi

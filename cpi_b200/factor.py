@@ -11,11 +11,12 @@ All arithmetic happens in libcpi_b200.so on the GPU.
 from __future__ import annotations
 
 import ctypes
+import math
 
 import numpy as np
 
 from . import capi
-from .capi import LOSS_CAUCHY, LOSS_GAUSSIAN, REC, REC_DOUBLES
+from .capi import FLAG_IMU_AVG, LOSS_CAUCHY, LOSS_GAUSSIAN, REC, REC_DOUBLES
 
 
 def _ptr(a):
@@ -191,6 +192,22 @@ def _chain_layout(chain_offsets, dev, n_factors=None, n_states=None, n_chains=No
     if (n_states is not None and n_states != n_chains * S) or (n_factors is not None and n_factors != n_chains * (S - 1)):
         raise ValueError(f"{n_chains} chains of {S} states do not match the given states / factors")
     return int(n_chains), None, S
+
+
+def _chain_factor_states(C, offs, S, nf, dev):
+    """(idx_i, idx_j) of the nf factors of a chain layout (chain c's factors stored back to back from index offsets[c] - c; factor
+    k links states idx_i[k] and idx_i[k] + 1), or (None, None) for one chain: the kernels' own chain indexing."""
+    import torch
+
+    if C <= 1:
+        return None, None
+    ar = torch.arange(nf, dtype=torch.int64, device=dev)
+    if offs is not None:
+        chain_of = torch.repeat_interleave(torch.arange(C, dtype=torch.int64, device=dev), offs[1:] - offs[:-1] - 1, output_size=nf)
+    else:
+        chain_of = ar // (S - 1) if S > 1 else ar
+    idx_i = ar + chain_of
+    return idx_i, idx_i + 1
 
 
 def chains_assemble(G11, G12, G22, g1, g2, chain_offsets, lam=0.0, prior_info=None, prior_rhs=None, diagonal_damping=False, n_chains=None,
@@ -488,15 +505,7 @@ def chains_lm_step(model, states, records, lin, chain_offsets, prior=None, lam=1
     if records.numel() != REC_DOUBLES[model] * nf:
         raise ValueError(f"{C} chains over {N} states hold {nf} factors: one record each")
     sp = _state_priors(state_priors, N, dev, offs, S, loss=state_prior_loss)
-    idx_i = idx_j = chain_of = None
-    if C > 1:                                                        # one chain: the eval kernel's own chain indexing
-        ar = torch.arange(nf, dtype=torch.int64, device=dev)
-        if offs is not None:
-            chain_of = torch.repeat_interleave(torch.arange(C, dtype=torch.int64, device=dev), offs[1:] - offs[:-1] - 1, output_size=nf)
-        else:
-            chain_of = ar // (S - 1) if S > 1 else ar
-        idx_i = ar + chain_of
-        idx_j = idx_i + 1
+    idx_i, idx_j = _chain_factor_states(C, offs, S, nf, dev)
     e, H1, H2 = factor_eval(model, states, records, lin, idx_i=idx_i, idx_j=idx_j, stream=stream)
     G11, G12, G22, g1, g2, f = factor_hessian(model, records, e, H1, H2, stream=stream)
     pi = pr = pf = None
@@ -667,15 +676,7 @@ def chains_lm(model, states, records, lin, chain_offsets, prior=None, lam=1e-5, 
     i32 = dict(dtype=torch.int32, device=dev)
     X = states.reshape(N, 16).clone()
     records, lin = records.contiguous(), lin.contiguous()
-    idx_i = idx_j = None
-    if C > 1:                                                        # as chains_lm_step
-        ar = torch.arange(nf, dtype=torch.int64, device=dev)
-        if offs is not None:
-            chain_of = torch.repeat_interleave(torch.arange(C, dtype=torch.int64, device=dev), offs[1:] - offs[:-1] - 1, output_size=nf)
-        else:
-            chain_of = ar // (S - 1) if S > 1 else ar
-        idx_i = ar + chain_of
-        idx_j = idx_i + 1
+    idx_i, idx_j = _chain_factor_states(C, offs, S, nf, dev)
     first = offs[:-1] if offs is not None else torch.arange(C, dtype=torch.int64, device=dev) * S
     pi = pr = pf = lin0 = None
     if prior is not None:
@@ -763,6 +764,73 @@ def chains_lm(model, states, records, lin, chain_offsets, prior=None, lam=1e-5, 
                 if check and int(flag.item()) == 0:
                     break
     return X, cost, lam_t, status, iters, tries
+
+
+def relinearize_records(model, states, records, lin, chain_offsets, samples, sigmas, sample_offsets=None, ns=None, flags=0, *, tol_bw, tol_ba,
+                        tol_theta=math.inf, stream=None, workspace=None):
+    """Re-preintegrate, on the device, the windows whose state bias left the records' linearisation point
+    (cpi_imu_records_relinearize; include/cpi_b200.h, DESIGN.md section 3i).  Between solves:
+    chains_lm -> relinearize_records -> if n > 0: chains_lm again from the new states.
+    states [N,16], records / lin: the factors of the chain layout (chain_offsets as chains_lm; factor k reads the bias of its state
+    i); samples / sample_offsets / ns / sigmas / flags: the windows as preint.preintegrate took them (sample_offsets a device int64
+    tensor [n_factors + 1], or None with ns steps per window).  tol_bw (rad/s), tol_ba (m/s^2), tol_theta (rad, model 2 only):
+    >= 0, math.inf disables a test.  A selected factor gets lin = [bg_i, ba_i, q_i (model 2; model 1 keeps its q), grav] and the
+    record of its window at that point; the others keep their bits.  records and lin are updated IN PLACE (both contiguous float64).
+    workspace: a CUDA tensor of at least cpi_imu_records_relinearize_workspace bytes, allocated here when absent or too small.
+    One host synchronisation (the count).  Returns (n_relinearized, mask [n_factors] int32 device tensor)."""
+    import torch
+
+    lib = capi.load()
+    if model not in (1, 2):
+        raise ValueError(f"model must be 1 or 2 (got {model})")
+    for name, t in (("tol_bw", tol_bw), ("tol_ba", tol_ba), ("tol_theta", tol_theta)):
+        if not float(t) >= 0.0:
+            raise ValueError(f"{name} must be >= 0 (math.inf disables the test; got {t})")
+    dev = states.device
+    for name, t in (("states", states), ("records", records), ("lin", lin), ("samples", samples)):
+        if t.dtype != torch.float64:
+            raise ValueError(f"{name} must be float64")
+    N = states.numel() // 16
+    C, offs, S = _chain_layout(chain_offsets, dev, n_states=N)
+    nf = N - C
+    if records.numel() != REC_DOUBLES[model] * nf or lin.numel() != 13 * nf:
+        raise ValueError(f"{C} chains over {N} states hold {nf} factors: one record ({REC_DOUBLES[model]} doubles) and one linearisation "
+                         f"point (13) each")
+    if not records.is_contiguous() or not lin.is_contiguous():
+        raise ValueError("records and lin are updated in place: they must be contiguous")
+    n_ent = samples.numel() // 7
+    avg = 1 if flags & FLAG_IMU_AVG else 0
+    if sample_offsets is not None:
+        if sample_offsets.dtype != torch.int64 or sample_offsets.numel() != nf + 1:
+            raise ValueError(f"sample_offsets must be an int64 tensor with n_factors + 1 = {nf + 1} entries")
+        sample_offsets, ns = sample_offsets.contiguous(), 0
+    else:
+        if ns is None or int(ns) < 0:
+            raise ValueError("give sample_offsets, or ns >= 0 steps per window")
+        ns = int(ns)
+        if n_ent < nf * (ns + avg):
+            raise ValueError("sample tensor shorter than n_factors * (ns + imu_avg)")
+    _check_f64(dev, states=states, records=records, lin=lin, samples=samples)
+    if sample_offsets is not None and (not sample_offsets.is_cuda or sample_offsets.device != dev):
+        raise ValueError(f"sample_offsets must be a CUDA tensor on {dev}")
+    idx_i, _ = _chain_factor_states(C, offs, S, nf, dev)
+    nbytes = int(lib.cpi_imu_records_relinearize_workspace(model, nf, n_ent))
+    if nbytes < 0:
+        capi.check(nbytes)
+    if workspace is None or workspace.numel() * workspace.element_size() < nbytes or not workspace.is_contiguous():
+        workspace = torch.empty((nbytes + 7) // 8, dtype=torch.float64, device=dev)
+    mask = torch.zeros(nf, dtype=torch.int32, device=dev)
+    sig = np.ascontiguousarray(sigmas, dtype=np.float64)
+    if sig.shape != (4,):
+        raise ValueError("sigmas must be the four sigmas (sigma_w, sigma_wb, sigma_a, sigma_ab)")
+    count = ctypes.c_int64(0)
+    with torch.cuda.device(dev):
+        st = stream if stream is not None else torch.cuda.current_stream(dev)
+        capi.check(lib.cpi_imu_records_relinearize(model, nf, _tptr(states.contiguous()), _tptr(idx_i), _tptr(sample_offsets), ns,
+                                                   _tptr(samples.contiguous()), _ptr(sig), int(flags), float(tol_bw), float(tol_ba),
+                                                   float(tol_theta), _tptr(lin), _tptr(records), _tptr(mask), ctypes.byref(count),
+                                                   _tptr(workspace), ctypes.c_void_p(st.cuda_stream)))
+    return int(count.value), mask
 
 
 def predict_state(model, states_k, records, lin, stream=None):

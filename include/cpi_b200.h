@@ -446,6 +446,56 @@ int cpi_imu_state_priors_fold(int64_t n_chains, const int64_t* chain_offsets, in
 int cpi_imu_state_priors_robust(int64_t n, const int32_t* loss, const double* loss_k, const double* info, const double* rhs, const double* f,
                                 double* info_out, double* rhs_out, double* f_out, void* stream);
 
+/*
+ * Re-preintegration of the windows whose bias estimate left the records' linearisation point (DESIGN.md section 3i): the
+ * re-integration VINS-Mono and OKVIS run between solves, on the device.  A factor corrects its record to the bias of its state i
+ * only to first order (J_q, J_a, J_b, H_a, H_b; model 2 also O_a, O_b in the orientation), which limits accuracy once the
+ * estimate is 1e-2 .. 1e-1 rad/s from `lin`.  Intended use, between solves: chains_lm -> relinearize -> if any: chains_lm again.
+ * fp64, DEVICE pointers except sigmas and n_relinearized, no allocation.  PARITY UNPINNED (the rule is the library's own);
+ * tests/test_relinearize.py holds the numpy statement.
+ *
+ *   n_factors        factor k has records[k] and lin[k] and reads the bias of state idx_i[k] (idx_i NULL: state k, as
+ *                    cpi_imu_factor_eval_batch); device indices are not checked
+ *   sample_offsets / ns_uniform / samples / sigmas / flags
+ *                    factor k's window in the layout of cpi_preintegrate_batch, and the sigmas and flags the records were
+ *                    preintegrated with (every combination cpi_preintegrate_batch accepts; an imu_avg window's trailing entry is in
+ *                    its range)
+ *   tol_bw, tol_ba, tol_theta   rad/s, m/s^2, rad; each >= 0, +inf disables that test; tol_theta is read by model 2 only
+ * Factor k is SELECTED when  |bg_i - lin_bw|^2 > tol_bw^2  or  |ba_i - lin_ba|^2 > tol_ba^2  or (model 2)  |theta|^2 > tol_theta^2,
+ * theta the rotation part of local(lin_q, q_i) (cpi_imu_prior_at's local); squared norms summed x, y, z in that order in fp64,
+ * without contraction.  A NaN in what the rule reads (the state's biases, model 2 its quaternion) leaves the factor unselected, so
+ * a chain that LM ended non-finite keeps its records.  For a selected factor
+ *     lin[k]     <- [bg_i, ba_i, q_lin', grav]   q_lin' = q_i (model 2), unchanged (model 1); gravity is never changed
+ *     records[k] <- the record cpi_preintegrate_batch gives for the window at the new lin, with the same sigmas and flags
+ * Unselected records and lin entries are not written.  relinearized (device int32 [n_factors], may be NULL) receives the 0/1 mask,
+ * *n_relinearized (host, may be NULL) the count.
+ *
+ * Launches: selection (one thread per factor), a scan of the per-CTA totals, the stable compaction (integer sums, no atomics: the
+ * same bits on every run); then ONE 16-byte device-to-host read of the selected windows and entries and a synchronise of
+ * `stream`, the call's only host synchronisation (the re-preintegration's grid depends on it); with none selected nothing more is
+ * launched.  Otherwise: a gather of the selected windows' samples into a compact 16-byte aligned CSR batch, the unchanged K1/K2
+ * launch of cpi_preintegrate_batch on it, a scatter of the records and lin back into their slots.
+ *
+ * workspace   device, 16-byte aligned, cpi_imu_records_relinearize_workspace(model, n_factors, n_entries) bytes with n_entries >=
+ *             every entry a window of the call spans: the worst case, every window selected.  That is 8 RD + 124 bytes per factor
+ *             (2 444 for model 1, 2 588 for model 2; RD the record doubles), 32 bytes per 256 factors, 56 bytes per entry, and at most
+ *             136 bytes more (alignment and the totals).  The compact samples dominate: 10 000 chains x 30 states x 200 samples need about 3.3 GB.
+ *
+ * Out of scope: fp32-storage records; records built by cpi_merge_records or cpi_scan_records (re-integration is one-shot over the
+ * window's full sample range, so the result differs from a merged record by the RK4 truncation of DESIGN.md section 3b); a cap on
+ * the windows re-integrated per call; relinearising inside an LM round (it would change the cost between the linearisation and the
+ * acceptance test).
+ */
+int64_t cpi_imu_records_relinearize_workspace(int model, int64_t n_factors, int64_t n_entries);
+int cpi_imu_records_relinearize(int model, int64_t n_factors, const double* states, const int64_t* idx_i,
+                                const int64_t* sample_offsets, int64_t ns_uniform, const double* samples,
+                                const double* sigmas /* host[4] */, int flags,
+                                double tol_bw, double tol_ba, double tol_theta,
+                                double* lin /* in/out */, double* records /* in/out */,
+                                int32_t* relinearized /* device [n_factors] 0/1, may be NULL */,
+                                int64_t* n_relinearized /* host, may be NULL */,
+                                void* workspace, void* stream);
+
 /* ---- callers either side of the factor ("next" rows) ----------------------------------------------------------------- */
 
 /* x_{k+1} prediction from x_k and a record: getpredictedstate_v1/_v2 (GraphSolver_IMU.cpp:263-307).
