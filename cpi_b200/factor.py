@@ -27,6 +27,33 @@ def _tptr(t):
     return None if t is None else ctypes.c_void_p(t.data_ptr())
 
 
+def _stream(dev, stream):
+    """The handle of stream, or of dev's current stream when it is None."""
+    import torch
+
+    return ctypes.c_void_p((stream if stream is not None else torch.cuda.current_stream(dev)).cuda_stream)
+
+
+def _launch(fn, dev, stream, *args):
+    """fn(*args, stream handle) with dev current: the library launches on the current device, so a call on another device's tensors
+    makes theirs current for the call.  stream: a stream of dev, or None for dev's current stream."""
+    import torch
+
+    with torch.cuda.device(dev):
+        capi.check(fn(*args, _stream(dev, stream)))
+
+
+def _staged(run, *arrays):
+    """run(*arrays) on device tensors; numpy arrays are staged to the current device as float64 and run's results (a tensor or a
+    tuple of them) copied back to numpy."""
+    import torch
+
+    if not isinstance(arrays[0], np.ndarray):
+        return run(*arrays)
+    out = run(*(torch.from_numpy(np.ascontiguousarray(a, dtype=np.float64)).cuda() for a in arrays))
+    return tuple(t.cpu().numpy() for t in out) if isinstance(out, tuple) else out.cpu().numpy()
+
+
 def factor_eval_host(model, states, records, lin, idx_i=None, idx_j=None, want_H1=True, want_H2=True):
     """HOST numpy in/out through ``cpi_imu_factor_eval_batch_host``.  Returns (e[n,15], H1[n,225]|None, H2[n,225]|None);
     H blocks are column-major 15x15 (reshape(15,15,order='F'))."""
@@ -53,6 +80,23 @@ def factor_eval_host(model, states, records, lin, idx_i=None, idx_j=None, want_H
     return e, H1, H2
 
 
+def _factor_indices(n, dev, states, lin, idx_i, idx_j):
+    """The checks factor_eval and factor_cost share: states, lin, idx_i and idx_j (both or neither; int64, one entry per factor of
+    the n) CUDA tensors on dev.  Returns (idx_i, idx_j) contiguous."""
+    import torch
+
+    for name, t in (("states", states), ("lin", lin), ("idx_i", idx_i), ("idx_j", idx_j)):
+        if t is not None and (not t.is_cuda or t.device != dev):
+            raise ValueError(f"{name} must be a CUDA tensor on {dev}")
+    if (idx_i is None) != (idx_j is None):
+        raise ValueError("idx_i and idx_j must both be given or both be None")
+    if idx_i is None:
+        return None, None
+    if idx_i.dtype != torch.int64 or idx_j.dtype != torch.int64 or idx_i.numel() != n or idx_j.numel() != n:
+        raise ValueError("idx_i / idx_j must be int64 tensors with one entry per factor")
+    return idx_i.contiguous(), idx_j.contiguous()
+
+
 def factor_eval(model, states, records, lin, idx_i=None, idx_j=None, want_H1=True, want_H2=True, out=None, stream=None):
     """DEVICE torch tensors (float64 / int64, contiguous).  Enqueues on ``stream`` (default: torch's current stream)."""
     import torch
@@ -60,84 +104,50 @@ def factor_eval(model, states, records, lin, idx_i=None, idx_j=None, want_H1=Tru
     lib = capi.load()
     n = records.numel() // REC_DOUBLES[model]
     dev = records.device
-    for name, t in (("states", states), ("lin", lin), ("idx_i", idx_i), ("idx_j", idx_j)):
-        if t is not None and (not t.is_cuda or t.device != dev):
-            raise ValueError(f"{name} must be a CUDA tensor on {dev}")
-    if (idx_i is None) != (idx_j is None):
-        raise ValueError("idx_i and idx_j must both be given or both be None")
-    if idx_i is not None:
-        if idx_i.dtype != torch.int64 or idx_j.dtype != torch.int64 or idx_i.numel() != n or idx_j.numel() != n:
-            raise ValueError("idx_i / idx_j must be int64 tensors with one entry per factor")
-        idx_i = idx_i.contiguous(); idx_j = idx_j.contiguous()
+    idx_i, idx_j = _factor_indices(n, dev, states, lin, idx_i, idx_j)
     if out is None:
         e = torch.empty((n, 15), dtype=torch.float64, device=dev)
         H1 = torch.empty((n, 225), dtype=torch.float64, device=dev) if want_H1 else None
         H2 = torch.empty((n, 225), dtype=torch.float64, device=dev) if want_H2 else None
     else:
         e, H1, H2 = out
-    with torch.cuda.device(dev):
-        st = stream if stream is not None else torch.cuda.current_stream(dev)
-        capi.check(lib.cpi_imu_factor_eval_batch(model, n, _tptr(states.contiguous()), _tptr(idx_i), _tptr(idx_j), _tptr(records.contiguous()),
-                                                 _tptr(lin.contiguous()), _tptr(e), _tptr(H1), _tptr(H2), ctypes.c_void_p(st.cuda_stream)))
+    _launch(lib.cpi_imu_factor_eval_batch, dev, stream, model, n, _tptr(states.contiguous()), _tptr(idx_i), _tptr(idx_j),
+            _tptr(records.contiguous()), _tptr(lin.contiguous()), _tptr(e), _tptr(H1), _tptr(H2))
     return e, H1, H2
 
 
 def factor_hessian(model, records, e, H1, H2, stream=None):
     """Information-form linearisation (cpi_imu_factor_hessian_batch): returns (G11, G12, G22 [n,225 col-major], g1, g2 [n,15], f [n]).
     Device tensors in/out, or numpy (staged through torch).  Parity vs GTSAM unpinned (GTSAM is not in the reference tree)."""
-    import torch
-
-    lib = capi.load()
-    host = isinstance(records, np.ndarray)
-    if host:
-        records, e, H1, H2 = (torch.from_numpy(np.ascontiguousarray(a, dtype=np.float64)).cuda() for a in (records, e, H1, H2))
-    n = records.numel() // REC_DOUBLES[model]
-    dev = records.device
-    G11, G12, G22 = (torch.empty((n, 225), dtype=torch.float64, device=dev) for _ in range(3))
-    g1, g2 = (torch.empty((n, 15), dtype=torch.float64, device=dev) for _ in range(2))
-    f = torch.empty((n,), dtype=torch.float64, device=dev)
-    st = stream if stream is not None else torch.cuda.current_stream()
-    capi.check(lib.cpi_imu_factor_hessian_batch(model, n, _tptr(records.contiguous()), _tptr(e.contiguous()), _tptr(H1.contiguous()), _tptr(H2.contiguous()),
-                                                _tptr(G11), _tptr(G12), _tptr(G22), _tptr(g1), _tptr(g2), _tptr(f), ctypes.c_void_p(st.cuda_stream)))
-    out = (G11, G12, G22, g1, g2, f)
-    return tuple(t.cpu().numpy() for t in out) if host else out
+    return _from_residuals(capi.load().cpi_imu_factor_hessian_batch, model, records, e, H1, H2, stream, (225,), (225,), (225,), (15,), (15,), ())
 
 
 def factor_whiten(model, records, e, H1, H2, stream=None):
     """Explicitly whitened form (cpi_imu_factor_whiten_batch): A1 = R_w H1, A2 = R_w H2 [n,225 col-major], b = -R_w e [n,15], with
     R_w the upper Cholesky factor of P_meas^-1 (GTSAM's Gaussian::Covariance).  Device tensors in/out, or numpy.  Parity unpinned."""
+    return _from_residuals(capi.load().cpi_imu_factor_whiten_batch, model, records, e, H1, H2, stream, (225,), (225,), (15,))
+
+
+def _from_residuals(fn, model, records, e, H1, H2, stream, *shapes):
+    """fn(model, n, records, e, H1, H2, outputs...) of factor_hessian / factor_whiten into new outputs [n, *shape] per shape."""
     import torch
 
-    lib = capi.load()
-    host = isinstance(records, np.ndarray)
-    if host:
-        records, e, H1, H2 = (torch.from_numpy(np.ascontiguousarray(a, dtype=np.float64)).cuda() for a in (records, e, H1, H2))
-    n = records.numel() // REC_DOUBLES[model]
-    A1, A2 = (torch.empty((n, 225), dtype=torch.float64, device=records.device) for _ in range(2))
-    b = torch.empty((n, 15), dtype=torch.float64, device=records.device)
-    st = stream if stream is not None else torch.cuda.current_stream()
-    capi.check(lib.cpi_imu_factor_whiten_batch(model, n, _tptr(records.contiguous()), _tptr(e.contiguous()), _tptr(H1.contiguous()), _tptr(H2.contiguous()),
-                                               _tptr(A1), _tptr(A2), _tptr(b), ctypes.c_void_p(st.cuda_stream)))
-    out = (A1, A2, b)
-    return tuple(t.cpu().numpy() for t in out) if host else out
+    def run(records, e, H1, H2):
+        dev = records.device
+        _check_f64(dev, records=records, e=e, H1=H1, H2=H2)
+        n = records.numel() // REC_DOUBLES[model]
+        out = tuple(torch.empty((n, *shape), dtype=torch.float64, device=dev) for shape in shapes)
+        _launch(fn, dev, stream, model, n, _tptr(records.contiguous()), _tptr(e.contiguous()), _tptr(H1.contiguous()), _tptr(H2.contiguous()),
+                *(_tptr(t) for t in out))
+        return out
+    return _staged(run, records, e, H1, H2)
 
 
 def chain_assemble(G11, G12, G22, g1, g2, lam=0.0, prior_info0=None, prior_rhs0=None, stream=None, diagonal_damping=False):
-    """Block-tridiagonal normal equations of the chain x_0 .. x_n from the per-factor information blocks (cpi_imu_chain_assemble).
-    Device tensors.  Damping: lam * I, or with diagonal_damping lam * clamp(diag, 1e-6, 1e32) (GTSAM's LevenbergMarquardtParams::diagonalDamping).
-    Returns (D [n+1,225], E [n,225], rhs [n+1,15])."""
-    import torch
-
-    lib = capi.load()
-    n = G11.shape[0]
-    dev = G11.device
-    D = torch.empty((n + 1, 225), dtype=torch.float64, device=dev)
-    E = torch.empty((max(n, 1), 225), dtype=torch.float64, device=dev)
-    rhs = torch.empty((n + 1, 15), dtype=torch.float64, device=dev)
-    st = stream if stream is not None else torch.cuda.current_stream()
-    capi.check(lib.cpi_imu_chain_assemble(n, _tptr(G11), _tptr(G12), _tptr(G22), _tptr(g1), _tptr(g2), float(lam), int(bool(diagonal_damping)), _tptr(prior_info0), _tptr(prior_rhs0),
-                                          _tptr(D), _tptr(E), _tptr(rhs), ctypes.c_void_p(st.cuda_stream)))
-    return D, E[:n], rhs
+    """Block-tridiagonal normal equations of the chain x_0 .. x_n from the per-factor information blocks: chains_assemble on one
+    chain of n + 1 states (the kernel cpi_imu_chain_assemble launches).  Device tensors.  Damping: lam * I, or with diagonal_damping
+    lam * clamp(diag, 1e-6, 1e32) (GTSAM's LevenbergMarquardtParams::diagonalDamping).  Returns (D [n+1,225], E [n,225], rhs [n+1,15])."""
+    return chains_assemble(G11, G12, G22, g1, g2, G11.shape[0] + 1, lam, prior_info0, prior_rhs0, diagonal_damping, n_chains=1, stream=stream)
 
 
 def chain_solve(D, E, rhs, stream=None, workspace=None):
@@ -145,13 +155,14 @@ def chain_solve(D, E, rhs, stream=None, workspace=None):
     import torch
 
     lib = capi.load()
+    dev = D.device
+    _check_f64(dev, D=D, E=E, rhs=rhs, workspace=workspace)
     n = D.shape[0]
-    x = torch.empty((n, 15), dtype=torch.float64, device=D.device)
+    x = torch.empty((n, 15), dtype=torch.float64, device=dev)
     nbytes = int(lib.cpi_imu_chain_solve_workspace(n))
     if workspace is None or workspace.numel() * 8 < nbytes:
-        workspace = torch.empty((nbytes + 7) // 8, dtype=torch.float64, device=D.device)
-    st = stream if stream is not None else torch.cuda.current_stream()
-    capi.check(lib.cpi_imu_chain_solve(n, _tptr(D), _tptr(E), _tptr(rhs), _tptr(x), _tptr(workspace), ctypes.c_void_p(st.cuda_stream)))
+        workspace = torch.empty((nbytes + 7) // 8, dtype=torch.float64, device=dev)
+    _launch(lib.cpi_imu_chain_solve, dev, stream, n, _tptr(D), _tptr(E), _tptr(rhs), _tptr(x), _tptr(workspace))
     return x
 
 
@@ -218,28 +229,32 @@ def chains_assemble(G11, G12, G22, g1, g2, chain_offsets, lam=0.0, prior_info=No
     on every chain's first state; damping as chain_assemble.  E is exactly 0 at chain boundaries, so chain_solve(D, E, rhs) solves every
     chain at once -- provided every chain is SPD (a NaN pivot spreads into the neighbouring chains).
     Returns (D [N,225], E [N-1,225], rhs [N,15]) for the N = n_factors + n_chains states."""
+    return _assemble(G11, G12, G22, g1, g2, chain_offsets, lam, prior_info, prior_rhs, diagonal_damping, n_chains, stream, per_chain=False)
+
+
+def _assemble(G11, G12, G22, g1, g2, chain_offsets, lam, prior_info, prior_rhs, diagonal_damping, n_chains, stream, per_chain):
+    """chains_assemble (lam a scalar), or with per_chain chains_assemble_lm (lam a device float64 [n_chains]; damp returned too)."""
     import torch
 
     dev = G11.device
-    _check_f64(dev, G11=G11, G12=G12, G22=G22, g1=g1, g2=g2, prior_info=prior_info, prior_rhs=prior_rhs)
+    _check_f64(dev, G11=G11, G12=G12, G22=G22, g1=g1, g2=g2, prior_info=prior_info, prior_rhs=prior_rhs, lam=lam if per_chain else None)
     nf = G11.numel() // 225
     C, offs, S = _chain_layout(chain_offsets, dev, n_factors=nf, n_chains=n_chains)
     if any(t.numel() != k * nf for t, k in ((G11, 225), (G12, 225), (G22, 225), (g1, 15), (g2, 15))):
         raise ValueError("G11 / G12 / G22 need 225 doubles and g1 / g2 15 per factor")
+    if per_chain and (lam is None or lam.numel() != C):
+        raise ValueError("lam needs one float64 CUDA entry per chain")
     if (prior_info is not None and prior_info.numel() != 225 * C) or (prior_rhs is not None and prior_rhs.numel() != 15 * C):
         raise ValueError("prior_info needs 225 doubles and prior_rhs 15 per chain")
     N = nf + C
-    D = torch.empty((N, 225), dtype=torch.float64, device=dev)
-    E = torch.empty((max(N - 1, 1), 225), dtype=torch.float64, device=dev)
-    rhs = torch.empty((N, 15), dtype=torch.float64, device=dev)
-    with torch.cuda.device(dev):
-        st = stream if stream is not None else torch.cuda.current_stream(dev)
-        capi.check(capi.load().cpi_imu_chains_assemble(C, _tptr(offs), S, _tptr(G11.contiguous()), _tptr(G12.contiguous()), _tptr(G22.contiguous()),
-                                                       _tptr(g1.contiguous()), _tptr(g2.contiguous()), float(lam), int(bool(diagonal_damping)),
-                                                       _tptr(None if prior_info is None else prior_info.contiguous()),
-                                                       _tptr(None if prior_rhs is None else prior_rhs.contiguous()), _tptr(D), _tptr(E), _tptr(rhs),
-                                                       ctypes.c_void_p(st.cuda_stream)))
-    return D, E[:N - 1], rhs
+    out = (torch.empty((N, 225), dtype=torch.float64, device=dev), torch.empty((max(N - 1, 1), 225), dtype=torch.float64, device=dev),
+           torch.empty((N, 15), dtype=torch.float64, device=dev)) + ((torch.empty((N, 15), dtype=torch.float64, device=dev),) if per_chain else ())
+    lib = capi.load()
+    c = lambda t: None if t is None else t.contiguous()
+    _launch(lib.cpi_imu_chains_assemble_lm if per_chain else lib.cpi_imu_chains_assemble, dev, stream, C, _tptr(offs), S, _tptr(c(G11)),
+            _tptr(c(G12)), _tptr(c(G22)), _tptr(c(g1)), _tptr(c(g2)), _tptr(c(lam)) if per_chain else float(lam), int(bool(diagonal_damping)),
+            _tptr(c(prior_info)), _tptr(c(prior_rhs)), *(_tptr(t) for t in out))
+    return (out[0], out[1][:N - 1]) + out[2:]
 
 
 def _loss_flags(code, k, rhs, f, measurement):
@@ -334,6 +349,45 @@ def _state_prior_csr(key, N):
     return order, torch.searchsorted(key_s, torch.arange(N + 1, dtype=torch.int64, device=key.device))
 
 
+class _StatePriors:
+    """The state priors of one call (the tuple of _state_priors) in the order the fold adds them: sorted stably by key (default:
+    their state), with the CSR of the keys below N, on the chain layout (C, offs, S), and the buffers their moved and reweighted
+    copies go to.  Its methods launch on the stream handle sp, with the priors' device current."""
+
+    def __init__(self, sp, N, layout, key=None):
+        import torch
+
+        idx, info, rhs, f, lin, self.single, loss = sp
+        order, self.sp_off = _state_prior_csr(idx if key is None else key, N)
+        self.C, self.offs, self.S = layout
+        self.M = M = idx.numel()
+        self.idx, self.info, self.rhs, self.lin = idx[order], info[order].contiguous(), rhs[order].contiguous(), lin[order].contiguous()
+        self.f = None if f is None else f[order].contiguous()
+        self.loss = None if loss is None else (loss[0][order].contiguous(), loss[1][order].contiguous())
+        f64 = dict(dtype=torch.float64, device=idx.device)
+        self.x, self.r, self.fm = torch.empty((M, 16), **f64), torch.empty((M, 15), **f64), torch.empty(M, **f64)
+        self.iw = self.info if loss is None else torch.empty((M, 225), **f64)     # the info the fold reads: weighted under a loss
+
+    def fold(self, lib, sp, rhs, f, G11=None, G22=None, g1=None, g2=None, f_out=None, pi=None, pr=None, pf=None):
+        """Reweight the priors (info, rhs, f) in place under their loss (s = f) and fold them into the targets; rhs None: f alone."""
+        p = _tptr
+        info, iw = (None, None) if rhs is None else (self.info, self.iw)
+        if self.loss is not None:
+            capi.check(lib.cpi_imu_state_priors_robust(self.M, p(self.loss[0]), p(self.loss[1]), p(info), p(rhs), p(f), p(iw), p(rhs), p(f), sp))
+        capi.check(lib.cpi_imu_state_priors_fold(self.C, p(self.offs), self.S, p(self.sp_off), p(iw), p(rhs), p(f), p(G11), p(G22), p(g1),
+                                                 p(g2), p(f_out), p(pi), p(pr), p(pf), sp))
+
+    def at(self, lib, sp, X, cost_only=False, **targets):
+        """Move the priors to the states X [N,16] (prior_at), reweight them there and fold them into the targets; cost_only: their
+        cost alone."""
+        import torch
+
+        p = _tptr
+        torch.index_select(X, 0, self.idx, out=self.x)
+        capi.check(lib.cpi_imu_prior_at(self.M, p(self.info), p(self.rhs), p(self.f), p(self.lin), p(self.x), p(self.r), p(self.fm), sp))
+        self.fold(lib, sp, None if cost_only else self.r, self.fm, **targets)
+
+
 def state_priors_fold(chain_offsets, sp_offsets, sp_info, sp_rhs, sp_f, G11=None, G22=None, g1=None, g2=None, f=None, prior_info=None,
                       prior_rhs=None, prior_f=None, n_chains=None, stream=None):
     """Add already-moved state priors IN PLACE into the factor blocks and chain priors (cpi_imu_state_priors_fold): a prior on state k
@@ -354,11 +408,9 @@ def state_priors_fold(chain_offsets, sp_offsets, sp_info, sp_rhs, sp_f, G11=None
         if t is not None and not t.is_contiguous():
             raise ValueError("the fold writes in place: its targets must be contiguous")
     c = lambda t: None if t is None else t.contiguous()
-    with torch.cuda.device(dev):
-        st = stream if stream is not None else torch.cuda.current_stream(dev)
-        capi.check(capi.load().cpi_imu_state_priors_fold(C, _tptr(offs), S, _tptr(sp_offsets.contiguous()), _tptr(c(sp_info)), _tptr(c(sp_rhs)),
-                                                         _tptr(c(sp_f)), _tptr(G11), _tptr(G22), _tptr(g1), _tptr(g2), _tptr(f), _tptr(prior_info),
-                                                         _tptr(prior_rhs), _tptr(prior_f), ctypes.c_void_p(st.cuda_stream)))
+    _launch(capi.load().cpi_imu_state_priors_fold, dev, stream, C, _tptr(offs), S, _tptr(sp_offsets.contiguous()), _tptr(c(sp_info)),
+            _tptr(c(sp_rhs)), _tptr(c(sp_f)), _tptr(G11), _tptr(G22), _tptr(g1), _tptr(g2), _tptr(f), _tptr(prior_info), _tptr(prior_rhs),
+            _tptr(prior_f))
 
 
 def state_priors_robust(loss, loss_k, info, rhs, f, info_out=None, rhs_out=None, f_out=None, stream=None):
@@ -388,11 +440,8 @@ def state_priors_robust(loss, loss_k, info, rhs, f, info_out=None, rhs_out=None,
         info_out = rhs_out = None
     f_out = torch.empty(M, dtype=torch.float64, device=dev) if f_out is None else f_out
     c = lambda t: None if t is None else t.contiguous()
-    with torch.cuda.device(dev):
-        st = stream if stream is not None else torch.cuda.current_stream(dev)
-        capi.check(capi.load().cpi_imu_state_priors_robust(M, _tptr(loss.contiguous()), _tptr(loss_k.contiguous()), _tptr(c(info)), _tptr(c(rhs)),
-                                                           _tptr(f.contiguous()), _tptr(info_out), _tptr(rhs_out), _tptr(f_out),
-                                                           ctypes.c_void_p(st.cuda_stream)))
+    _launch(capi.load().cpi_imu_state_priors_robust, dev, stream, M, _tptr(loss.contiguous()), _tptr(loss_k.contiguous()), _tptr(c(info)),
+            _tptr(c(rhs)), _tptr(f.contiguous()), _tptr(info_out), _tptr(rhs_out), _tptr(f_out))
     return info_out, rhs_out, f_out
 
 
@@ -411,14 +460,11 @@ def chain_marginalize(G11, G12, G22, g1, g2, f, chain_offsets, n_marg, prior=Non
 
     dev = G11.device
     nf = G11.numel() // 225
-    sp = None
-    if state_priors is not None or state_prior_loss is not None:
-        C, offs, S = _chain_layout(chain_offsets, dev, n_factors=nf, n_chains=n_chains)
-        if state_prior_loss is not None and state_priors is not None and len(state_priors) == 5 and state_priors[3] is None:
-            raise ValueError("state_prior_loss: chain_marginalize takes the priors moved, and a robust prior's f' is its s: f must be given")
-        sp = _state_priors(state_priors, nf + C, dev, loss=state_prior_loss, measurement=False)
-    _check_f64(dev, G11=G11, G12=G12, G22=G22, g1=g1, g2=g2, f=f)
     C, offs, S = _chain_layout(chain_offsets, dev, n_factors=nf, n_chains=n_chains)
+    if state_prior_loss is not None and state_priors is not None and len(state_priors) == 5 and state_priors[3] is None:
+        raise ValueError("state_prior_loss: chain_marginalize takes the priors moved, and a robust prior's f' is its s: f must be given")
+    sp = _state_priors(state_priors, nf + C, dev, loss=state_prior_loss, measurement=False)
+    _check_f64(dev, G11=G11, G12=G12, G22=G22, g1=g1, g2=g2, f=f)
     if any(t.numel() != k * nf for t, k in ((G11, 225), (G12, 225), (G22, 225), (g1, 15), (g2, 15), (f, 1))):
         raise ValueError("G11 / G12 / G22 need 225 doubles, g1 / g2 15 and f 1 per factor")
     pi = pr = pf = None
@@ -434,8 +480,9 @@ def chain_marginalize(G11, G12, G22, g1, g2, f, chain_offsets, n_marg, prior=Non
         nm, nmu = n_marg.contiguous(), 0
     else:
         nm, nmu = None, int(n_marg)
+    lib = capi.load()
     if sp is not None:                                               # eliminated states are never last: their priors land in G11 / g1 / f
-        idx, s_info, s_rhs, s_f, _, _, s_loss = sp
+        idx = sp[0]
         if offs is not None:
             c = (torch.searchsorted(offs, idx, right=True) - 1).clamp(0, C - 1)
             head = offs[c]
@@ -443,21 +490,16 @@ def chain_marginalize(G11, G12, G22, g1, g2, f, chain_offsets, n_marg, prior=Non
             c = idx // S
             head = c * S
         head = head + (nm[c] if nm is not None else nmu)
-        order, sp_off = _state_prior_csr(torch.where(idx < head, idx, idx + nf + C), nf + C)
-        s_info, s_rhs, s_f = s_info[order], s_rhs[order], None if s_f is None else s_f[order]
-        if s_loss is not None:                                       # the weights frozen at the blocks' point (s = the given f')
-            s_info, s_rhs, s_f = state_priors_robust(s_loss[0][order], s_loss[1][order], s_info, s_rhs, s_f, stream=stream)
+        sps = _StatePriors(sp, nf + C, (C, offs, S), key=torch.where(idx < head, idx, idx + nf + C))
         G11, g1, f = G11.contiguous().clone(), g1.contiguous().clone(), f.contiguous().clone()
-        state_priors_fold(offs if offs is not None else S, sp_off, s_info, s_rhs, s_f, G11=G11, g1=g1, f=f, n_chains=C, stream=stream)
+        with torch.cuda.device(dev):                                 # the weights frozen at the blocks' point (s = the given f')
+            sps.fold(lib, _stream(dev, stream), sps.rhs, sps.f, G11=G11, g1=g1, f_out=f)
     info = torch.empty((C, 225), dtype=torch.float64, device=dev)
     rhs = torch.empty((C, 15), dtype=torch.float64, device=dev)
     fo = torch.empty((C,), dtype=torch.float64, device=dev)
-    with torch.cuda.device(dev):
-        st = stream if stream is not None else torch.cuda.current_stream(dev)
-        capi.check(capi.load().cpi_imu_chain_marginalize(C, _tptr(offs), S, _tptr(nm), nmu, _tptr(G11.contiguous()), _tptr(G12.contiguous()),
-                                                         _tptr(G22.contiguous()), _tptr(g1.contiguous()), _tptr(g2.contiguous()), _tptr(f.contiguous()),
-                                                         _tptr(pi), _tptr(pr), _tptr(pf), _tptr(info), _tptr(rhs), _tptr(fo),
-                                                         ctypes.c_void_p(st.cuda_stream)))
+    _launch(lib.cpi_imu_chain_marginalize, dev, stream, C, _tptr(offs), S, _tptr(nm), nmu, _tptr(G11.contiguous()), _tptr(G12.contiguous()),
+            _tptr(G22.contiguous()), _tptr(g1.contiguous()), _tptr(g2.contiguous()), _tptr(f.contiguous()), _tptr(pi), _tptr(pr), _tptr(pf),
+            _tptr(info), _tptr(rhs), _tptr(fo))
     return info, rhs, fo
 
 
@@ -467,19 +509,22 @@ def prior_at(info, rhs, f, lin_states, states, stream=None):
     info is unchanged (the Jacobian of local taken as I, as GTSAM's LinearContainerFactor does).  Returns (rhs' [n,15], f' [n])."""
     import torch
 
+    dev, n = _prior_at_checks(info, rhs, f, lin_states, states)
+    rhs_out = torch.empty((n, 15), dtype=torch.float64, device=dev)
+    f_out = torch.empty((n,), dtype=torch.float64, device=dev)
+    _launch(capi.load().cpi_imu_prior_at, dev, stream, n, _tptr(info.contiguous()), _tptr(rhs.contiguous()),
+            _tptr(None if f is None else f.contiguous()), _tptr(lin_states.contiguous()), _tptr(states.contiguous()), _tptr(rhs_out), _tptr(f_out))
+    return rhs_out, f_out
+
+
+def _prior_at_checks(info, rhs, f, lin_states, states):
+    """prior_at's argument checks; returns (device, n)."""
     dev = info.device
     _check_f64(dev, info=info, rhs=rhs, f=f, lin_states=lin_states, states=states)
     n = info.numel() // 225
     if info.numel() != 225 * n or rhs.numel() != 15 * n or (f is not None and f.numel() != n) or lin_states.numel() != 16 * n or states.numel() != 16 * n:
         raise ValueError("prior_at needs info [n,225], rhs [n,15], f [n], lin_states and states [n,16]")
-    rhs_out = torch.empty((n, 15), dtype=torch.float64, device=dev)
-    f_out = torch.empty((n,), dtype=torch.float64, device=dev)
-    with torch.cuda.device(dev):
-        st = stream if stream is not None else torch.cuda.current_stream(dev)
-        capi.check(capi.load().cpi_imu_prior_at(n, _tptr(info.contiguous()), _tptr(rhs.contiguous()), _tptr(None if f is None else f.contiguous()),
-                                                _tptr(lin_states.contiguous()), _tptr(states.contiguous()), _tptr(rhs_out), _tptr(f_out),
-                                                ctypes.c_void_p(st.cuda_stream)))
-    return rhs_out, f_out
+    return dev, n
 
 
 def chains_lm_step(model, states, records, lin, chain_offsets, prior=None, lam=1e-5, diagonal_damping=True, stream=None, state_priors=None,
@@ -505,44 +550,68 @@ def chains_lm_step(model, states, records, lin, chain_offsets, prior=None, lam=1
     if records.numel() != REC_DOUBLES[model] * nf:
         raise ValueError(f"{C} chains over {N} states hold {nf} factors: one record each")
     sp = _state_priors(state_priors, N, dev, offs, S, loss=state_prior_loss)
-    idx_i, idx_j = _chain_factor_states(C, offs, S, nf, dev)
-    e, H1, H2 = factor_eval(model, states, records, lin, idx_i=idx_i, idx_j=idx_j, stream=stream)
-    G11, G12, G22, g1, g2, f = factor_hessian(model, records, e, H1, H2, stream=stream)
-    pi = pr = pf = None
-    if prior is not None:
-        pi, pr, pf, lin0 = prior
-        if lin0 is not None:
-            first = states.reshape(N, 16)[offs[:-1]] if offs is not None else states.reshape(N, 16)[::S]
-            pr, pf = prior_at(pi, pr, pf, lin0, first, stream=stream)
-    if sp is not None:
-        idx, s_info, s_rhs, s_f, s_lin, single, s_loss = sp
-        order, sp_off = _state_prior_csr(idx, N)
-        s_info, s_lin, idx = s_info[order], s_lin[order], idx[order]
-        r_m, f_m = prior_at(s_info, s_rhs[order], None if s_f is None else s_f[order], s_lin, states.reshape(N, 16).index_select(0, idx),
-                            stream=stream)
-        if s_loss is not None:                                       # reweighted at the states: (w W, w rhs', c(s))
-            s_info, _, _ = state_priors_robust(s_loss[0][order], s_loss[1][order], s_info, r_m, f_m, rhs_out=r_m, f_out=f_m, stream=stream)
-        if single:                                                   # the chain prior receives priors: fold into copies (zeros without one)
-            z = lambda t, *shape: torch.zeros(shape, dtype=torch.float64, device=dev) if t is None else t.contiguous().clone()
-            pi, pr, pf = z(pi, C, 225), z(pr, C, 15), z(pf, C)
-        state_priors_fold(offs if offs is not None else S, sp_off, s_info, r_m, f_m, G11=G11, G22=G22, g1=g1, g2=g2, f=f,
-                          prior_info=pi if single else None, prior_rhs=pr if single else None, prior_f=pf if single else None, n_chains=C,
-                          stream=stream)
-    D, E, rhs = chains_assemble(G11, G12, G22, g1, g2, chain_offsets, lam, pi, pr, diagonal_damping=diagonal_damping, n_chains=C, stream=stream)
+    idx_i, idx_j = _factor_indices(nf, records.device, states, lin, *_chain_factor_states(C, offs, S, nf, dev))
+    f64 = dict(dtype=torch.float64, device=dev)
+    c = lambda t: None if t is None else t.contiguous()
+    pi, pr, pf, lin0 = (None,) * 4 if prior is None else map(c, prior)
+    single = sp is not None and sp[5]
+    first, x0, pr_c, pf_c = None, None, pr, pf
+    if lin0 is not None:
+        first = offs[:-1] if offs is not None else torch.arange(C, dtype=torch.int64, device=dev) * S
+        x0, pr_c, pf_c = torch.empty((C, 16), **f64), torch.empty((C, 15), **f64), torch.empty(C, **f64)
+        _prior_at_checks(pi, pr, pf, lin0, x0)
+    elif single:                                                     # the chain prior receives priors: fold into copies (zeros without one)
+        pr_c, pf_c = (torch.zeros((C, 15), **f64) if pr is None else pr.clone()), (torch.zeros(C, **f64) if pf is None else pf.clone())
+    _check_f64(dev, prior_info=pi, prior_rhs=pr, prior_f=pf)
+    if single and pi is None:
+        pi = torch.zeros((C, 225), **f64)
+    pi_r = torch.empty((C, 225), **f64) if single else None
+    X = states.reshape(N, 16).contiguous()
+    e, H1, H2 = torch.empty((nf, 15), **f64), torch.empty((nf, 225), **f64), torch.empty((nf, 225), **f64)
+    G11, G12, G22 = (torch.empty((nf, 225), **f64) for _ in range(3))
+    g1, g2, f = torch.empty((nf, 15), **f64), torch.empty((nf, 15), **f64), torch.empty(nf, **f64)
+    sps = None if sp is None else _StatePriors(sp, N, (C, offs, S))
+    lib = capi.load()
+    with torch.cuda.device(dev), torch.cuda.stream(stream):
+        _linearize(lib, _stream(dev, stream), model, X, records.contiguous(), lin.contiguous(), idx_i, idx_j, (e, H1, H2, G11, G12, G22, g1, g2, f),
+                   (pi, pr, pf, lin0, first), (x0, pr_c, pf_c), sps, pi_r)
+    D, E, rhs = chains_assemble(G11, G12, G22, g1, g2, chain_offsets, lam, pi_r if single else pi, pr_c, diagonal_damping=diagonal_damping,
+                                n_chains=C, stream=stream)
     dx = chain_solve(D, E, rhs, stream=stream)
     # per-chain cost: one chain sums like chain_lm_step always has; many chains sum their factors' f in a fixed order
     # (cpi_imu_chains_cost_sum: an atomic scatter-add would give different bits from run to run)
     if C == 1:
         cost = f.sum().reshape(1)
     else:
-        cost = torch.empty(C, dtype=torch.float64, device=dev)
-        with torch.cuda.device(dev):
-            st = stream if stream is not None else torch.cuda.current_stream(dev)
-            capi.check(capi.load().cpi_imu_chains_cost_sum(C, _tptr(offs), S, _tptr(f), _tptr(cost),
-                                                           ctypes.c_void_p(st.cuda_stream)))
-    if pf is not None:
-        cost = cost + pf
-    return retract(states, dx, stream=stream), dx, cost
+        cost = torch.empty(C, **f64)
+        _launch(lib.cpi_imu_chains_cost_sum, dev, stream, C, _tptr(offs), S, _tptr(f), _tptr(cost))
+    if pf_c is not None:
+        cost = cost + pf_c
+    return retract(X, dx, stream=stream), dx, cost
+
+
+def _linearize(lib, sp, model, X, records, lin, idx_i, idx_j, blocks, prior, moved, sps, pi_r):
+    """The linearisation at the states X [N,16] that chains_lm_step and every round of chains_lm share, on the stream handle sp:
+    eval and the information blocks into blocks = (e, H1, H2, G11, G12, G22, g1, g2, f); the chain prior (pi, pr, pf, lin0, first)
+    moved to X[first] into moved = (x0, pr_c, pf_c) unless lin0 is None; the state priors sps (or None) moved to X, reweighted and
+    folded into the blocks and, on single-state chains, into pi_r (a copy of pi), pr_c and pf_c."""
+    import torch
+
+    p = _tptr
+    e, H1, H2, G11, G12, G22, g1, g2, f = blocks
+    pi, pr, pf, lin0, first = prior
+    x0, pr_c, pf_c = moved
+    if f.numel():
+        capi.check(lib.cpi_imu_factor_eval_batch(model, f.numel(), p(X), p(idx_i), p(idx_j), p(records), p(lin), p(e), p(H1), p(H2), sp))
+        capi.check(lib.cpi_imu_factor_hessian_batch(model, f.numel(), p(records), p(e), p(H1), p(H2), p(G11), p(G12), p(G22), p(g1), p(g2),
+                                                    p(f), sp))
+    if lin0 is not None:
+        torch.index_select(X, 0, first, out=x0)
+        capi.check(lib.cpi_imu_prior_at(x0.shape[0], p(pi), p(pr), p(pf), p(lin0), p(x0), p(pr_c), p(pf_c), sp))
+    if sps is not None:
+        if sps.single:
+            pi_r.copy_(pi)
+        sps.at(lib, sp, X, G11=G11, G22=G22, g1=g1, g2=g2, f_out=f, pi=pi_r, pr=pr_c if sps.single else None, pf=pf_c if sps.single else None)
 
 
 _PRIOR = {}
@@ -572,22 +641,14 @@ def factor_cost(model, states, records, lin, idx_i=None, idx_j=None, out=None, s
     Device tensors; returns f [n]."""
     import torch
 
+    import torch
+
     n = records.numel() // REC_DOUBLES[model]
     dev = records.device
-    for name, t in (("states", states), ("lin", lin), ("idx_i", idx_i), ("idx_j", idx_j)):
-        if t is not None and (not t.is_cuda or t.device != dev):
-            raise ValueError(f"{name} must be a CUDA tensor on {dev}")
-    if (idx_i is None) != (idx_j is None):
-        raise ValueError("idx_i and idx_j must both be given or both be None")
-    if idx_i is not None:
-        if idx_i.dtype != torch.int64 or idx_j.dtype != torch.int64 or idx_i.numel() != n or idx_j.numel() != n:
-            raise ValueError("idx_i / idx_j must be int64 tensors with one entry per factor")
-        idx_i = idx_i.contiguous(); idx_j = idx_j.contiguous()
+    idx_i, idx_j = _factor_indices(n, dev, states, lin, idx_i, idx_j)
     f = torch.empty((n,), dtype=torch.float64, device=dev) if out is None else out
-    with torch.cuda.device(dev):
-        st = stream if stream is not None else torch.cuda.current_stream(dev)
-        capi.check(capi.load().cpi_imu_factor_cost_batch(model, n, _tptr(states.contiguous()), _tptr(idx_i), _tptr(idx_j), _tptr(records.contiguous()),
-                                                         _tptr(lin.contiguous()), _tptr(f), ctypes.c_void_p(st.cuda_stream)))
+    _launch(capi.load().cpi_imu_factor_cost_batch, dev, stream, model, n, _tptr(states.contiguous()), _tptr(idx_i), _tptr(idx_j),
+            _tptr(records.contiguous()), _tptr(lin.contiguous()), _tptr(f))
     return f
 
 
@@ -595,30 +656,7 @@ def chains_assemble_lm(G11, G12, G22, g1, g2, chain_offsets, lam, prior_info=Non
                        stream=None):
     """chains_assemble with one lambda per chain (cpi_imu_chains_assemble_lm): lam is a device float64 [n_chains].
     Returns (D [N,225], E [N-1,225], rhs [N,15], damp [N,15]) -- damp the diagonal the damping added."""
-    import torch
-
-    dev = G11.device
-    _check_f64(dev, G11=G11, G12=G12, G22=G22, g1=g1, g2=g2, prior_info=prior_info, prior_rhs=prior_rhs, lam=lam)
-    nf = G11.numel() // 225
-    C, offs, S = _chain_layout(chain_offsets, dev, n_factors=nf, n_chains=n_chains)
-    if lam is None or lam.numel() != C:
-        raise ValueError("lam needs one float64 CUDA entry per chain")
-    if (prior_info is not None and prior_info.numel() != 225 * C) or (prior_rhs is not None and prior_rhs.numel() != 15 * C):
-        raise ValueError("prior_info needs 225 doubles and prior_rhs 15 per chain")
-    N = nf + C
-    D = torch.empty((N, 225), dtype=torch.float64, device=dev)
-    E = torch.empty((max(N - 1, 1), 225), dtype=torch.float64, device=dev)
-    rhs = torch.empty((N, 15), dtype=torch.float64, device=dev)
-    damp = torch.empty((N, 15), dtype=torch.float64, device=dev)
-    with torch.cuda.device(dev):
-        st = stream if stream is not None else torch.cuda.current_stream(dev)
-        capi.check(capi.load().cpi_imu_chains_assemble_lm(C, _tptr(offs), S, _tptr(G11.contiguous()), _tptr(G12.contiguous()), _tptr(G22.contiguous()),
-                                                          _tptr(g1.contiguous()), _tptr(g2.contiguous()), _tptr(lam.contiguous()),
-                                                          int(bool(diagonal_damping)),
-                                                          _tptr(None if prior_info is None else prior_info.contiguous()),
-                                                          _tptr(None if prior_rhs is None else prior_rhs.contiguous()), _tptr(D), _tptr(E), _tptr(rhs),
-                                                          _tptr(damp), ctypes.c_void_p(st.cuda_stream)))
-    return D, E[:N - 1], rhs, damp
+    return _assemble(G11, G12, G22, g1, g2, chain_offsets, lam, prior_info, prior_rhs, diagonal_damping, n_chains, stream, per_chain=True)
 
 
 def chains_solve(D, E, rhs, chain_offsets, n_chains=None, workspace=None, stream=None):
@@ -634,10 +672,8 @@ def chains_solve(D, E, rhs, chain_offsets, n_chains=None, workspace=None, stream
     nbytes = int(lib.cpi_imu_chains_solve_workspace(C, N))
     if workspace is None or workspace.numel() * 8 < nbytes:
         workspace = torch.empty((nbytes + 7) // 8, dtype=torch.float64, device=dev)
-    with torch.cuda.device(dev):
-        st = stream if stream is not None else torch.cuda.current_stream(dev)
-        capi.check(lib.cpi_imu_chains_solve(C, _tptr(offs), S, N, _tptr(D.contiguous()), _tptr(E.contiguous()), _tptr(rhs.contiguous()), _tptr(x),
-                                            _tptr(workspace), ctypes.c_void_p(st.cuda_stream)))
+    _launch(lib.cpi_imu_chains_solve, dev, stream, C, _tptr(offs), S, N, _tptr(D.contiguous()), _tptr(E.contiguous()), _tptr(rhs.contiguous()),
+            _tptr(x), _tptr(workspace))
     return x
 
 
@@ -659,13 +695,9 @@ def chains_lm(model, states, records, lin, chain_offsets, prior=None, lam=1e-5, 
     lib = capi.load()
     dev = states.device
     N = states.numel() // 16
-    if state_priors is not None or state_prior_loss is not None:
-        C, offs, S = _chain_layout(chain_offsets, dev, n_states=N)
-        sp = _state_priors(state_priors, N, dev, offs, S, loss=state_prior_loss)
-    else:
-        sp = None
-    _check_f64(dev, states=states, records=records, lin=lin)
     C, offs, S = _chain_layout(chain_offsets, dev, n_states=N)
+    sps = _state_priors(state_priors, N, dev, offs, S, loss=state_prior_loss)
+    _check_f64(dev, states=states, records=records, lin=lin)
     nf = N - C
     if records.numel() != REC_DOUBLES[model] * nf or lin.numel() != 13 * nf:
         raise ValueError(f"{C} chains over {N} states hold {nf} factors: one record and one linearisation point each")
@@ -686,18 +718,10 @@ def chains_lm(model, states, records, lin, chain_offsets, prior=None, lam=1e-5, 
         pr = torch.zeros((C, 15), **f64) if pr is None else pr.contiguous()
         pf = torch.zeros(C, **f64) if pf is None else pf.contiguous()
         lin0 = X.index_select(0, first) if lin0 is None else lin0.contiguous()
-    use_prior, single, s_lin, s_loss = prior is not None, False, None, None
-    if sp is not None:
-        s_idx, s_info, s_rhs, s_f, s_lin, single, s_loss = sp
-        order, sp_off = _state_prior_csr(s_idx, N)
-        s_idx, s_info, s_rhs, s_lin = s_idx[order], s_info[order].contiguous(), s_rhs[order].contiguous(), s_lin[order].contiguous()
-        s_f = None if s_f is None else s_f[order].contiguous()
-        M = s_idx.numel()
-        s_x, s_r, s_fc, s_fn = torch.empty((M, 16), **f64), torch.empty((M, 15), **f64), torch.empty(M, **f64), torch.empty(M, **f64)
-        s_iw = s_info                                                # the info the fold reads: the round's weighted copy under a loss
-        if s_loss is not None:
-            s_code, s_k = s_loss[0][order].contiguous(), s_loss[1][order].contiguous()
-            s_iw = torch.empty((M, 225), **f64)
+    use_prior, single = prior is not None, False
+    if sps is not None:
+        sps = _StatePriors(sps, N, (C, offs, S))
+        single = sps.single
         if single and not use_prior:                                 # a chain of one state carries priors: a zero chain prior receives them
             pi, pr, pf, lin0 = torch.zeros((C, 225), **f64), torch.zeros((C, 15), **f64), torch.zeros(C, **f64), X.index_select(0, first)
             use_prior = True
@@ -716,53 +740,31 @@ def chains_lm(model, states, records, lin, chain_offsets, prior=None, lam=1e-5, 
     ws_solve = torch.empty((int(lib.cpi_imu_chains_solve_workspace(C, N)) + 7) // 8, **f64)
     ws_lm = torch.empty((int(lib.cpi_imu_chains_lm_workspace(N)) + 7) // 8, **f64)
     p = _tptr
-    rd = REC_DOUBLES[model]
-    with torch.cuda.device(dev):
-        st = stream if stream is not None else torch.cuda.current_stream(dev)
-        sp = ctypes.c_void_p(st.cuda_stream)
-        with torch.cuda.stream(st):
-            for r in range(max_rounds):
-                check = check_every > 0 and (r + 1) % check_every == 0
-                if nf:
-                    capi.check(lib.cpi_imu_factor_eval_batch(model, nf, p(X), p(idx_i), p(idx_j), p(records), p(lin), p(e), p(H1), p(H2), sp))
-                    capi.check(lib.cpi_imu_factor_hessian_batch(model, nf, p(records), p(e), p(H1), p(H2), p(G11), p(G12), p(G22), p(g1), p(g2),
-                                                                p(f_cur), sp))
-                if use_prior:
-                    torch.index_select(X, 0, first, out=x0)
-                    capi.check(lib.cpi_imu_prior_at(C, p(pi), p(pr), p(pf), p(lin0), p(x0), p(pr_c), p(pf_c), sp))
-                if s_lin is not None:                                # the state priors at X, folded into this round's blocks
-                    torch.index_select(X, 0, s_idx, out=s_x)
-                    capi.check(lib.cpi_imu_prior_at(M, p(s_info), p(s_rhs), p(s_f), p(s_lin), p(s_x), p(s_r), p(s_fc), sp))
-                    if s_loss is not None:                           # reweighted at X: (w W, w rhs', c(s))
-                        capi.check(lib.cpi_imu_state_priors_robust(M, p(s_code), p(s_k), p(s_info), p(s_r), p(s_fc), p(s_iw), p(s_r), p(s_fc), sp))
-                    if single:
-                        pi_r.copy_(pi)
-                    capi.check(lib.cpi_imu_state_priors_fold(C, p(offs), S, p(sp_off), p(s_iw), p(s_r), p(s_fc), p(G11), p(G22), p(g1), p(g2),
-                                                             p(f_cur), p(pi_r), p(pr_c if single else None), p(pf_c if single else None), sp))
-                capi.check(lib.cpi_imu_chains_assemble_lm(C, p(offs), S, p(G11), p(G12), p(G22), p(g1), p(g2), p(lam_t), int(bool(diagonal_damping)),
-                                                          p(pi_r if single else pi), p(pr_c if use_prior else None), p(D), p(E), p(rhs), p(damp), sp))
-                capi.check(lib.cpi_imu_chains_solve(C, p(offs), S, N, p(D), p(E), p(rhs), p(dx), p(ws_solve), sp))
-                capi.check(lib.cpi_retract_batch(N, p(X), p(dx), p(Xn), sp))
-                if nf:
-                    capi.check(lib.cpi_imu_factor_cost_batch(model, nf, p(Xn), p(idx_i), p(idx_j), p(records), p(lin), p(f_new), sp))
-                if use_prior:
-                    torch.index_select(Xn, 0, first, out=x0)
-                    capi.check(lib.cpi_imu_prior_at(C, p(pi), p(pr), p(pf), p(lin0), p(x0), p(pr_n), p(pf_n), sp))
-                if s_lin is not None:                                # their f' at the candidate, into its cost
-                    torch.index_select(Xn, 0, s_idx, out=s_x)
-                    capi.check(lib.cpi_imu_prior_at(M, p(s_info), p(s_rhs), p(s_f), p(s_lin), p(s_x), p(s_r), p(s_fn), sp))
-                    if s_loss is not None:                           # c(s) at the candidate
-                        capi.check(lib.cpi_imu_state_priors_robust(M, p(s_code), p(s_k), None, None, p(s_fn), None, None, p(s_fn), sp))
-                    capi.check(lib.cpi_imu_state_priors_fold(C, p(offs), S, p(sp_off), None, None, p(s_fn), None, None, None, None, p(f_new), None,
-                                                             None, p(pf_n if single else None), sp))
-                if check:
-                    flag.zero_()
-                capi.check(lib.cpi_imu_chains_lm_update(C, p(offs), S, N, ctypes.byref(params), p(f_cur), p(pf_c if use_prior else None),
-                                                        p(f_new), p(pf_n if use_prior else None), p(rhs), p(D), p(E), p(damp), p(dx), p(Xn),
-                                                        p(X), p(lam_t), p(cost), p(status), p(iters), p(tries), p(flag if check else None),
-                                                        p(ws_lm), sp))
-                if check and int(flag.item()) == 0:
-                    break
+    blocks, chain_prior, moved = (e, H1, H2, G11, G12, G22, g1, g2, f_cur), (pi, pr, pf, lin0, first), (x0, pr_c, pf_c)
+    with torch.cuda.device(dev), torch.cuda.stream(stream):
+        sp = _stream(dev, stream)
+        for r in range(max_rounds):
+            check = check_every > 0 and (r + 1) % check_every == 0
+            _linearize(lib, sp, model, X, records, lin, idx_i, idx_j, blocks, chain_prior, moved, sps, pi_r)
+            capi.check(lib.cpi_imu_chains_assemble_lm(C, p(offs), S, p(G11), p(G12), p(G22), p(g1), p(g2), p(lam_t), int(bool(diagonal_damping)),
+                                                      p(pi_r if single else pi), p(pr_c if use_prior else None), p(D), p(E), p(rhs), p(damp), sp))
+            capi.check(lib.cpi_imu_chains_solve(C, p(offs), S, N, p(D), p(E), p(rhs), p(dx), p(ws_solve), sp))
+            capi.check(lib.cpi_retract_batch(N, p(X), p(dx), p(Xn), sp))
+            if nf:
+                capi.check(lib.cpi_imu_factor_cost_batch(model, nf, p(Xn), p(idx_i), p(idx_j), p(records), p(lin), p(f_new), sp))
+            if use_prior:
+                torch.index_select(Xn, 0, first, out=x0)
+                capi.check(lib.cpi_imu_prior_at(C, p(pi), p(pr), p(pf), p(lin0), p(x0), p(pr_n), p(pf_n), sp))
+            if sps is not None:                                      # the state priors' cost at the candidate
+                sps.at(lib, sp, Xn, cost_only=True, f_out=f_new, pf=pf_n if single else None)
+            if check:
+                flag.zero_()
+            capi.check(lib.cpi_imu_chains_lm_update(C, p(offs), S, N, ctypes.byref(params), p(f_cur), p(pf_c if use_prior else None),
+                                                    p(f_new), p(pf_n if use_prior else None), p(rhs), p(D), p(E), p(damp), p(dx), p(Xn),
+                                                    p(X), p(lam_t), p(cost), p(status), p(iters), p(tries), p(flag if check else None),
+                                                    p(ws_lm), sp))
+            if check and int(flag.item()) == 0:
+                break
     return X, cost, lam_t, status, iters, tries
 
 
@@ -824,12 +826,9 @@ def relinearize_records(model, states, records, lin, chain_offsets, samples, sig
     if sig.shape != (4,):
         raise ValueError("sigmas must be the four sigmas (sigma_w, sigma_wb, sigma_a, sigma_ab)")
     count = ctypes.c_int64(0)
-    with torch.cuda.device(dev):
-        st = stream if stream is not None else torch.cuda.current_stream(dev)
-        capi.check(lib.cpi_imu_records_relinearize(model, nf, _tptr(states.contiguous()), _tptr(idx_i), _tptr(sample_offsets), ns,
-                                                   _tptr(samples.contiguous()), _ptr(sig), int(flags), float(tol_bw), float(tol_ba),
-                                                   float(tol_theta), _tptr(lin), _tptr(records), _tptr(mask), ctypes.byref(count),
-                                                   _tptr(workspace), ctypes.c_void_p(st.cuda_stream)))
+    _launch(lib.cpi_imu_records_relinearize, dev, stream, model, nf, _tptr(states.contiguous()), _tptr(idx_i), _tptr(sample_offsets), ns,
+            _tptr(samples.contiguous()), _ptr(sig), int(flags), float(tol_bw), float(tol_ba), float(tol_theta), _tptr(lin), _tptr(records),
+            _tptr(mask), ctypes.byref(count), _tptr(workspace))
     return int(count.value), mask
 
 
@@ -838,15 +837,16 @@ def predict_state(model, states_k, records, lin, stream=None):
     import torch
 
     lib = capi.load()
-    host = isinstance(states_k, np.ndarray)
-    if host:
-        states_k, records, lin = (torch.from_numpy(np.ascontiguousarray(a, dtype=np.float64)).cuda() for a in (states_k, records, lin))
-    n = states_k.numel() // 16
-    out = torch.empty((n, 16), dtype=torch.float64, device=states_k.device)
-    st = stream if stream is not None else torch.cuda.current_stream()
-    capi.check(lib.cpi_predict_state_batch(model, n, _tptr(states_k.contiguous()), _tptr(records.contiguous()), _tptr(lin.contiguous()), _tptr(out),
-                                           ctypes.c_void_p(st.cuda_stream)))
-    return out.cpu().numpy() if host else out
+
+    def run(states_k, records, lin):
+        dev = states_k.device
+        _check_f64(dev, states_k=states_k, records=records, lin=lin)
+        n = states_k.numel() // 16
+        out = torch.empty((n, 16), dtype=torch.float64, device=dev)
+        _launch(lib.cpi_predict_state_batch, dev, stream, model, n, _tptr(states_k.contiguous()), _tptr(records.contiguous()),
+                _tptr(lin.contiguous()), _tptr(out))
+        return out
+    return _staged(run, states_k, records, lin)
 
 
 def propagate(model, states_k, cov_k, records, lin, anchor=None, want_cross=False, stream=None):
@@ -879,11 +879,8 @@ def propagate(model, states_k, cov_k, records, lin, anchor=None, want_cross=Fals
     x1 = torch.empty((n, 16), dtype=torch.float64, device=dev)
     c1 = torch.empty((n, 225), dtype=torch.float64, device=dev)
     cr = torch.empty((n, 225), dtype=torch.float64, device=dev) if want_cross else None
-    with torch.cuda.device(dev):
-        st = stream if stream is not None else torch.cuda.current_stream(dev)
-        capi.check(lib.cpi_propagate_batch(model, n, _tptr(states_k.contiguous()), _tptr(cov_k.contiguous()), _tptr(anchor),
-                                           _tptr(records.contiguous()), _tptr(lin.contiguous()), _tptr(x1), _tptr(c1), _tptr(cr),
-                                           ctypes.c_void_p(st.cuda_stream)))
+    _launch(lib.cpi_propagate_batch, dev, stream, model, n, _tptr(states_k.contiguous()), _tptr(cov_k.contiguous()), _tptr(anchor),
+            _tptr(records.contiguous()), _tptr(lin.contiguous()), _tptr(x1), _tptr(c1), _tptr(cr))
     return x1, c1, cr
 
 
@@ -912,14 +909,15 @@ def retract(states, xi, stream=None):
     import torch
 
     lib = capi.load()
-    host = isinstance(states, np.ndarray)
-    if host:
-        states, xi = (torch.from_numpy(np.ascontiguousarray(a, dtype=np.float64)).cuda() for a in (states, xi))
-    n = states.numel() // 16
-    out = torch.empty((n, 16), dtype=torch.float64, device=states.device)
-    st = stream if stream is not None else torch.cuda.current_stream()
-    capi.check(lib.cpi_retract_batch(n, _tptr(states.contiguous()), _tptr(xi.contiguous()), _tptr(out), ctypes.c_void_p(st.cuda_stream)))
-    return out.cpu().numpy() if host else out
+
+    def run(states, xi):
+        dev = states.device
+        _check_f64(dev, states=states, xi=xi)
+        n = states.numel() // 16
+        out = torch.empty((n, 16), dtype=torch.float64, device=dev)
+        _launch(lib.cpi_retract_batch, dev, stream, n, _tptr(states.contiguous()), _tptr(xi.contiguous()), _tptr(out))
+        return out
+    return _staged(run, states, xi)
 
 
 class JPLNavState:

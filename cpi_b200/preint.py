@@ -23,6 +23,7 @@ import numpy as np
 
 from . import capi
 from .capi import FLAG_ANALYTIC_JACOBIANS, FLAG_IMU_AVG, REC, REC_DOUBLES
+from .factor import _launch
 
 _RESULT_FIELDS = ("DT", "alpha_tau", "beta_tau", "q_k2tau", "R_k2tau", "J_q", "J_a", "J_b", "H_a", "H_b", "P_meas", "O_a", "O_b")
 
@@ -113,12 +114,8 @@ def preintegrate(model, samples, lin, sigmas, flags=0, offsets=None, ns=None, ou
     elif out.numel() < n * REC_DOUBLES[model] or not out.is_contiguous() or out.dtype != tdt:
         raise ValueError("out must be a contiguous tensor of n_windows * record_doubles in the input dtype")
     sig = np.ascontiguousarray(sigmas, dtype=np.float64)
-    # the library launches on the CURRENT device: make the tensors' device current for the call and take its stream
-    with torch.cuda.device(dev):
-        st = stream if stream is not None else torch.cuda.current_stream(dev)
-        fn = lib.cpi_preintegrate_batch if continue_records is None else lib.cpi_preintegrate_batch_continue
-        capi.check(fn(model, 64 if tdt == torch.float64 else 32, n, _tptr(offsets), int(ns), _tptr(samples), _tptr(lin), _ptr(sig), int(flags),
-                      _tptr(out), ctypes.c_void_p(st.cuda_stream)))
+    _launch(lib.cpi_preintegrate_batch if continue_records is None else lib.cpi_preintegrate_batch_continue, dev, stream, model,
+            64 if tdt == torch.float64 else 32, n, _tptr(offsets), int(ns), _tptr(samples), _tptr(lin), _ptr(sig), int(flags), _tptr(out))
     return out
 
 
@@ -186,10 +183,8 @@ def merge(model, records, lin, group_offsets=None, group=None, out=None, stream=
         out = torch.empty((max(n, 0), rd), dtype=records.dtype, device=dev)
     elif out.numel() < n * rd or not out.is_contiguous() or out.dtype != records.dtype:
         raise ValueError("out must be a contiguous tensor of n_groups * 290 elements in the records' dtype")
-    with torch.cuda.device(dev):
-        st = stream if stream is not None else torch.cuda.current_stream(dev)
-        capi.check(lib.cpi_merge_records(model, 64 if records.dtype == torch.float64 else 32, n, _tptr(group_offsets), uniform,
-                                         _tptr(records), _tptr(lin), _tptr(out), ctypes.c_void_p(st.cuda_stream)))
+    _launch(lib.cpi_merge_records, dev, stream, model, 64 if records.dtype == torch.float64 else 32, n, _tptr(group_offsets), uniform,
+            _tptr(records), _tptr(lin), _tptr(out))
     return out
 
 
@@ -248,10 +243,8 @@ def scan(model, records, lin, group_offsets=None, group=None, out=None, stream=N
     nbytes = int(lib.cpi_scan_records_workspace(max(n, 0), n_rec))
     if workspace is None or workspace.numel() * workspace.element_size() < nbytes or not workspace.is_contiguous():
         workspace = torch.empty((nbytes + 7) // 8, dtype=torch.float64, device=dev)
-    with torch.cuda.device(dev):
-        st = stream if stream is not None else torch.cuda.current_stream(dev)
-        capi.check(lib.cpi_scan_records(model, 64 if records.dtype == torch.float64 else 32, n, _tptr(group_offsets), uniform,
-                                        _tptr(records), _tptr(lin), _tptr(out), _tptr(workspace), ctypes.c_void_p(st.cuda_stream)))
+    _launch(lib.cpi_scan_records, dev, stream, model, 64 if records.dtype == torch.float64 else 32, n, _tptr(group_offsets), uniform,
+            _tptr(records), _tptr(lin), _tptr(out), _tptr(workspace))
     return out
 
 
