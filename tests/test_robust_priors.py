@@ -43,6 +43,9 @@ def np_loss(code, k, s):
         ca = (code == capi.LOSS_CAUCHY) & ok
         u = s[ca] / k2[ca]
         w[ca], c[ca] = 1.0 / (1.0 + u), k2[ca] * np.log1p(u)
+        big = np.zeros(s.shape, bool)
+        big[ca] = np.isinf(u)                                      # k < 1 and finite s above k^2 DBL_MAX: u overflows
+        w[big], c[big] = k2[big] / s[big], k2[big] * (np.log(s[big]) - np.log(k2[big]))
     return w, c
 
 
