@@ -597,6 +597,30 @@ int cpi_imu_chains_solve(int64_t n_chains, const int64_t* chain_offsets, int64_t
     return CPI_OK;
 }
 
+int64_t cpi_imu_chains_marginals_workspace(int64_t n_chains, int64_t n_states) {
+    if (n_chains < 0 || n_states < 0 || n_states < n_chains) return (int64_t)CPI_EINVAL;
+    return cpi::chains_marginals_workspace_bytes(n_states);
+}
+
+int cpi_imu_chains_marginals(int64_t n_chains, const int64_t* chain_offsets, int64_t chain_uniform, int64_t n_states, const double* D, const double* E,
+                             double* cov, double* cross, void* workspace, void* stream) {
+    int rc = chain_layout_check(n_chains, chain_offsets, chain_uniform);
+    if (rc) return rc;
+    if (n_states < n_chains) return fail(CPI_EINVAL, "n_states (%lld) below n_chains (%lld): every chain holds a state", (long long)n_states,
+                                         (long long)n_chains);
+    if (!chain_offsets && n_states != n_chains * chain_uniform)
+        return fail(CPI_EINVAL, "n_states (%lld) must be n_chains x chain_uniform (%lld)", (long long)n_states, (long long)(n_chains * chain_uniform));
+    if (n_chains == 0) return CPI_OK;
+    if (!D || !cov || !workspace || (n_states > 1 && !E)) return fail(CPI_EINVAL, "null pointer argument");
+    DevInfo d;
+    if ((rc = device_info(d))) return rc;
+    int launches = 0;
+    CU(cpi::chains_marginals_launch(n_chains, chain_offsets, chain_uniform, n_states, D, E, cov, cross, (double*)workspace, d.sms, (cudaStream_t)stream,
+                                    &launches));
+    g_launches += launches;
+    return CPI_OK;
+}
+
 int64_t cpi_imu_chains_lm_workspace(int64_t n_states) { return n_states < 0 ? (int64_t)CPI_EINVAL : cpi::lm_workspace_bytes(n_states); }
 
 int cpi_imu_chains_lm_update(int64_t n_chains, const int64_t* chain_offsets, int64_t chain_uniform, int64_t n_states, const cpi_lm_params* params,

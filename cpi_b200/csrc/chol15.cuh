@@ -32,6 +32,16 @@ CPI_DEV void fwd15(const double* L, double* y) {
         y[i] = t / L[i * 16 + i];
     }
 }
+// y = L^-T b  for a per-lane right-hand side held in registers (b -> y in place)
+CPI_DEV void bwd15(const double* L, double* y) {
+#pragma unroll
+    for (int i = 14; i >= 0; i--) {
+        double t = y[i];
+#pragma unroll
+        for (int k = i + 1; k < 15; k++) t = fma(-L[k * 16 + i], y[k], t);
+        y[i] = t / L[i * 16 + i];
+    }
+}
 // x = L^-T r : lane k (< 15) passes r_k and receives x_k; column-oriented backward substitution with shuffles
 CPI_DEV double warp_bwd15(const double* L, double r, int lane) {
     double x = 0.0;

@@ -70,6 +70,10 @@ cudaError_t chains_assemble_lm_launch(int64_t n_chains, const int64_t* offs, int
 int64_t chains_solve_workspace_bytes(int64_t n_states);
 cudaError_t chains_solve_launch(int64_t n_chains, const int64_t* offs, int64_t uniform, int64_t n_states, const double* D, const double* E, const double* b,
                                 double* x, double* ws, int sms, cudaStream_t st, int* launches);
+// the diagonal and neighbour blocks of the inverse by selected inversion of the isolated solve's levels (cpi_imu_chains_marginals)
+int64_t chains_marginals_workspace_bytes(int64_t n_states);
+cudaError_t chains_marginals_launch(int64_t n_chains, const int64_t* offs, int64_t uniform, int64_t n_states, const double* D, const double* E,
+                                    double* cov, double* cross, double* ws, int sms, cudaStream_t st, int* launches);
 // merge.cu: one merged model-1 record per group (dtype 64 or 32)
 cudaError_t merge_launch(int dtype, int64_t n_groups, const int64_t* offsets, int64_t uniform, const void* records, const void* lin,
                          void* out, cudaStream_t st);

@@ -335,6 +335,130 @@ __global__ void k_chain_ids(int64_t n_chains, const int64_t* offs, int64_t unifo
     }
 }
 
+// ---- selected inversion: the block-tridiagonal part of the inverse (cpi_imu_chains_marginals) -----------------------------------------
+// Level l+1's system is the Schur complement of level l's on its even nodes, so its inverse is the full inverse on the states level l+1
+// keeps.  Top-down over the levels of the forward phase, odd node i = 2t+1 of level l (nodes at original states i * stride), whose
+// neighbours i-1, i+1 are nodes t, t+1 of level l+1 with known blocks (diagonal ones in cov at their original state, Sigma_{i-1,i+1} in
+// Nin[t]):
+//   Sigma_{i,i-1} = -Lc^-T (Za Sigma_{i-1,i-1} + Zb Sigma_{i+1,i-1}),   Sigma_{i,i+1} = -Lc^-T (Za Sigma_{i-1,i+1} + Zb Sigma_{i+1,i+1}),
+//   Sigma_{i,i}   =  Lc^-T (Lc^-1 - Za Sigma_{i,i-1}^T - Zb Sigma_{i,i+1}^T)
+// Isolated as the solve: a neighbour of another chain is not loaded and not multiplied, and its coupling is written as exact 0.
+
+// the root (one node): cov = D^-1, the lower triangle of column `lane` by lane `lane`, mirrored
+__global__ void k_bcr_selinv_root(const double* D, double* cov) {
+    __shared__ double L[15 * 16];
+    const int lane = threadIdx.x;
+    for (int k = lane; k < 225; k += 32) { const int r = k % 15, c = k / 15; if (r >= c) L[r * 16 + c] = D[k]; }
+    __syncwarp();
+    warp_chol15(L, lane);
+    if (lane < 15) {
+        double y[15];
+#pragma unroll
+        for (int r = 0; r < 15; r++) y[r] = (r == lane) ? 1.0 : 0.0;
+        fwd15(L, y);
+        __syncwarp(0x7fffu);                                       // L is reloaded for the backward pass: 120 entries held live would spill
+        bwd15(L, y);
+#pragma unroll
+        for (int r = 0; r < 15; r++) if (r >= lane) { cov[r + 15 * lane] = y[r]; cov[lane + 15 * r] = y[r]; }
+    }
+}
+
+// One warp per odd node of a level.  Writes Sigma_ii to cov[i * stride] and the level's neighbour blocks Sigma_{k,k+1} of the pairs
+// (i-1, i) and (i, i+1): to Nout slot k (levels >= 1; exact 0 across chains) or, with Nout NULL (level 0), to cross slot k - cid[k]
+// (factor order; pairs across chains have no slot; cross may be NULL).  Nin is read only for two neighbours of i's chain.
+__global__ void __launch_bounds__(128) k_bcr_selinv_iso(int64_t m, int64_t stride, const int64_t* cid, const double* Lc, const double* Za,
+                                                        const double* Zb, const double* Nin, double* cov, double* Nout, double* cross) {
+    __shared__ double sL[4][15 * 16];
+    __shared__ double sM[4][5][225];           // [warp][Za | Zb | Sigma_{i-1,i-1} -> Sigma_{i,i-1} | Sigma_{i-1,i+1} | Sigma_{i+1,i+1} -> Sigma_{i,i+1}]
+    const int wib = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int64_t t = (int64_t)blockIdx.x * 4 + wib;
+    const int64_t i = 2 * t + 1;
+    if (i >= m) return;
+    const int64_t ci = cid[i * stride];
+    const bool has_left = cid[(i - 1) * stride] == ci;
+    const bool has_right = i + 1 < m && cid[(i + 1) * stride] == ci;
+    double *L = sL[wib], *A = sM[wib][0], *B = sM[wib][1], *XL = sM[wib][2], *N = sM[wib][3], *XR = sM[wib][4];
+    for (int k = lane; k < 225; k += 32) {
+        const int r = k % 15, c = k / 15;
+        if (r >= c) L[r * 16 + c] = Lc[t * 225 + k];
+        if (has_left) { A[k] = Za[t * 225 + k]; XL[k] = cov[(i - 1) * stride * 225 + k]; }
+        if (has_right) { B[k] = Zb[t * 225 + k]; XR[k] = cov[(i + 1) * stride * 225 + k]; }
+        if (has_left && has_right) N[k] = Nin[t * 225 + k];
+    }
+    __syncwarp();
+    // lanes 0..14: column c of Sigma_{i,i-1}; lanes 15..29: column c of Sigma_{i,i+1}  (Sigma_{i+1,i-1} = N^T)
+    const int c = lane % 15;
+    const bool right = lane >= 15;
+    const bool active = lane < 30 && (right ? has_right : has_left);
+    double y[15];
+#pragma unroll
+    for (int r = 0; r < 15; r++) y[r] = 0.0;
+    if (active) {
+        if (has_left) {
+#pragma unroll
+            for (int q = 0; q < 15; q++) {
+                const double v = right ? N[q + 15 * c] : XL[q + 15 * c];
+#pragma unroll
+                for (int r = 0; r < 15; r++) y[r] = fma(A[r + 15 * q], v, y[r]);
+            }
+        }
+        if (has_right) {
+#pragma unroll
+            for (int q = 0; q < 15; q++) {
+                const double v = right ? XR[q + 15 * c] : N[c + 15 * q];
+#pragma unroll
+                for (int r = 0; r < 15; r++) y[r] = fma(B[r + 15 * q], v, y[r]);
+            }
+        }
+        bwd15(L, y);
+    }
+    __syncwarp();
+    if (active) {
+        double* X = right ? XR : XL;
+#pragma unroll
+        for (int r = 0; r < 15; r++) X[r + 15 * c] = -y[r];
+    }
+    __syncwarp();
+    // the level's neighbour blocks: Sigma_{i-1,i} = Sigma_{i,i-1}^T in slot i-1, Sigma_{i,i+1} in slot i
+    for (int k = lane; k < 225; k += 32) {
+        const int r = k % 15, cc = k / 15;
+        if (Nout) {
+            Nout[(i - 1) * 225 + k] = has_left ? XL[cc + 15 * r] : 0.0;
+            if (i + 1 < m) Nout[i * 225 + k] = has_right ? XR[k] : 0.0;
+        } else if (cross) {
+            if (has_left) cross[(i - 1 - ci) * 225 + k] = XL[cc + 15 * r];
+            if (has_right) cross[(i - ci) * 225 + k] = XR[k];
+        }
+    }
+    // Sigma_ii: column `lane` of Lc^-T (Lc^-1 - Za Sigma_{i,i-1}^T - Zb Sigma_{i,i+1}^T), its lower triangle mirrored
+    if (lane < 15) {
+#pragma unroll
+        for (int r = 0; r < 15; r++) y[r] = (r == lane) ? 1.0 : 0.0;
+        fwd15(L, y);
+        __syncwarp(0x7fffu);                                       // as in k_bcr_selinv_root
+        if (has_left) {
+#pragma unroll
+            for (int q = 0; q < 15; q++) {
+                const double v = XL[lane + 15 * q];
+#pragma unroll
+                for (int r = 0; r < 15; r++) y[r] = fma(-A[r + 15 * q], v, y[r]);
+            }
+        }
+        if (has_right) {
+#pragma unroll
+            for (int q = 0; q < 15; q++) {
+                const double v = XR[lane + 15 * q];
+#pragma unroll
+                for (int r = 0; r < 15; r++) y[r] = fma(-B[r + 15 * q], v, y[r]);
+            }
+        }
+        bwd15(L, y);
+        double* S = cov + i * stride * 225;
+#pragma unroll
+        for (int r = 0; r < 15; r++) if (r >= lane) { S[r + 15 * lane] = y[r]; S[lane + 15 * r] = y[r]; }
+    }
+}
+
 // ---- launchers ----------------------------------------------------------------------------------------------------------------------
 cudaError_t whiten_launch(int rd, int64_t n, const double* records, const double* e, const double* H1, const double* H2, double* A1, double* A2, double* b, cudaStream_t st) {
     if (n == 0) return cudaSuccess;
@@ -361,24 +485,77 @@ cudaError_t chains_assemble_lm_launch(int64_t n_chains, const int64_t* offs, int
     return cudaGetLastError();
 }
 
-// workspace layout: for every level l >= 1 the reduced system (D, E, b), for every level l >= 0 the eliminated nodes (Lc, Za, Zb, zb)
-static int64_t bcr_doubles(int64_t m) {
-    int64_t tot = 0;
+// The workspace of the block cyclic reduction, level by level: level l has m nodes (node i is original state i * 2^l); the workspace
+// holds, for l = 0, 1, ..., the eliminated odd nodes' Lc, Za, Zb, zb, then the next level's reduced system D, E, b.  The last level
+// (one node) is the root.  Offsets in doubles.
+struct BcrLevel { int64_t m, Lc, Za, Zb, zb, D, E, b; };
+// fills lv[0 .. nl) and returns nl (at most 63: m < 2^63); *end: the doubles the levels take
+static int bcr_levels(int64_t m, BcrLevel* lv, int64_t* end) {
+    int nl = 0;
+    int64_t p = 0;
     while (m > 1) {
         const int64_t odd = m / 2, even = (m + 1) / 2;
-        tot += odd * (3 * 225 + 15);            // Lc, Za, Zb, zb of this level's odd nodes
-        tot += even * (2 * 225 + 15);           // D, E, b of the next level
+        BcrLevel& L = lv[nl++];
+        L.m = m;
+        L.Lc = p; p += odd * 225; L.Za = p; p += odd * 225; L.Zb = p; p += odd * 225; L.zb = p; p += odd * 15;
+        L.D = p; p += even * 225; L.E = p; p += even * 225; L.b = p; p += even * 15;
         m = even;
     }
-    return tot + 16;
+    *end = p;
+    return nl;
 }
+static int64_t bcr_doubles(int64_t m) {
+    BcrLevel lv[64];
+    int64_t end;
+    bcr_levels(m, lv, &end);
+    return end + 16;
+}
+// The forward phase (elimination and reduction of every level) on the level table; the root's system is left at level nl's D, b.
+static void bcr_forward(const BcrLevel* lv, int nl, const double* D, const double* E, const double* b, double* ws, const int64_t* cid,
+                        cudaStream_t st) {
+    for (int l = 0; l < nl; l++) {
+        const BcrLevel& L = lv[l];
+        const double *cD = l ? ws + lv[l - 1].D : D, *cE = l ? ws + lv[l - 1].E : E, *cb = l ? ws + lv[l - 1].b : b;
+        const int64_t odd = L.m / 2, even = (L.m + 1) / 2;
+        const int64_t stride = (int64_t)1 << l;
+        if (cid) {
+            k_bcr_eliminate_iso<<<(int)((odd + 3) / 4), 128, 0, st>>>(L.m, stride, cid, cD, cE, cb, ws + L.Lc, ws + L.Za, ws + L.Zb, ws + L.zb);
+            k_bcr_reduce_iso<<<(int)((even + 3) / 4), 128, 0, st>>>(L.m, stride, cid, cD, cb, ws + L.Za, ws + L.Zb, ws + L.zb, ws + L.D, ws + L.E,
+                                                                     ws + L.b);
+        } else {
+            k_bcr_eliminate<<<(int)((odd + 3) / 4), 128, 0, st>>>(L.m, cD, cE, cb, ws + L.Lc, ws + L.Za, ws + L.Zb, ws + L.zb);
+            k_bcr_reduce<<<(int)((even + 3) / 4), 128, 0, st>>>(L.m, cD, cb, ws + L.Za, ws + L.Zb, ws + L.zb, ws + L.D, ws + L.E, ws + L.b);
+        }
+    }
+}
+// What follows the levels (offsets in doubles): the isolated solve's chain id of every state (int64), then the selected inversion's
+// zero right-hand side [n_states, 15] for the forward phase and the neighbour blocks Sigma_{k,k+1} of every level l >= 1 with two nodes
+// or more (m_l - 1 blocks each, level order).  solve_end / selinv_end: the doubles the isolated solve / the selected inversion take.
+struct BcrTail { int64_t cid, solve_end, b0, nbr[64], selinv_end; };
+static BcrTail bcr_tail(int64_t n_states, const BcrLevel* lv, int nl) {
+    BcrTail t;
+    t.cid = bcr_doubles(n_states);
+    t.solve_end = t.b0 = t.cid + n_states;
+    int64_t p = t.b0 + n_states * 15;
+    for (int l = 0; l < 64; l++) t.nbr[l] = -1;
+    for (int l = 1; l < nl; l++) { t.nbr[l] = p; p += (lv[l].m - 1) * 225; }
+    t.selinv_end = p;
+    return t;
+}
+static BcrTail bcr_tail(int64_t n_states) {
+    BcrLevel lv[64];
+    int64_t end;
+    const int nl = bcr_levels(n_states, lv, &end);
+    return bcr_tail(n_states, lv, nl);
+}
+
 int64_t chain_solve_workspace_bytes(int64_t n_states) { return bcr_doubles(n_states) * 8; }
 // the isolated solve: the same, followed by the chain id of every state
-int64_t chains_solve_workspace_bytes(int64_t n_states) { return bcr_doubles(n_states) * 8 + n_states * 8; }
+int64_t chains_solve_workspace_bytes(int64_t n_states) { return bcr_tail(n_states).solve_end * 8; }
 
 cudaError_t chains_solve_launch(int64_t n_chains, const int64_t* offs, int64_t uniform, int64_t n_states, const double* D, const double* E, const double* b,
                                 double* x, double* ws, int sms, cudaStream_t st, int* launches) {
-    int64_t* cid = reinterpret_cast<int64_t*>(ws + bcr_doubles(n_states));
+    int64_t* cid = reinterpret_cast<int64_t*>(ws + bcr_tail(n_states).cid);
     const int64_t blocks = (n_states + 255) / 256, cap = (int64_t)sms * 8;
     k_chain_ids<<<(int)(blocks < cap ? blocks : cap), 256, 0, st>>>(n_chains, offs, uniform, n_states, cid);
     const cudaError_t e = chain_solve_launch(n_states, D, E, b, x, ws, st, launches, cid);
@@ -388,41 +565,46 @@ cudaError_t chains_solve_launch(int64_t n_chains, const int64_t* offs, int64_t u
 
 cudaError_t chain_solve_launch(int64_t n_states, const double* D, const double* E, const double* b, double* x, double* ws, cudaStream_t st, int* launches,
                                const int64_t* cid) {
-    struct Level { int64_t m; const double *D, *E, *b; double *Lc, *Za, *Zb, *zb; };
-    Level lv[64];
-    int nl = 0;
-    int64_t m = n_states;
-    const double *cD = D, *cE = E, *cb = b;
-    double* p = ws;
-    int nk = 0;
-    while (m > 1) {
-        const int64_t odd = m / 2, even = (m + 1) / 2;
-        Level& L = lv[nl++];
-        L.m = m; L.D = cD; L.E = cE; L.b = cb;
-        L.Lc = p; p += odd * 225; L.Za = p; p += odd * 225; L.Zb = p; p += odd * 225; L.zb = p; p += odd * 15;
-        double* nD = p; p += even * 225; double* nE = p; p += even * 225; double* nb = p; p += even * 15;
-        const int64_t stride = (int64_t)1 << (nl - 1);              // level nl - 1: node i is original state i * 2^(nl-1)
-        if (cid) {
-            k_bcr_eliminate_iso<<<(int)((odd + 3) / 4), 128, 0, st>>>(m, stride, cid, cD, cE, cb, L.Lc, L.Za, L.Zb, L.zb);
-            k_bcr_reduce_iso<<<(int)((even + 3) / 4), 128, 0, st>>>(m, stride, cid, cD, cb, L.Za, L.Zb, L.zb, nD, nE, nb);
-        } else {
-            k_bcr_eliminate<<<(int)((odd + 3) / 4), 128, 0, st>>>(m, cD, cE, cb, L.Lc, L.Za, L.Zb, L.zb);
-            k_bcr_reduce<<<(int)((even + 3) / 4), 128, 0, st>>>(m, cD, cb, L.Za, L.Zb, L.zb, nD, nE, nb);
-        }
-        nk += 2;
-        cD = nD; cE = nE; cb = nb; m = even;
-    }
-    k_bcr_root<<<1, 32, 0, st>>>(cD, cb, x, 1);
-    nk++;
-    int64_t stride = (int64_t)1 << nl;
+    BcrLevel lv[64];
+    int64_t end;
+    const int nl = bcr_levels(n_states, lv, &end);
+    bcr_forward(lv, nl, D, E, b, ws, cid, st);
+    k_bcr_root<<<1, 32, 0, st>>>(nl ? ws + lv[nl - 1].D : D, nl ? ws + lv[nl - 1].b : b, x, 1);
     for (int l = nl - 1; l >= 0; l--) {
-        stride >>= 1;
-        const int64_t odd = lv[l].m / 2;
-        if (cid) k_bcr_backsub_iso<<<(int)((odd + 3) / 4), 128, 0, st>>>(lv[l].m, stride, cid, lv[l].Lc, lv[l].Za, lv[l].Zb, lv[l].zb, x);
-        else k_bcr_backsub<<<(int)((odd + 3) / 4), 128, 0, st>>>(lv[l].m, stride, lv[l].Lc, lv[l].Za, lv[l].Zb, lv[l].zb, x);
-        nk++;
+        const int64_t stride = (int64_t)1 << l, odd = lv[l].m / 2;
+        const double *Lc = ws + lv[l].Lc, *Za = ws + lv[l].Za, *Zb = ws + lv[l].Zb, *zb = ws + lv[l].zb;
+        if (cid) k_bcr_backsub_iso<<<(int)((odd + 3) / 4), 128, 0, st>>>(lv[l].m, stride, cid, Lc, Za, Zb, zb, x);
+        else k_bcr_backsub<<<(int)((odd + 3) / 4), 128, 0, st>>>(lv[l].m, stride, Lc, Za, Zb, zb, x);
     }
-    if (launches) *launches = nk;
+    if (launches) *launches = 3 * nl + 1;
+    return cudaGetLastError();
+}
+
+// the selected inversion's workspace: the levels, then the tail of bcr_tail
+int64_t chains_marginals_workspace_bytes(int64_t n_states) { return bcr_tail(n_states).selinv_end * 8; }
+
+cudaError_t chains_marginals_launch(int64_t n_chains, const int64_t* offs, int64_t uniform, int64_t n_states, const double* D, const double* E,
+                                    double* cov, double* cross, double* ws, int sms, cudaStream_t st, int* launches) {
+    BcrLevel lv[64];
+    int64_t end;
+    const int nl = bcr_levels(n_states, lv, &end);
+    const BcrTail tail = bcr_tail(n_states, lv, nl);
+    int64_t* cid = reinterpret_cast<int64_t*>(ws + tail.cid);
+    double* b0 = ws + tail.b0;
+    double* nbr[65];                                                // level l's neighbour blocks (l >= 1; NULL: none)
+    for (int l = 0; l < 65; l++) nbr[l] = l < 64 && tail.nbr[l] >= 0 ? ws + tail.nbr[l] : nullptr;
+    cudaError_t e = cudaMemsetAsync(b0, 0, (size_t)n_states * 15 * 8, st);
+    if (e != cudaSuccess) return e;
+    const int64_t blocks = (n_states + 255) / 256, cap = (int64_t)sms * 8;
+    k_chain_ids<<<(int)(blocks < cap ? blocks : cap), 256, 0, st>>>(n_chains, offs, uniform, n_states, cid);
+    bcr_forward(lv, nl, D, E, b0, ws, cid, st);
+    k_bcr_selinv_root<<<1, 32, 0, st>>>(nl ? ws + lv[nl - 1].D : D, cov);
+    for (int l = nl - 1; l >= 0; l--) {
+        const int64_t odd = lv[l].m / 2;
+        k_bcr_selinv_iso<<<(int)((odd + 3) / 4), 128, 0, st>>>(lv[l].m, (int64_t)1 << l, cid, ws + lv[l].Lc, ws + lv[l].Za, ws + lv[l].Zb,
+                                                               nbr[l + 1], cov, nbr[l], l ? nullptr : cross);
+    }
+    if (launches) *launches = 3 * nl + 2;
     return cudaGetLastError();
 }
 

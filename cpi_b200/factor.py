@@ -543,6 +543,30 @@ def chains_lm_step(model, states, records, lin, chain_offsets, prior=None, lam=1
     Returns (new_states, delta [N,15], cost per chain before the step [n_chains] = sum of e^T P^-1 e + the moved priors' f')."""
     import torch
 
+    (C, offs, S), X, (G11, G12, G22, g1, g2, f), (pi_a, pr_c, pf_c) = _linearized(model, states, records, lin, chain_offsets, prior, stream,
+                                                                                  state_priors, state_prior_loss)
+    D, E, rhs = chains_assemble(G11, G12, G22, g1, g2, chain_offsets, lam, pi_a, pr_c, diagonal_damping=diagonal_damping, n_chains=C, stream=stream)
+    dx = chain_solve(D, E, rhs, stream=stream)
+    dev, lib, f64 = X.device, capi.load(), dict(dtype=torch.float64, device=X.device)
+    # per-chain cost: one chain sums like chain_lm_step always has; many chains sum their factors' f in a fixed order
+    # (cpi_imu_chains_cost_sum: an atomic scatter-add would give different bits from run to run)
+    if C == 1:
+        cost = f.sum().reshape(1)
+    else:
+        cost = torch.empty(C, **f64)
+        _launch(lib.cpi_imu_chains_cost_sum, dev, stream, C, _tptr(offs), S, _tptr(f), _tptr(cost))
+    if pf_c is not None:
+        cost = cost + pf_c
+    return retract(X, dx, stream=stream), dx, cost
+
+
+def _linearized(model, states, records, lin, chain_offsets, prior, stream, state_priors, state_prior_loss):
+    """What chains_lm_step and chains_marginals do before the assembly: the layout and argument checks, the state priors (their one
+    host read), the factors' state indices, the buffers and one _linearize at the states.  Returns ((C, offs, S), X [N,16], the
+    blocks (G11, G12, G22, g1, g2, f) with the state priors folded in, and the chain prior as the assembly and the cost read it:
+    (info, rhs, f), each possibly None)."""
+    import torch
+
     dev = states.device
     N = states.numel() // 16
     C, offs, S = _chain_layout(chain_offsets, dev, n_states=N)
@@ -575,19 +599,7 @@ def chains_lm_step(model, states, records, lin, chain_offsets, prior=None, lam=1
     with torch.cuda.device(dev), torch.cuda.stream(stream):
         _linearize(lib, _stream(dev, stream), model, X, records.contiguous(), lin.contiguous(), idx_i, idx_j, (e, H1, H2, G11, G12, G22, g1, g2, f),
                    (pi, pr, pf, lin0, first), (x0, pr_c, pf_c), sps, pi_r)
-    D, E, rhs = chains_assemble(G11, G12, G22, g1, g2, chain_offsets, lam, pi_r if single else pi, pr_c, diagonal_damping=diagonal_damping,
-                                n_chains=C, stream=stream)
-    dx = chain_solve(D, E, rhs, stream=stream)
-    # per-chain cost: one chain sums like chain_lm_step always has; many chains sum their factors' f in a fixed order
-    # (cpi_imu_chains_cost_sum: an atomic scatter-add would give different bits from run to run)
-    if C == 1:
-        cost = f.sum().reshape(1)
-    else:
-        cost = torch.empty(C, **f64)
-        _launch(lib.cpi_imu_chains_cost_sum, dev, stream, C, _tptr(offs), S, _tptr(f), _tptr(cost))
-    if pf_c is not None:
-        cost = cost + pf_c
-    return retract(X, dx, stream=stream), dx, cost
+    return (C, offs, S), X, (G11, G12, G22, g1, g2, f), (pi_r if single else pi, pr_c, pf_c)
 
 
 def _linearize(lib, sp, model, X, records, lin, idx_i, idx_j, blocks, prior, moved, sps, pi_r):
@@ -675,6 +687,57 @@ def chains_solve(D, E, rhs, chain_offsets, n_chains=None, workspace=None, stream
     _launch(lib.cpi_imu_chains_solve, dev, stream, C, _tptr(offs), S, N, _tptr(D.contiguous()), _tptr(E.contiguous()), _tptr(rhs.contiguous()),
             _tptr(x), _tptr(workspace))
     return x
+
+
+def chains_covariance(D, E, chain_offsets, cross=False, n_chains=None, workspace=None, stream=None):
+    """The diagonal blocks and the blocks next to them of A^-1, A = tridiag(E^T, D, E) the system chains_solve solves, by selected
+    inversion of its block cyclic reduction (cpi_imu_chains_marginals; DESIGN.md section 3j).  D [N,225], E [N-1,225] as chains_assemble
+    returns them; chain_offsets as chains_assemble.  Every coupling between two chains is structurally absent: a chain that is not SPD
+    gets NaN blocks and leaves every other chain as it is.  workspace: a float64 CUDA tensor of at least
+    cpi_imu_chains_marginals_workspace bytes, or None (allocated).  The call inverts whatever system it is given: marginal covariances
+    need the undamped system at the estimate (chains_marginals).  Returns (cov [N,225] with cov[k] = (A^-1)_{k,k}, exactly symmetric;
+    with cross, [N - n_chains, 225] with chain c's slot o[c] - c + j = (A^-1)_{o[c]+j, o[c]+j+1}, the factors' order; else None)."""
+    import torch
+
+    for name, t in (("D", D), ("E", E), ("workspace", workspace)):
+        if t is not None and (not isinstance(t, torch.Tensor) or t.dtype != torch.float64):
+            raise ValueError(f"{name} must be a float64 tensor")
+    N = D.numel() // 225
+    if N < 1 or D.numel() != 225 * N or (E.numel() if E is not None else 0) != 225 * (N - 1):
+        raise ValueError("D needs 225 doubles per state (at least one) and E 225 per state but the last")
+    if isinstance(chain_offsets, torch.Tensor) and chain_offsets.numel() - 1 > N:
+        raise ValueError(f"chain_offsets has {chain_offsets.numel()} entries: more chains than the {N} states")
+    if isinstance(chain_offsets, torch.Tensor) and n_chains is not None and n_chains != chain_offsets.numel() - 1:
+        raise ValueError(f"chain_offsets has {chain_offsets.numel()} entries, not n_chains + 1 = {n_chains + 1}")
+    lib = capi.load()
+    dev = D.device
+    C, offs, S = _chain_layout(chain_offsets, dev, n_states=N, n_chains=n_chains)
+    nbytes = int(lib.cpi_imu_chains_marginals_workspace(C, N))
+    if nbytes < 0:
+        raise ValueError(f"{C} chains over {N} states: every chain holds a state")
+    if workspace is not None and (workspace.numel() * 8 < nbytes or not workspace.is_contiguous()):
+        raise ValueError(f"workspace needs {nbytes} contiguous bytes (cpi_imu_chains_marginals_workspace), got {workspace.numel() * 8}")
+    _check_f64(dev, D=D, E=E, workspace=workspace)
+    if workspace is None:
+        workspace = torch.empty((nbytes + 7) // 8, dtype=torch.float64, device=dev)
+    cov = torch.empty((N, 225), dtype=torch.float64, device=dev)
+    cr = torch.empty((N - C, 225), dtype=torch.float64, device=dev) if cross else None
+    _launch(lib.cpi_imu_chains_marginals, dev, stream, C, _tptr(offs), S, N, _tptr(D.contiguous()), _tptr(None if E is None else E.contiguous()),
+            _tptr(cov), _tptr(cr), _tptr(workspace))
+    return cov, cr
+
+
+def chains_marginals(model, states, records, lin, chain_offsets, prior=None, state_priors=None, state_prior_loss=None, cross=False, stream=None):
+    """Marginal covariances of every keyframe of many IMU chains at the states (GTSAM's Marginals / BatchFixedLagSmoother::
+    marginalCovariance; DESIGN.md section 3j): the linearisation of chains_lm_step at `states` (the chain prior moved there by prior_at,
+    the state priors folded in, robust weights frozen at `states` as GTSAM linearises a robust factor for Marginals), assembled with
+    lambda = 0, then chains_covariance.  Arguments as chains_lm_step; call it at an estimate (chains_lm's result).  Long IMU-only chains
+    without priors on later states are numerically singular in fp64: their covariances are meaningless.  Returns (cov [N,225],
+    cross [N - n_chains,225] or None) as chains_covariance, in the tangent space of retract at the states."""
+    (C, _, _), _, (G11, G12, G22, g1, g2, _), (pi_a, pr_c, _) = _linearized(model, states, records, lin, chain_offsets, prior, stream,
+                                                                            state_priors, state_prior_loss)
+    D, E, _ = chains_assemble(G11, G12, G22, g1, g2, chain_offsets, 0.0, pi_a, pr_c, n_chains=C, stream=stream)
+    return chains_covariance(D, E, chain_offsets, cross=cross, n_chains=C, stream=stream)
 
 
 def chains_lm(model, states, records, lin, chain_offsets, prior=None, lam=1e-5, diagonal_damping=True, params=None, max_rounds=200, check_every=8,

@@ -447,6 +447,26 @@ int cpi_imu_state_priors_robust(int64_t n, const int32_t* loss, const double* lo
                                 double* info_out, double* rhs_out, double* f_out, void* stream);
 
 /*
+ * Marginal covariances of many chains (DESIGN.md section 3j): what GTSAM's Marginals / BatchFixedLagSmoother::marginalCovariance give
+ * for every keyframe of a window, for every chain at once.  fp64, DEVICE pointers, asynchronous on `stream`, no allocation.  PARITY
+ * UNPINNED; tests/test_chain_marginals.py holds the numpy statement of the level walk.
+ *
+ *   cpi_imu_chains_marginals   the diagonal blocks and the blocks next to them of A^-1, A = tridiag(E^T, D, E) the system of
+ *       cpi_imu_chains_solve (same layout, same validation, same error codes): cov[k] = (A^-1)_{k,k} (device double[n_states*225],
+ *       column-major, exactly symmetric) and, unless cross is NULL, cross[o[c] - c + j] = (A^-1)_{o[c]+j, o[c]+j+1} for j < S_c - 1
+ *       (device double[(n_states - n_chains)*225], the factors' order).  Selected inversion of the block cyclic reduction: the forward
+ *       phase of cpi_imu_chains_solve on a zero right-hand side, then one launch per level top-down (3 log2(n_states) + 2 launches in
+ *       all).  Every coupling between two chains is structurally absent: a chain that is not SPD gets NaN blocks, and only that chain.
+ *       workspace: cpi_imu_chains_marginals_workspace(n_chains, n_states) bytes.
+ *   The call inverts whatever system it is given.  A marginal covariance needs the UNDAMPED system (lambda = 0) at the estimate:
+ *   factor.chains_marginals assembles it.  Long IMU-only chains without priors on later states are numerically singular in fp64
+ *   (DESIGN.md sections 3e, 3f): their covariances are meaningless (finite or not), as is any fp64 inverse of that system.
+ */
+int64_t cpi_imu_chains_marginals_workspace(int64_t n_chains, int64_t n_states);
+int cpi_imu_chains_marginals(int64_t n_chains, const int64_t* chain_offsets, int64_t chain_uniform, int64_t n_states,
+                             const double* D, const double* E, double* cov, double* cross, void* workspace, void* stream);
+
+/*
  * Re-preintegration of the windows whose bias estimate left the records' linearisation point (DESIGN.md section 3i): the
  * re-integration VINS-Mono and OKVIS run between solves, on the device.  A factor corrects its record to the bias of its state i
  * only to first order (J_q, J_a, J_b, H_a, H_b; model 2 also O_a, O_b in the orientation), which limits accuracy once the
