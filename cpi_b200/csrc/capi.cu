@@ -6,6 +6,7 @@
 #include <cstdio>
 #include <cstring>
 #include <mutex>
+#include <optional>
 #include <string>
 
 #include "cpi_common.cuh"
@@ -498,13 +499,19 @@ int cpi_imu_chain_assemble(int64_t n_factors, const double* G11, const double* G
 }  // extern "C"
 
 namespace {
-// the chain layout shared by the many-chain entry points: chain_offsets (device, not inspected here) or chain_uniform >= 1 states per chain
-int chain_layout_check(int64_t n_chains, const int64_t* chain_offsets, int64_t chain_uniform) {
+// the chain layout shared by the many-chain entry points: chain_offsets (device, not inspected here) or chain_uniform >= 1 states per chain;
+// n_states, where the entry point takes it, is the layout's state count
+int chain_layout_check(int64_t n_chains, const int64_t* chain_offsets, int64_t chain_uniform, std::optional<int64_t> n_states = std::nullopt) {
     if (n_chains < 0) return fail(CPI_EINVAL, "negative count");
     if (n_chains > ((int64_t)1 << 31)) return fail(CPI_EINVAL, "too many chains (%lld; at most 2^31 per call)", (long long)n_chains);
     if (!chain_offsets && chain_uniform < 1) return fail(CPI_EINVAL, "chain_uniform must be >= 1 state per chain (got %lld)", (long long)chain_uniform);
     if (!chain_offsets && n_chains > 0 && chain_uniform > ((int64_t)1 << 40) / n_chains)
         return fail(CPI_EINVAL, "chain_uniform out of range: %lld x %lld states", (long long)n_chains, (long long)chain_uniform);
+    if (!n_states) return CPI_OK;
+    if (*n_states < n_chains) return fail(CPI_EINVAL, "n_states (%lld) below n_chains (%lld): every chain holds a state", (long long)*n_states,
+                                          (long long)n_chains);
+    if (!chain_offsets && *n_states != n_chains * chain_uniform)
+        return fail(CPI_EINVAL, "n_states (%lld) must be n_chains x chain_uniform (%lld)", (long long)*n_states, (long long)(n_chains * chain_uniform));
     return CPI_OK;
 }
 }  // namespace
@@ -580,12 +587,8 @@ int64_t cpi_imu_chains_solve_workspace(int64_t n_chains, int64_t n_states) {
 
 int cpi_imu_chains_solve(int64_t n_chains, const int64_t* chain_offsets, int64_t chain_uniform, int64_t n_states, const double* D, const double* E,
                          const double* rhs, double* x, void* workspace, void* stream) {
-    int rc = chain_layout_check(n_chains, chain_offsets, chain_uniform);
+    int rc = chain_layout_check(n_chains, chain_offsets, chain_uniform, n_states);
     if (rc) return rc;
-    if (n_states < n_chains) return fail(CPI_EINVAL, "n_states (%lld) below n_chains (%lld): every chain holds a state", (long long)n_states,
-                                         (long long)n_chains);
-    if (!chain_offsets && n_states != n_chains * chain_uniform)
-        return fail(CPI_EINVAL, "n_states (%lld) must be n_chains x chain_uniform (%lld)", (long long)n_states, (long long)(n_chains * chain_uniform));
     if (n_chains == 0) return CPI_OK;
     if (!D || !rhs || !x || !workspace || (n_states > 1 && !E)) return fail(CPI_EINVAL, "null pointer argument");
     DevInfo d;
@@ -604,12 +607,8 @@ int64_t cpi_imu_chains_marginals_workspace(int64_t n_chains, int64_t n_states) {
 
 int cpi_imu_chains_marginals(int64_t n_chains, const int64_t* chain_offsets, int64_t chain_uniform, int64_t n_states, const double* D, const double* E,
                              double* cov, double* cross, void* workspace, void* stream) {
-    int rc = chain_layout_check(n_chains, chain_offsets, chain_uniform);
+    int rc = chain_layout_check(n_chains, chain_offsets, chain_uniform, n_states);
     if (rc) return rc;
-    if (n_states < n_chains) return fail(CPI_EINVAL, "n_states (%lld) below n_chains (%lld): every chain holds a state", (long long)n_states,
-                                         (long long)n_chains);
-    if (!chain_offsets && n_states != n_chains * chain_uniform)
-        return fail(CPI_EINVAL, "n_states (%lld) must be n_chains x chain_uniform (%lld)", (long long)n_states, (long long)(n_chains * chain_uniform));
     if (n_chains == 0) return CPI_OK;
     if (!D || !cov || !workspace || (n_states > 1 && !E)) return fail(CPI_EINVAL, "null pointer argument");
     DevInfo d;
@@ -628,12 +627,8 @@ int cpi_imu_chains_lm_update(int64_t n_chains, const int64_t* chain_offsets, int
                              const double* D, const double* E, const double* damp, const double* delta, const double* states_new, double* states,
                              double* lambda, double* cost, int32_t* status, int32_t* iterations, int32_t* tries, int32_t* any_running,
                              void* workspace, void* stream) {
-    int rc = chain_layout_check(n_chains, chain_offsets, chain_uniform);
+    int rc = chain_layout_check(n_chains, chain_offsets, chain_uniform, n_states);
     if (rc) return rc;
-    if (n_states < n_chains) return fail(CPI_EINVAL, "n_states (%lld) below n_chains (%lld): every chain holds a state", (long long)n_states,
-                                         (long long)n_chains);
-    if (!chain_offsets && n_states != n_chains * chain_uniform)
-        return fail(CPI_EINVAL, "n_states (%lld) must be n_chains x chain_uniform (%lld)", (long long)n_states, (long long)(n_chains * chain_uniform));
     if (!params) return fail(CPI_EINVAL, "null pointer argument (params)");
     const cpi_lm_params& p = *params;
     if (!(p.lambda_factor > 1.0)) return fail(CPI_EINVAL, "lambda_factor must be > 1 (got %g)", p.lambda_factor);
@@ -731,7 +726,7 @@ int cpi_imu_state_priors_robust(int64_t n, const int32_t* loss, const double* lo
     return CPI_OK;
 }
 
-int64_t cpi_imu_chain_solve_workspace(int64_t n_states) { return n_states < 0 ? (int64_t)CPI_EINVAL : cpi::chain_solve_workspace_bytes(n_states); }
+int64_t cpi_imu_chain_solve_workspace(int64_t n_states) { return n_states < 0 ? (int64_t)CPI_EINVAL : cpi::chains_solve_workspace_bytes(n_states); }
 
 int cpi_imu_chain_solve(int64_t n_states, const double* D, const double* E, const double* rhs, double* x, void* workspace, void* stream) {
     if (n_states < 0) return fail(CPI_EINVAL, "negative count");
@@ -741,7 +736,7 @@ int cpi_imu_chain_solve(int64_t n_states, const double* D, const double* E, cons
     int rc = device_info(d);
     if (rc) return rc;
     int launches = 0;
-    CU(cpi::chain_solve_launch(n_states, D, E, rhs, x, (double*)workspace, (cudaStream_t)stream, &launches));
+    CU(cpi::chains_solve_launch(1, nullptr, n_states, n_states, D, E, rhs, x, (double*)workspace, d.sms, (cudaStream_t)stream, &launches));
     g_launches += launches;
     return CPI_OK;
 }

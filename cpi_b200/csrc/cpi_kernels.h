@@ -59,11 +59,8 @@ cudaError_t whiten_launch(int rd, int64_t n, const double* records, const double
 cudaError_t chains_assemble_launch(int64_t n_chains, const int64_t* offs, int64_t uniform, const double* G11, const double* G12, const double* G22,
                                    const double* g1, const double* g2, double lambda, int diagonal_damping, const double* prior_info,
                                    const double* prior_rhs, double* D, double* E, double* rhs, int sms, cudaStream_t st);
-int64_t chain_solve_workspace_bytes(int64_t n_states);
-// cid (device int64[n_states], may be NULL): every state's chain; given, couplings between chains are never loaded (the isolated solve)
-cudaError_t chain_solve_launch(int64_t n_states, const double* D, const double* E, const double* b, double* x, double* ws, cudaStream_t st, int* launches,
-                               const int64_t* cid = nullptr);
-// the per-chain-lambda assembly and the isolated solve of many chains (cpi_imu_chains_assemble_lm / cpi_imu_chains_solve)
+// the per-chain-lambda assembly, and the solve with couplings between chains never loaded (cpi_imu_chains_assemble_lm /
+// cpi_imu_chains_solve; cpi_imu_chain_solve is its one-chain case)
 cudaError_t chains_assemble_lm_launch(int64_t n_chains, const int64_t* offs, int64_t uniform, const double* G11, const double* G12, const double* G22,
                                       const double* g1, const double* g2, const double* lams, int diagonal_damping, const double* prior_info,
                                       const double* prior_rhs, double* D, double* E, double* rhs, double* damp, int sms, cudaStream_t st);

@@ -1,5 +1,5 @@
 // Levenberg-Marquardt over many IMU chains on the device (DESIGN.md section 3f): the pieces a round needs besides the linearisation,
-// the per-chain-damped assembly (k_chain_assemble_lm) and the isolated solve (k_bcr_*_iso) of solve.cu.
+// the per-chain-damped assembly (k_chain_assemble_lm) and the isolated solve (chains_solve_launch) of solve.cu.
 //   k_factor_cost (K9)  the whitened cost f = e^T P_meas^-1 e of each factor at given states: evaluateError's residual without
 //                       Jacobians, the warp Cholesky of P_meas and one forward substitution -- k_factor_hessian's f without its blocks.
 //   k_lm_terms          per state k: the model decrease term delta_k^T (2 rhs_k - (H delta)_k) of the UNDAMPED system (H delta from

@@ -128,15 +128,12 @@ __global__ void k_chain_assemble_lm(int64_t n_chains, const int64_t* offs, int64
 }
 
 // ---- block cyclic reduction ---------------------------------------------------------------------------------------------------------
-// Level with m nodes: row i reads  E[i-1]^T x_{i-1} + D[i] x_i + E[i] x_{i+1} = b[i].
-// ISO (cpi_imu_chains_solve): node i of the level sits at original state i * stride, cid[] holds each original state's chain, and a
-// coupling between nodes of different chains is structurally absent: not loaded, not multiplied, written as exact 0.  With finite
-// input those couplings are exact zeros anyway, so the ISO kernels give the plain kernels' bits; a NaN stays inside its chain.
-#define CPI_SAME(p, q) (!ISO || cid[(p) * stride] == cid[(q) * stride])
+// Level with m nodes: row i reads  E[i-1]^T x_{i-1} + D[i] x_i + E[i] x_{i+1} = b[i].  Node i of the level sits at original state
+// i * stride, and cid[] holds each original state's chain.  The coupling of two nodes is used only when both share a chain: otherwise
+// it is not loaded, not multiplied, and written as exact 0, so a NaN stays inside its chain.
 #define SAME(p, q) (cid[(p) * stride] == cid[(q) * stride])
 
 // Odd node i = 2t+1:  D_i = Lc Lc^T,  Za = Lc^-1 E[i-1]^T,  Zb = Lc^-1 E[i] (if i+1 < m),  zb = Lc^-1 b_i      (kept for the back-substitution)
-template <bool ISO>
 CPI_DEV void bcr_eliminate(int64_t m, int64_t stride, const int64_t* cid, const double* D, const double* E, const double* b, double* Lc, double* Za,
                            double* Zb, double* zb) {
     __shared__ double sL[4][15 * 16];
@@ -149,8 +146,8 @@ CPI_DEV void bcr_eliminate(int64_t m, int64_t stride, const int64_t* cid, const 
     __syncwarp();
     warp_chol15(L, lane);
     for (int k = lane; k < 225; k += 32) { const int r = k % 15, c = k / 15; Lc[t * 225 + k] = (r >= c) ? L[r * 16 + c] : 0.0; }
-    const bool has_left = CPI_SAME(i - 1, i);
-    const bool has_right = i + 1 < m && CPI_SAME(i + 1, i);
+    const bool has_left = SAME(i - 1, i);
+    const bool has_right = i + 1 < m && SAME(i + 1, i);
     if (lane < 31) {
         double y[15];
         if (lane < 15) {
@@ -165,7 +162,7 @@ CPI_DEV void bcr_eliminate(int64_t m, int64_t stride, const int64_t* cid, const 
         }
         fwd15(L, y);
         double* dst = lane < 15 ? Za + t * 225 + 15 * lane : (lane < 30 ? Zb + t * 225 + 15 * (lane - 15) : zb + t * 15);
-        if (ISO && ((lane < 15 && !has_left) || (lane >= 15 && lane < 30 && !has_right))) {
+        if ((lane < 15 && !has_left) || (lane >= 15 && lane < 30 && !has_right)) {
 #pragma unroll
             for (int r = 0; r < 15; r++) y[r] = 0.0;
         }
@@ -214,49 +211,9 @@ CPI_DEV void bcr_reduce_iso(int64_t m, int64_t stride, const int64_t* cid, const
     }
 }
 
-__global__ void __launch_bounds__(128) k_bcr_eliminate(int64_t m, const double* D, const double* E, const double* b, double* Lc, double* Za, double* Zb, double* zb) {
-    bcr_eliminate<false>(m, 0, nullptr, D, E, b, Lc, Za, Zb, zb);
-}
-// (k_bcr_reduce keeps its own copy of the body: through bcr_reduce<false> its register allocation changes)
-__global__ void __launch_bounds__(128) k_bcr_reduce(int64_t m, const double* D, const double* b, const double* Za, const double* Zb, const double* zb,
-                                                    double* Dn, double* En, double* bn) {
-    __shared__ double sZ[4][4][225 + 15];      // [warp][ZbL | ZaR | ZbR | (zbL, zbR)]
-    const int wib = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int64_t u = (int64_t)blockIdx.x * 4 + wib;
-    const int64_t j = 2 * u;
-    if (j >= m) return;
-    const bool hasL = j >= 1, hasR = j + 1 < m, hasRR = j + 2 < m;
-    const int64_t tl = (j - 2) / 2, tr = j / 2;                     // odd-node slots of j-1 and j+1
-    double *ZbL = sZ[wib][0], *ZaR = sZ[wib][1], *ZbR = sZ[wib][2], *zz = sZ[wib][3];
-    for (int k = lane; k < 225; k += 32) {
-        ZbL[k] = hasL ? Zb[tl * 225 + k] : 0.0;
-        ZaR[k] = hasR ? Za[tr * 225 + k] : 0.0;
-        ZbR[k] = hasRR ? Zb[tr * 225 + k] : 0.0;
-    }
-    if (lane < 15) { zz[lane] = hasL ? zb[tl * 15 + lane] : 0.0; zz[15 + lane] = hasR ? zb[tr * 15 + lane] : 0.0; }
-    __syncwarp();
-    for (int k = lane; k < 225; k += 32) {
-        const int r = k % 15, c = k / 15;                          // column-major 15x15; Z matrices are column-major: Z[q + 15 col]
-        double d = D[j * 225 + k], en = 0.0;
-#pragma unroll
-        for (int q = 0; q < 15; q++) {
-            d = fma(-ZbL[q + 15 * r], ZbL[q + 15 * c], d);
-            d = fma(-ZaR[q + 15 * r], ZaR[q + 15 * c], d);
-            en = fma(-ZaR[q + 15 * r], ZbR[q + 15 * c], en);
-        }
-        Dn[u * 225 + k] = d;
-        if (hasRR) En[u * 225 + k] = en;
-    }
-    if (lane < 15) {
-        double v = b[j * 15 + lane];
-#pragma unroll
-        for (int q = 0; q < 15; q++) { v = fma(-ZbL[q + 15 * lane], zz[q], v); v = fma(-ZaR[q + 15 * lane], zz[15 + q], v); }
-        bn[u * 15 + lane] = v;
-    }
-}
 __global__ void __launch_bounds__(128) k_bcr_eliminate_iso(int64_t m, int64_t stride, const int64_t* cid, const double* D, const double* E, const double* b,
                                                            double* Lc, double* Za, double* Zb, double* zb) {
-    bcr_eliminate<true>(m, stride, cid, D, E, b, Lc, Za, Zb, zb);
+    bcr_eliminate(m, stride, cid, D, E, b, Lc, Za, Zb, zb);
 }
 __global__ void __launch_bounds__(128) k_bcr_reduce_iso(int64_t m, int64_t stride, const int64_t* cid, const double* D, const double* b, const double* Za,
                                                         const double* Zb, const double* zb, double* Dn, double* En, double* bn) {
@@ -264,7 +221,7 @@ __global__ void __launch_bounds__(128) k_bcr_reduce_iso(int64_t m, int64_t strid
 }
 
 // last level (one node): x = D^-1 b
-__global__ void k_bcr_root(const double* D, const double* b, double* x, int64_t stride) {
+__global__ void k_bcr_root(const double* D, const double* b, double* x) {
     __shared__ double L[15 * 16];
     const int lane = threadIdx.x;
     for (int k = lane; k < 225; k += 32) { const int r = k % 15, c = k / 15; if (r >= c) L[r * 16 + c] = D[k]; }
@@ -279,11 +236,9 @@ __global__ void k_bcr_root(const double* D, const double* b, double* x, int64_t 
     for (int q = 0; q < 15; q++) if (lane == q) r = y[q];
     const double xv = warp_bwd15(L, r, lane);
     if (lane < 15) x[lane] = xv;
-    (void)stride;
 }
 
 // odd node i = 2t+1 of a level whose nodes sit at original indices i * stride:  Lc^T x_i = zb - Za x_{i-1} - Zb x_{i+1}
-template <bool ISO>
 CPI_DEV void bcr_backsub(int64_t m, int64_t stride, const int64_t* cid, const double* Lc, const double* Za, const double* Zb, const double* zb, double* x) {
     __shared__ double sL[4][15 * 16];
     const int wib = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -293,8 +248,8 @@ CPI_DEV void bcr_backsub(int64_t m, int64_t stride, const int64_t* cid, const do
     double* L = sL[wib];
     for (int k = lane; k < 225; k += 32) { const int r = k % 15, c = k / 15; if (r >= c) L[r * 16 + c] = Lc[t * 225 + k]; }
     __syncwarp();
-    const bool has_left = CPI_SAME(i - 1, i);
-    const bool has_right = i + 1 < m && CPI_SAME(i + 1, i);
+    const bool has_left = SAME(i - 1, i);
+    const bool has_right = i + 1 < m && SAME(i + 1, i);
     double r = 0.0;
     if (lane < 15) {
         r = zb[t * 15 + lane];
@@ -309,18 +264,14 @@ CPI_DEV void bcr_backsub(int64_t m, int64_t stride, const int64_t* cid, const do
     const double xv = warp_bwd15(L, r, lane);
     if (lane < 15) x[i * stride * 15 + lane] = xv;
 }
-#undef CPI_SAME
 #undef SAME
 
-__global__ void __launch_bounds__(128) k_bcr_backsub(int64_t m, int64_t stride, const double* Lc, const double* Za, const double* Zb, const double* zb, double* x) {
-    bcr_backsub<false>(m, stride, nullptr, Lc, Za, Zb, zb, x);
-}
 __global__ void __launch_bounds__(128) k_bcr_backsub_iso(int64_t m, int64_t stride, const int64_t* cid, const double* Lc, const double* Za, const double* Zb,
                                                          const double* zb, double* x) {
-    bcr_backsub<true>(m, stride, cid, Lc, Za, Zb, zb, x);
+    bcr_backsub(m, stride, cid, Lc, Za, Zb, zb, x);
 }
 
-// the chain of every state, for the ISO kernels (grid-stride; a device-resident layout is searched per state)
+// the chain of every state, for the level kernels (grid-stride; a device-resident layout is searched per state)
 __global__ void k_chain_ids(int64_t n_chains, const int64_t* offs, int64_t uniform, int64_t n_states, int64_t* cid) {
     for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < n_states; k += (int64_t)gridDim.x * blockDim.x) {
         int64_t c;
@@ -518,19 +469,13 @@ static void bcr_forward(const BcrLevel* lv, int nl, const double* D, const doubl
         const double *cD = l ? ws + lv[l - 1].D : D, *cE = l ? ws + lv[l - 1].E : E, *cb = l ? ws + lv[l - 1].b : b;
         const int64_t odd = L.m / 2, even = (L.m + 1) / 2;
         const int64_t stride = (int64_t)1 << l;
-        if (cid) {
-            k_bcr_eliminate_iso<<<(int)((odd + 3) / 4), 128, 0, st>>>(L.m, stride, cid, cD, cE, cb, ws + L.Lc, ws + L.Za, ws + L.Zb, ws + L.zb);
-            k_bcr_reduce_iso<<<(int)((even + 3) / 4), 128, 0, st>>>(L.m, stride, cid, cD, cb, ws + L.Za, ws + L.Zb, ws + L.zb, ws + L.D, ws + L.E,
-                                                                     ws + L.b);
-        } else {
-            k_bcr_eliminate<<<(int)((odd + 3) / 4), 128, 0, st>>>(L.m, cD, cE, cb, ws + L.Lc, ws + L.Za, ws + L.Zb, ws + L.zb);
-            k_bcr_reduce<<<(int)((even + 3) / 4), 128, 0, st>>>(L.m, cD, cb, ws + L.Za, ws + L.Zb, ws + L.zb, ws + L.D, ws + L.E, ws + L.b);
-        }
+        k_bcr_eliminate_iso<<<(int)((odd + 3) / 4), 128, 0, st>>>(L.m, stride, cid, cD, cE, cb, ws + L.Lc, ws + L.Za, ws + L.Zb, ws + L.zb);
+        k_bcr_reduce_iso<<<(int)((even + 3) / 4), 128, 0, st>>>(L.m, stride, cid, cD, cb, ws + L.Za, ws + L.Zb, ws + L.zb, ws + L.D, ws + L.E, ws + L.b);
     }
 }
-// What follows the levels (offsets in doubles): the isolated solve's chain id of every state (int64), then the selected inversion's
+// What follows the levels (offsets in doubles): the solve's chain id of every state (int64), then the selected inversion's
 // zero right-hand side [n_states, 15] for the forward phase and the neighbour blocks Sigma_{k,k+1} of every level l >= 1 with two nodes
-// or more (m_l - 1 blocks each, level order).  solve_end / selinv_end: the doubles the isolated solve / the selected inversion take.
+// or more (m_l - 1 blocks each, level order).  solve_end / selinv_end: the doubles the solve / the selected inversion take.
 struct BcrTail { int64_t cid, solve_end, b0, nbr[64], selinv_end; };
 static BcrTail bcr_tail(int64_t n_states, const BcrLevel* lv, int nl) {
     BcrTail t;
@@ -549,34 +494,29 @@ static BcrTail bcr_tail(int64_t n_states) {
     return bcr_tail(n_states, lv, nl);
 }
 
-int64_t chain_solve_workspace_bytes(int64_t n_states) { return bcr_doubles(n_states) * 8; }
-// the isolated solve: the same, followed by the chain id of every state
+// the solve's workspace: the levels, then the chain id of every state
 int64_t chains_solve_workspace_bytes(int64_t n_states) { return bcr_tail(n_states).solve_end * 8; }
 
+// The chain ids, the forward phase, the root and the back-substitution levels.  One state has no level: nothing reads the chain ids
+// and the workspace is not touched (it may be NULL).
 cudaError_t chains_solve_launch(int64_t n_chains, const int64_t* offs, int64_t uniform, int64_t n_states, const double* D, const double* E, const double* b,
                                 double* x, double* ws, int sms, cudaStream_t st, int* launches) {
-    int64_t* cid = reinterpret_cast<int64_t*>(ws + bcr_tail(n_states).cid);
-    const int64_t blocks = (n_states + 255) / 256, cap = (int64_t)sms * 8;
-    k_chain_ids<<<(int)(blocks < cap ? blocks : cap), 256, 0, st>>>(n_chains, offs, uniform, n_states, cid);
-    const cudaError_t e = chain_solve_launch(n_states, D, E, b, x, ws, st, launches, cid);
-    if (launches) *launches += 1;
-    return e;
-}
-
-cudaError_t chain_solve_launch(int64_t n_states, const double* D, const double* E, const double* b, double* x, double* ws, cudaStream_t st, int* launches,
-                               const int64_t* cid) {
     BcrLevel lv[64];
     int64_t end;
     const int nl = bcr_levels(n_states, lv, &end);
+    int64_t* cid = nullptr;
+    if (n_states > 1) {
+        cid = reinterpret_cast<int64_t*>(ws + bcr_tail(n_states, lv, nl).cid);
+        const int64_t blocks = (n_states + 255) / 256, cap = (int64_t)sms * 8;
+        k_chain_ids<<<(int)(blocks < cap ? blocks : cap), 256, 0, st>>>(n_chains, offs, uniform, n_states, cid);
+    }
     bcr_forward(lv, nl, D, E, b, ws, cid, st);
-    k_bcr_root<<<1, 32, 0, st>>>(nl ? ws + lv[nl - 1].D : D, nl ? ws + lv[nl - 1].b : b, x, 1);
+    k_bcr_root<<<1, 32, 0, st>>>(nl ? ws + lv[nl - 1].D : D, nl ? ws + lv[nl - 1].b : b, x);
     for (int l = nl - 1; l >= 0; l--) {
         const int64_t stride = (int64_t)1 << l, odd = lv[l].m / 2;
-        const double *Lc = ws + lv[l].Lc, *Za = ws + lv[l].Za, *Zb = ws + lv[l].Zb, *zb = ws + lv[l].zb;
-        if (cid) k_bcr_backsub_iso<<<(int)((odd + 3) / 4), 128, 0, st>>>(lv[l].m, stride, cid, Lc, Za, Zb, zb, x);
-        else k_bcr_backsub<<<(int)((odd + 3) / 4), 128, 0, st>>>(lv[l].m, stride, Lc, Za, Zb, zb, x);
+        k_bcr_backsub_iso<<<(int)((odd + 3) / 4), 128, 0, st>>>(lv[l].m, stride, cid, ws + lv[l].Lc, ws + lv[l].Za, ws + lv[l].Zb, ws + lv[l].zb, x);
     }
-    if (launches) *launches = 3 * nl + 1;
+    if (launches) *launches = 3 * nl + 1 + (n_states > 1);
     return cudaGetLastError();
 }
 

@@ -151,7 +151,8 @@ def chain_assemble(G11, G12, G22, g1, g2, lam=0.0, prior_info0=None, prior_rhs0=
 
 
 def chain_solve(D, E, rhs, stream=None, workspace=None):
-    """x = A^-1 rhs for the SPD block-tridiagonal A = tridiag(E^T, D, E) by block cyclic reduction on the device (cpi_imu_chain_solve)."""
+    """x = A^-1 rhs for the SPD block-tridiagonal A = tridiag(E^T, D, E) by block cyclic reduction on the device (cpi_imu_chain_solve):
+    chains_solve with every state in one chain, so the NaN of a non-SPD part spreads into the rest through its zero couplings."""
     import torch
 
     lib = capi.load()
@@ -672,8 +673,9 @@ def chains_assemble_lm(G11, G12, G22, g1, g2, chain_offsets, lam, prior_info=Non
 
 
 def chains_solve(D, E, rhs, chain_offsets, n_chains=None, workspace=None, stream=None):
-    """chain_solve with every coupling between two chains structurally absent (cpi_imu_chains_solve): a chain that is not SPD gets NaN
-    and leaves every other chain as it is; on SPD input bitwise chain_solve.  chain_offsets as chains_assemble."""
+    """x = A^-1 rhs by block cyclic reduction with every coupling between two chains structurally absent (cpi_imu_chains_solve): a
+    chain that is not SPD gets NaN and leaves every other chain as it is; on SPD input bitwise chain_solve.  chain_offsets as
+    chains_assemble."""
     import torch
 
     dev = D.device

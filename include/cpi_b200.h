@@ -259,8 +259,9 @@ int cpi_imu_factor_whiten_batch(int model, int64_t n_factors, const double* reco
  *       diagonal damping (or the camera factors of the real graph) restores a well-posed system (DESIGN.md section 5); so do priors
  *       on later states (position fixes: cpi_imu_state_priors_fold, DESIGN.md section 3g).
  *   cpi_imu_chain_solve      x = (that SPD block-tridiagonal matrix)^-1 rhs by block cyclic reduction (Cholesky on the 15x15 pivots):
- *       ~2 log2(n) + 1 kernel launches instead of an n-step sequential block recurrence.  `workspace`: device buffer of
- *       cpi_imu_chain_solve_workspace(n_states) bytes.  The step is then applied with cpi_retract_batch.
+ *       cpi_imu_chains_solve on one chain of n_states states, ~3 log2(n) + 2 kernel launches instead of an n-step sequential block
+ *       recurrence.  `workspace`: device buffer of cpi_imu_chain_solve_workspace(n_states) bytes; with n_states = 1, E and the
+ *       workspace may be NULL.  The step is then applied with cpi_retract_batch.
  * All pointers are DEVICE pointers.  PARITY UNPINNED; validated against banded / dense CPU solves of the same system.
  */
 int cpi_imu_chain_assemble(int64_t n_factors, const double* G11, const double* G12, const double* G22,
@@ -299,8 +300,8 @@ int cpi_imu_chain_solve(int64_t n_states, const double* D, const double* E, cons
  *   cpi_imu_chains_assemble     one block-tridiagonal system over all states: as cpi_imu_chain_assemble per chain (same damping),
  *       prior c on chain c's first state (prior_info / prior_rhs may be NULL), E exactly 0 at chain boundaries, E = n_states - 1
  *       blocks.  cpi_imu_chain_assemble is its n_chains = 1 case.  cpi_imu_chain_solve(n_states, D, E, rhs, ...) then solves every
- *       chain at once: the zero couplings keep the chains exactly decoupled -- PROVIDED EVERY CHAIN IS SPD: a NaN pivot of one chain
- *       spreads into its neighbours through 0 * NaN in the reduction.
+ *       chain at once as one chain: the zero couplings keep the chains exactly decoupled -- PROVIDED EVERY CHAIN IS SPD: a NaN pivot
+ *       of one chain spreads into its neighbours through 0 * NaN in the reduction (cpi_imu_chains_solve keeps it in its chain).
  */
 int cpi_imu_chain_marginalize(int64_t n_chains, const int64_t* chain_offsets, int64_t chain_uniform,
                               const int64_t* n_marg, int64_t n_marg_uniform,
@@ -341,9 +342,10 @@ int cpi_imu_chains_assemble(int64_t n_chains, const int64_t* chain_offsets, int6
  *       chain c's factors, in a fixed order (no atomics: the same bits on every run).  Layout as cpi_imu_chains_assemble.
  *   cpi_imu_chains_assemble_lm   cpi_imu_chains_assemble with lambda[n_chains] (device) per chain; damp (device double[n_states*15],
  *       may be NULL) receives the diagonal the damping added.
- *   cpi_imu_chains_solve         the block cyclic reduction of cpi_imu_chain_solve over n_states = the layout's state count, with every
- *       coupling between two chains structurally absent (not loaded, not multiplied, written as exact 0): a NaN stays in its chain, and
- *       on SPD input the result is cpi_imu_chain_solve's bit for bit.  workspace: cpi_imu_chains_solve_workspace(n_chains, n_states) bytes.
+ *   cpi_imu_chains_solve         block cyclic reduction over n_states = the layout's state count, with every coupling between two
+ *       chains structurally absent (not loaded, not multiplied, written as exact 0): a NaN stays in its chain, and on SPD input the
+ *       result is cpi_imu_chain_solve's (all states one chain) bit for bit.  workspace: cpi_imu_chains_solve_workspace(n_chains, n_states)
+ *       bytes.
  *   cpi_imu_chains_lm_update     the decision above for every RUNNING chain: f_cur / f_new per factor, prior_f_cur / prior_f_new per chain
  *       (NULL: no prior), rhs / D / E / damp / delta of the round, states_new the candidate states; writes lambda, cost, status,
  *       iterations, tries, copies states_new into `states` for the accepted chains, and sets *any_running = 1 (may be NULL; the caller

@@ -1028,7 +1028,7 @@ static void bcr_level(int64_t m, const real* D, const real* Eb, const real* b, r
         mat_zero(Ej, B15);
         const real *ZbL = j >= 1 ? Zb + ((j - 2) / 2) * B15 : 0, *zbL = j >= 1 ? zb + ((j - 2) / 2) * 15 : 0;
         const real *ZaR = j + 1 < m ? Za + (j / 2) * B15 : 0, *ZbR = j + 1 < m ? Zb + (j / 2) * B15 : 0, *zbR = j + 1 < m ? zb + (j / 2) * 15 : 0;
-        for (int c2 = 0; c2 < 15; c2++) {                       /* the products subtracted one by one, interleaved, as k_bcr_reduce */
+        for (int c2 = 0; c2 < 15; c2++) {                       /* the products subtracted one by one, interleaved, as k_bcr_reduce_iso */
             for (int r = 0; r < 15; r++) {
                 real d = E(Dj, 15, r, c2), e = 0;
                 for (int q = 0; q < 15; q++) {

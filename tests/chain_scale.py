@@ -251,7 +251,7 @@ def tie_cases(tol, n_each, seed):
 def bcr_pattern(o, L):
     """What the isolated solve does to a chain of L states at global offset o, level by level until the chain has one node left: per
     surviving state, (odd: eliminated at this level, has_left, has_right).  Level l keeps the states k with k mod 2^l = 0, and node
-    k >> l is odd or even (solve.cu, chain_solve_launch)."""
+    k >> l is odd or even (solve.cu, chains_solve_launch)."""
     out, nodes, lev = [], list(range(o, o + L)), 0
     while len(nodes) > 1:
         out.append(tuple(((k >> lev) & 1, i > 0, i < len(nodes) - 1) for i, k in enumerate(nodes)))

@@ -1,5 +1,5 @@
 """Precision of the solver side of the IMU chain -- the chain marginalisation (K8, cpi_imu_chain_marginalize), the prior move
-(k_prior_at), the chain assembly (k_chain_assemble / _lm), the block cyclic reduction (k_bcr_*, k_bcr_*_iso, k_chain_ids) and the
+(k_prior_at), the chain assembly (k_chain_assemble / _lm), the block cyclic reduction (k_chain_ids, k_bcr_*) and the
 LM model decrease (k_lm_terms, k_lm_decide) -- against an extended-precision truth.
 
 The truths are the long-double build of the oracle's dense statements (oracle/cpi_oracle.c: oracle_chain_marginalize, oracle_local /

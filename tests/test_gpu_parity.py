@@ -554,6 +554,28 @@ def test_chain_assemble_and_block_cyclic_reduction_solve(cuda, n, damping):
         assert err <= 1e-9
 
 
+def test_chain_solve_of_one_state_needs_no_workspace(cuda):
+    """cpi_imu_chain_solve through the C ABI at n_states = 1 with E and the workspace NULL: one state has no level, so the call is the
+    root alone and writes no chain ids.  x = D^-1 rhs under the gate of test_chain_assemble_and_block_cyclic_reduction_solve."""
+    from cpi_b200 import capi
+    torch = cuda
+    rng = np.random.default_rng(11)
+    A = rng.normal(size=(15, 15))
+    Dh = (A @ A.T + 15 * np.eye(15)).reshape(1, 225)                 # symmetric: the same in column-major storage
+    bh = rng.normal(size=(1, 15))
+    D, rhs = torch.from_numpy(Dh).cuda(), torch.from_numpy(bh).cuda()
+    x = torch.full((1, 15), float("nan"), dtype=torch.float64, device="cuda")
+    before = capi.launch_count()
+    capi.check(capi.load().cpi_imu_chain_solve(1, D.data_ptr(), None, rhs.data_ptr(), x.data_ptr(), None, None))
+    torch.cuda.synchronize()
+    assert capi.launch_count() - before == 1
+    xt, x64 = _chain_truth(Dh, np.zeros((0, 225)), bh)
+    nt = np.linalg.norm(xt)
+    err, err64 = np.linalg.norm(x.cpu().numpy() - xt) / nt, np.linalg.norm(x64 - xt) / nt
+    print("one state: device rel err vs refined truth", err, "| fp64 banded Cholesky (CPU)", err64)
+    assert err <= 50 * max(err64, 1e-13)
+
+
 def test_chain_lm_step_reduces_the_cost(cuda):
     """eval -> Hessian blocks -> assemble -> solve -> retract, all on device: a Gauss-Newton step on a perturbed 5k-keyframe chain must
     reduce sum e^T P^-1 e by orders of magnitude (the chain started from the exact prediction has zero residual)."""
