@@ -990,35 +990,33 @@ static void seq_chain(int64_t lo, int64_t hi, const double* D, const double* Eb,
     free(L); free(y);
 }
 
-/* The block cyclic reduction of the whole system (rows 0 .. m-1, couplings as given), level by level in the order of solve.cu:
+/* One level of the block cyclic reduction (rows 0 .. m-1), in the order of solve.cu's forward phase:
  * odd node i: D_i = Lc Lc^T, Za = Lc^-1 E_{i-1}^T, Zb = Lc^-1 E_i (0 for the last node), zb = Lc^-1 b_i; even node j -> node j/2 of the
  * next level: D' = D_j - Zb_{j-1}^T Zb_{j-1} - Za_{j+1}^T Za_{j+1}, b' = b_j - Zb_{j-1}^T zb_{j-1} - Za_{j+1}^T zb_{j+1},
- * E' = -Za_{j+1}^T Zb_{j+1}; one node: x = D^-1 b; back: Lc^T x_i = zb - Za x_{i-1} - Zb x_{i+1}.  Blocks held full (D symmetric);
- * products are subtracted one at a time in the kernels' order, and L^-T runs column by column as warp_bwd15 does. */
-static void bcr_level(int64_t m, const real* D, const real* Eb, const real* b, real* x) {
-    if (m == 1) {
-        real L[B15], v[15];
-        memcpy(L, D, sizeof L);
-        if (!chol15(L)) { for (int r = 0; r < 15; r++) x[r] = NAN; return; }
-        memcpy(v, b, sizeof v);
-        fwd_n(L, v, 1); bwd_col(L, v);
-        memcpy(x, v, sizeof v);
-        return;
-    }
+ * E' = -Za_{j+1}^T Zb_{j+1}.  Blocks held full (D symmetric); products are subtracted one at a time in the kernels' order.
+ * cid (may be NULL: every coupling used as given) [m]: the chain of every node.  With it, as k_bcr_eliminate_iso / k_bcr_reduce_iso, a
+ * coupling between two chains is not read and its Za, Zb or E' is exact 0, so that a NaN stays inside its chain.  The buffer at Lc
+ * (free it) also holds xn [even, 15] for the next level's solution. */
+typedef struct { real *Lc, *Za, *Zb, *zb, *Dn, *En, *bn, *xn; } bcr_t;
+#define SAME(p, q) (!cid || cid[p] == cid[q])
+static void bcr_forward(int64_t m, const int64_t* cid, const real* D, const real* Eb, const real* b, bcr_t* v) {
     const int64_t odd = m / 2, even = (m + 1) / 2;
     real* Lc = (real*)malloc((size_t)(odd * (3 * B15 + 15) + even * (2 * B15 + 30)) * sizeof(real));
     real *Za = Lc + odd * B15, *Zb = Za + odd * B15, *zb = Zb + odd * B15;
     real *Dn = zb + odd * 15, *En = Dn + even * B15, *bn = En + even * B15, *xn = bn + even * 15;
     for (int64_t t = 0; t < odd; t++) {
         const int64_t i = 2 * t + 1;
+        const int hl = SAME(i - 1, i), hr = i + 1 < m && SAME(i + 1, i);
         real* L = Lc + t * B15;
         memcpy(L, D + i * B15, B15 * sizeof(real));
         int ok = chol15(L);
-        transpose(15, 15, Eb + (i - 1) * B15, Za + t * B15);
-        if (i + 1 < m) memcpy(Zb + t * B15, Eb + i * B15, B15 * sizeof(real)); else mat_zero(Zb + t * B15, B15);
+        if (hl) transpose(15, 15, Eb + (i - 1) * B15, Za + t * B15); else mat_zero(Za + t * B15, B15);
+        if (hr) memcpy(Zb + t * B15, Eb + i * B15, B15 * sizeof(real)); else mat_zero(Zb + t * B15, B15);
         memcpy(zb + t * 15, b + i * 15, 15 * sizeof(real));
         if (!ok) for (int e = 0; e < B15; e++) L[e] = NAN;
         fwd_n(L, Za + t * B15, 15); fwd_n(L, Zb + t * B15, 15); fwd_n(L, zb + t * 15, 1);
+        if (cid && !hl) mat_zero(Za + t * B15, B15);
+        if (cid && !hr) mat_zero(Zb + t * B15, B15);
     }
     for (int64_t u = 0; u < even; u++) {
         const int64_t j = 2 * u;
@@ -1026,15 +1024,16 @@ static void bcr_level(int64_t m, const real* D, const real* Eb, const real* b, r
         memcpy(Dj, D + j * B15, B15 * sizeof(real));
         memcpy(bj, b + j * 15, 15 * sizeof(real));
         mat_zero(Ej, B15);
-        const real *ZbL = j >= 1 ? Zb + ((j - 2) / 2) * B15 : 0, *zbL = j >= 1 ? zb + ((j - 2) / 2) * 15 : 0;
-        const real *ZaR = j + 1 < m ? Za + (j / 2) * B15 : 0, *ZbR = j + 1 < m ? Zb + (j / 2) * B15 : 0, *zbR = j + 1 < m ? zb + (j / 2) * 15 : 0;
+        const int hasL = j >= 1 && SAME(j - 1, j), hasR = j + 1 < m && SAME(j + 1, j), linkRR = j + 2 < m && SAME(j + 2, j);
+        const real *ZbL = hasL ? Zb + ((j - 2) / 2) * B15 : 0, *zbL = hasL ? zb + ((j - 2) / 2) * 15 : 0;
+        const real *ZaR = hasR ? Za + (j / 2) * B15 : 0, *ZbR = linkRR ? Zb + (j / 2) * B15 : 0, *zbR = hasR ? zb + (j / 2) * 15 : 0;
         for (int c2 = 0; c2 < 15; c2++) {                       /* the products subtracted one by one, interleaved, as k_bcr_reduce_iso */
             for (int r = 0; r < 15; r++) {
                 real d = E(Dj, 15, r, c2), e = 0;
                 for (int q = 0; q < 15; q++) {
                     if (ZbL) d -= E(ZbL, 15, q, r) * E(ZbL, 15, q, c2);
                     if (ZaR) d -= E(ZaR, 15, q, r) * E(ZaR, 15, q, c2);
-                    if (ZaR && j + 2 < m) e -= E(ZaR, 15, q, r) * E(ZbR, 15, q, c2);
+                    if (ZaR && ZbR) e -= E(ZaR, 15, q, r) * E(ZbR, 15, q, c2);
                 }
                 E(Dj, 15, r, c2) = d;
                 E(Ej, 15, r, c2) = e;
@@ -1047,23 +1046,187 @@ static void bcr_level(int64_t m, const real* D, const real* Eb, const real* b, r
             bj[c2] = v;
         }
     }
-    bcr_level(even, Dn, En, bn, xn);
-    for (int64_t u = 0; u < even; u++) memcpy(x + 2 * u * 15, xn + u * 15, 15 * sizeof(real));
+    v->Lc = Lc; v->Za = Za; v->Zb = Zb; v->zb = zb; v->Dn = Dn; v->En = En; v->bn = bn; v->xn = xn;
+}
+#undef SAME
+
+/* The block cyclic reduction of the whole system (rows 0 .. m-1, couplings as given), level by level in the order of solve.cu: the
+ * forward phase of bcr_forward, one node: x = D^-1 b, back: Lc^T x_i = zb - Za x_{i-1} - Zb x_{i+1}, L^-T column by column as
+ * warp_bwd15 does. */
+static void bcr_level(int64_t m, const real* D, const real* Eb, const real* b, real* x) {
+    if (m == 1) {
+        real L[B15], v[15];
+        memcpy(L, D, sizeof L);
+        if (!chol15(L)) { for (int r = 0; r < 15; r++) x[r] = NAN; return; }
+        memcpy(v, b, sizeof v);
+        fwd_n(L, v, 1); bwd_col(L, v);
+        memcpy(x, v, sizeof v);
+        return;
+    }
+    const int64_t odd = m / 2, even = (m + 1) / 2;
+    bcr_t lv;
+    bcr_forward(m, 0, D, Eb, b, &lv);
+    bcr_level(even, lv.Dn, lv.En, lv.bn, lv.xn);
+    for (int64_t u = 0; u < even; u++) memcpy(x + 2 * u * 15, lv.xn + u * 15, 15 * sizeof(real));
     for (int64_t t = 0; t < odd; t++) {
         const int64_t i = 2 * t + 1;
         real v[15];
         for (int r = 0; r < 15; r++) {
-            real s = zb[t * 15 + r];
+            real s = lv.zb[t * 15 + r];
             for (int q = 0; q < 15; q++) {
-                s -= E(Za + t * B15, 15, r, q) * x[(i - 1) * 15 + q];
-                if (i + 1 < m) s -= E(Zb + t * B15, 15, r, q) * x[(i + 1) * 15 + q];
+                s -= E(lv.Za + t * B15, 15, r, q) * x[(i - 1) * 15 + q];
+                if (i + 1 < m) s -= E(lv.Zb + t * B15, 15, r, q) * x[(i + 1) * 15 + q];
             }
             v[r] = s;
         }
-        bwd_col(Lc + t * B15, v);
+        bwd_col(lv.Lc + t * B15, v);
         memcpy(x + i * 15, v, sizeof v);
     }
-    free(Lc);
+    free(lv.Lc);
+}
+
+/* S = L^-T L^-1 (the inverse of L L^T), column c solved as k_bcr_selinv_root's lane c, its lower triangle mirrored */
+static void chol_inverse(const real* L, real* S) {
+    for (int c = 0; c < 15; c++) {
+        real y[15];
+        for (int r = 0; r < 15; r++) y[r] = r == c;
+        fwd_n(L, y, 1); bwd_1(L, y);
+        for (int r = c; r < 15; r++) E(S, 15, r, c) = E(S, 15, c, r) = y[r];
+    }
+}
+
+/* The selected inversion of one level in the order of cpi_imu_chains_marginals (DESIGN.md 3j): the isolated forward phase of
+ * bcr_forward on a zero right-hand side, the next level's blocks, then per odd node i (neighbours: nodes t, t+1 of the next level)
+ *   Sigma_{i,i-1} = -Lc^-T (Za Sigma_{i-1,i-1} + Zb Sigma_{i+1,i-1}),   Sigma_{i,i+1} = -Lc^-T (Za Sigma_{i-1,i+1} + Zb Sigma_{i+1,i+1}),
+ *   Sigma_{i,i}   =  Lc^-T (Lc^-1 - Za Sigma_{i,i-1}^T - Zb Sigma_{i,i+1}^T)   (lower triangle mirrored),
+ * a term with a neighbour of another chain left out, as k_bcr_selinv_iso.  cid [m]: the chain of every node.  Out: cov [m] and the
+ * neighbour blocks nb [m-1] (Sigma_{k,k+1}; exact 0 between chains).  One node: cov = D^-1, NaN if its pivot is not positive. */
+static void bcr_selinv(int64_t m, const int64_t* cid, const real* D, const real* Eb, real* cov, real* nb) {
+    if (m == 1) {
+        real L[B15];
+        memcpy(L, D, sizeof L);
+        if (chol15(L)) chol_inverse(L, cov); else for (int e = 0; e < B15; e++) cov[e] = NAN;
+        return;
+    }
+    const int64_t odd = m / 2, even = (m + 1) / 2;
+    real* z = (real*)calloc((size_t)m * 15, sizeof(real));
+    bcr_t lv;
+    bcr_forward(m, cid, D, Eb, z, &lv);
+    free(z);
+    int64_t* cn = (int64_t*)malloc((size_t)even * sizeof(int64_t));
+    real* covn = (real*)malloc((size_t)(2 * even) * B15 * sizeof(real));
+    real* nbn = covn + even * B15;
+    for (int64_t u = 0; u < even; u++) cn[u] = cid[2 * u];
+    bcr_selinv(even, cn, lv.Dn, lv.En, covn, nbn);
+    for (int64_t u = 0; u < even; u++) memcpy(cov + 2 * u * B15, covn + u * B15, B15 * sizeof(real));
+    for (int64_t t = 0; t < odd; t++) {
+        const int64_t i = 2 * t + 1;
+        const int hl = cid[i - 1] == cid[i], hr = i + 1 < m && cid[i + 1] == cid[i];
+        const real *L = lv.Lc + t * B15, *A = lv.Za + t * B15, *B = lv.Zb + t * B15;
+        const real *XLi = covn + t * B15, *XRi = hr ? covn + (t + 1) * B15 : 0, *N = hl && hr ? nbn + t * B15 : 0;
+        real XL[B15], XR[B15], y[15];
+        mat_zero(XL, B15); mat_zero(XR, B15);
+        for (int c = 0; c < 15; c++) {
+            if (hl) {                                               /* column c of Sigma_{i,i-1}; Sigma_{i+1,i-1} = N^T */
+                for (int r = 0; r < 15; r++) {
+                    real s = 0;
+                    for (int q = 0; q < 15; q++) s += E(A, 15, r, q) * E(XLi, 15, q, c);
+                    if (hr) for (int q = 0; q < 15; q++) s += E(B, 15, r, q) * E(N, 15, c, q);
+                    y[r] = s;
+                }
+                bwd_1(L, y);
+                for (int r = 0; r < 15; r++) E(XL, 15, r, c) = -y[r];
+            }
+            if (hr) {                                               /* column c of Sigma_{i,i+1} */
+                for (int r = 0; r < 15; r++) {
+                    real s = 0;
+                    if (hl) for (int q = 0; q < 15; q++) s += E(A, 15, r, q) * E(N, 15, q, c);
+                    for (int q = 0; q < 15; q++) s += E(B, 15, r, q) * E(XRi, 15, q, c);
+                    y[r] = s;
+                }
+                bwd_1(L, y);
+                for (int r = 0; r < 15; r++) E(XR, 15, r, c) = -y[r];
+            }
+        }
+        real* S = cov + i * B15;
+        for (int c = 0; c < 15; c++) {
+            for (int r = 0; r < 15; r++) y[r] = r == c;
+            fwd_n(L, y, 1);
+            for (int r = 0; r < 15; r++) {
+                real s = y[r];
+                if (hl) for (int q = 0; q < 15; q++) s -= E(A, 15, r, q) * E(XL, 15, c, q);
+                if (hr) for (int q = 0; q < 15; q++) s -= E(B, 15, r, q) * E(XR, 15, c, q);
+                y[r] = s;
+            }
+            bwd_1(L, y);
+            for (int r = c; r < 15; r++) E(S, 15, r, c) = E(S, 15, c, r) = y[r];
+        }
+        transpose(15, 15, XL, nb + (i - 1) * B15);                 /* Sigma_{i-1,i} = Sigma_{i,i-1}^T */
+        if (i + 1 < m) memcpy(nb + i * B15, XR, sizeof XR);
+    }
+    free(cn); free(covn); free(lv.Lc);
+}
+
+/* The selected inversion of one chain (rows lo .. hi-1), sequentially: the block Cholesky of seq_chain, M_k = D_k - U_{k-1}^T U_{k-1}
+ * = L_k L_k^T, U_k = L_k^-1 E_k, then backwards Sigma_{n-1} = M_{n-1}^-1, Sigma_{k,k+1} = -L_k^-T U_k Sigma_{k+1,k+1},
+ * Sigma_kk = L_k^-T (L_k^-1 - U_k Sigma_{k,k+1}^T) (lower triangle mirrored).  cov [n], cross [n-1] (may be NULL); a pivot that is not
+ * positive: NaN for the chain. */
+static void seq_marginals(int64_t lo, int64_t hi, const double* D, const double* Eb, double* cov, double* cross) {
+    const int64_t n = hi - lo;
+    real* L = (real*)malloc((size_t)n * 2 * B15 * sizeof(real));
+    real* U = L + n * B15;
+    int ok = 1;
+    for (int64_t k = 0; k < n && ok; k++) {
+        real* Lk = L + k * B15;
+        sym_lower(Lk, D + (lo + k) * B15);
+        if (k > 0) {
+            const real* Up = U + (k - 1) * B15;
+            for (int j = 0; j < 15; j++)
+                for (int i = 0; i < 15; i++) {
+                    real s = 0;
+                    for (int q = 0; q < 15; q++) s += E(Up, 15, q, i) * E(Up, 15, q, j);
+                    E(Lk, 15, i, j) -= s;
+                }
+        }
+        ok = chol15(Lk);
+        if (ok && k + 1 < n) { load(U + k * B15, Eb + (lo + k) * B15, B15); fwd_n(Lk, U + k * B15, 15); }
+    }
+    if (!ok) {
+        fill_nan(cov + lo * B15, n * B15);
+        if (cross) fill_nan(cross, (n - 1) * B15);
+        free(L);
+        return;
+    }
+    real S[B15], Sn[B15], X[B15], y[15];
+    chol_inverse(L + (n - 1) * B15, Sn);
+    store(cov + (hi - 1) * B15, Sn, B15);
+    for (int64_t k = n - 2; k >= 0; k--) {
+        const real *Lk = L + k * B15, *Uk = U + k * B15;
+        for (int c = 0; c < 15; c++) {                              /* X = Sigma_{k,k+1} = -L_k^-T U_k Sigma_{k+1,k+1} */
+            for (int r = 0; r < 15; r++) {
+                real s = 0;
+                for (int q = 0; q < 15; q++) s += E(Uk, 15, r, q) * E(Sn, 15, q, c);
+                y[r] = s;
+            }
+            bwd_1(Lk, y);
+            for (int r = 0; r < 15; r++) E(X, 15, r, c) = -y[r];
+        }
+        for (int c = 0; c < 15; c++) {
+            for (int r = 0; r < 15; r++) y[r] = r == c;
+            fwd_n(Lk, y, 1);
+            for (int r = 0; r < 15; r++) {
+                real s = y[r];
+                for (int q = 0; q < 15; q++) s -= E(Uk, 15, r, q) * E(X, 15, c, q);
+                y[r] = s;
+            }
+            bwd_1(Lk, y);
+            for (int r = c; r < 15; r++) E(S, 15, r, c) = E(S, 15, c, r) = y[r];
+        }
+        store(cov + (lo + k) * B15, S, B15);
+        if (cross) store(cross + k * B15, X, B15);
+        memcpy(Sn, S, sizeof S);
+    }
+    free(L);
 }
 
 /* the LM model decrease of one chain (k_lm_terms + k_lm_decide's sums): out[5] = (m, the size of its terms, cur, new, moved)
@@ -1093,11 +1256,11 @@ static void lm_chain(int64_t c, int64_t lo, int64_t hi, const double* rhs, const
 }
 
 typedef struct {
-    int kind, t, nt; int64_t n;                  /* kind 0: marginalise, 1: sequential solve, 2: LM terms */
+    int kind, t, nt; int64_t n;                  /* kind 0: marginalise, 1: sequential solve, 2: LM terms, 3: marginals */
     const int64_t *offsets, *n_marg; int64_t uniform, marg_uniform;
     const double *G11, *G12, *G22, *g1, *g2, *f, *pi, *pr, *pf;
     const double *D, *E, *b, *damp, *delta, *f_cur, *pf_cur, *f_new, *pf_new;
-    double *oi, *orr, *of, *sc, *x;
+    double *oi, *orr, *of, *sc, *x, *cov, *cross;
 } cjob_t;
 
 static void* cworker(void* arg) {
@@ -1109,6 +1272,8 @@ static void* cworker(void* arg) {
                        j->oi + c * B15, j->orr + c * 15, j->of + c, j->sc ? j->sc + c * 242 : 0);
         else if (j->kind == 1)
             seq_chain(lo, hi, j->D, j->E, j->b, j->x);
+        else if (j->kind == 3)
+            seq_marginals(lo, hi, j->D, j->E, j->cov, j->cross ? j->cross + (lo - c) * B15 : 0);
         else
             lm_chain(c, lo, hi, j->b, j->D, j->E, j->damp, j->delta, j->f_cur, j->pf_cur, j->f_new, j->pf_new, j->x + c * 5);
     }
@@ -1159,6 +1324,37 @@ int oracle_chain_solve(int64_t n_chains, const int64_t* offsets, int64_t uniform
     bcr_level(n, Dl, El, bl, xl);
     store(x, xl, n * 15);
     free(Dl);
+    return 0;
+}
+
+int oracle_chain_marginals(int64_t n_chains, const int64_t* offsets, int64_t uniform, const double* D, const double* E, double* cov,
+                           double* cross, int order, int nthreads) {
+    if (n_chains < 0 || (!offsets && uniform < 1) || (order != 0 && order != 1)) return -1;
+    const int64_t n = offsets ? offsets[n_chains] : n_chains * uniform;
+    if (n == 0) return 0;
+    if (order == 0) {
+        cjob_t j; memset(&j, 0, sizeof j);
+        j.kind = 3; j.n = n_chains; j.offsets = offsets; j.uniform = uniform; j.D = D; j.E = E; j.cov = cov; j.cross = cross;
+        crun(&j, nthreads);
+        return 0;
+    }
+    real* Dl = (real*)malloc((size_t)n * 4 * B15 * sizeof(real));
+    real *El = Dl + n * B15, *cl = El + n * B15, *nl = cl + n * B15;
+    int64_t* cid = (int64_t*)malloc((size_t)n * sizeof(int64_t));
+    for (int64_t c = 0; c < n_chains; c++) {
+        const int64_t lo = offsets ? offsets[c] : c * uniform, hi = offsets ? offsets[c + 1] : lo + uniform;
+        for (int64_t k = lo; k < hi; k++) cid[k] = c;
+    }
+    for (int64_t k = 0; k < n; k++) {
+        sym_lower(Dl + k * B15, D + k * B15);
+        if (k + 1 < n) load(El + k * B15, E + k * B15, B15); else mat_zero(El + k * B15, B15);
+    }
+    bcr_selinv(n, cid, Dl, El, cl, nl);
+    store(cov, cl, n * B15);
+    if (cross)
+        for (int64_t k = 0; k + 1 < n; k++)
+            if (cid[k] == cid[k + 1]) store(cross + (k - cid[k]) * B15, nl + k * B15, B15);
+    free(Dl); free(cid);
     return 0;
 }
 

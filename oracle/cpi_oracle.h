@@ -33,7 +33,11 @@ int oracle_scan_records(int64_t n_groups, const int64_t* offsets, int64_t unifor
  * states when offsets is NULL).  chain_marginalize: K8's recurrence with a plain 15x15 Cholesky, NaN rule and m = 0 copy as
  * cpi_imu_chain_marginalize; scale (may be NULL) [n_chains, 242]: per chain the size of the terms that cancel into info (225), rhs
  * (15) and f (1), and the last step's z^T z.  chain_solve: x = A^-1 b of the SPD block-tridiagonal system, order 0 a sequential block
- * Cholesky per chain, order 1 the block cyclic reduction of the whole system in the order of solve.cu.  lm_terms: out [n_chains, 5] =
+ * Cholesky per chain, order 1 the block cyclic reduction of the whole system in the order of solve.cu.  chain_marginals: the
+ * selected inversion of the same system, cov [N, 225] = Sigma_kk and cross [N - n_chains, 225] = Sigma_{k,k+1} in the slots of
+ * cpi_imu_chains_marginals (cross may be NULL), order 0 a sequential block Cholesky and backward recurrence per chain, order 1 the
+ * isolated block cyclic reduction and top-down level walk of solve.cu (DESIGN.md 3j); NaN for a chain with a pivot that is not
+ * positive.  lm_terms: out [n_chains, 5] =
  * (model decrease, the size of its terms, current cost, candidate cost, delta != 0).  local / prior_at: the inverse of retract and
  * cpi_imu_prior_at. */
 int oracle_chain_marginalize(int64_t n_chains, const int64_t* offsets, int64_t uniform, const int64_t* n_marg, int64_t marg_uniform,
@@ -42,6 +46,8 @@ int oracle_chain_marginalize(int64_t n_chains, const int64_t* offsets, int64_t u
                              double* out_f, double* scale, int nthreads);
 int oracle_chain_solve(int64_t n_chains, const int64_t* offsets, int64_t uniform, const double* D, const double* E, const double* b, double* x,
                        int order, int nthreads);
+int oracle_chain_marginals(int64_t n_chains, const int64_t* offsets, int64_t uniform, const double* D, const double* E, double* cov,
+                           double* cross, int order, int nthreads);
 int oracle_lm_terms(int64_t n_chains, const int64_t* offsets, int64_t uniform, const double* rhs, const double* D, const double* E,
                     const double* damp, const double* delta, const double* f_cur, const double* pf_cur, const double* f_new,
                     const double* pf_new, double* out, int nthreads);

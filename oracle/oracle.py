@@ -240,6 +240,20 @@ class Oracle(_Base):
         assert fn(C, _i(offs), u, _d(D), _d(E), _d(b), _d(x), int(order), int(nthreads)) == 0
         return x
 
+    def chain_marginals(self, D, E, order, chain_offsets=None, uniform=None, n_chains=None, nthreads=1):
+        """(cov [N,225], cross [N-C,225]): Sigma_kk of every state and Sigma_{k,k+1} of every pair of neighbours in a chain (slot k - c,
+        as cpi_imu_chains_marginals) of tridiag(E^T, D, E): order 0 a sequential block Cholesky and backward recurrence per chain, 1 the
+        isolated block cyclic reduction and level walk of solve.cu.  NaN for a chain with a pivot that is not positive."""
+        fn = self._rec_fn("oracle_chain_marginals", [ctypes.c_int64, _PI, ctypes.c_int64, _P, _P, _P, _P, ctypes.c_int, ctypes.c_int])
+        C, offs, u, N = self._chains(chain_offsets, uniform, n_chains)
+        D = np.ascontiguousarray(D, dtype=np.float64).reshape(N, 225)
+        E = np.ascontiguousarray(E, dtype=np.float64).reshape(-1, 225)
+        if E.shape[0] < max(N - 1, 1):
+            E = np.concatenate([E, np.zeros((max(N - 1, 1) - E.shape[0], 225))])
+        cov, cross = np.zeros((N, 225)), np.zeros((max(N - C, 0), 225))
+        assert fn(C, _i(offs), u, _d(D), _d(E), _d(cov), _d(cross) if len(cross) else None, int(order), int(nthreads)) == 0
+        return cov, cross
+
     def lm_terms(self, rhs, D, E, damp, delta, f_cur, f_new, pf_cur=None, pf_new=None, chain_offsets=None, uniform=None, n_chains=None, nthreads=1):
         """Per chain [C,5]: (model decrease m, sum |delta|^T (2|rhs| + |H||delta|), current cost, candidate cost, delta != 0)."""
         fn = self._rec_fn("oracle_lm_terms", [ctypes.c_int64, _PI, ctypes.c_int64] + [_P] * 10 + [ctypes.c_int])

@@ -4,7 +4,9 @@ factor.chains_covariance / chains_marginals; DESIGN.md section 3j).
 GTSAM is not in the reference tree, so parity with its Marginals is UNPINNED.  The truths are ``selinv_ref`` (the level walk in
 numpy, pinned on the CPU against the dense inverse) and, on the GPU, the dense per-chain inverse of the assembled system refined with
 80-bit residuals, K7's propagated covariance (a chain at its exact prediction), K8's marginal prior, and the Monte-Carlo spread of
-the smoother's error against the truth."""
+the smoother's error against the truth.  These systems are short (at most 33 states) or checked only for finite, positive-definite
+blocks; tests/test_marginals_precision.py gates every block of the long chains, the chain stress batch and the tiled production
+batch per component against the extended-precision oracle (oracle_chain_marginals)."""
 import ctypes
 
 import numpy as np
@@ -20,11 +22,12 @@ from test_state_priors import _dev, _fix, _meas_priors, _sp_dev
 P = lambda a: ctypes.c_void_p(a.ctypes.data)
 
 
-def selinv_ref(D, E, cid):
+def selinv_ref(D, E, cid, far=None):
     """numpy statement of the level walk of cpi_imu_chains_marginals on D [n,15,15], E [n-1,15,15] (block (k, k+1)), cid [n] the
     chain of every state: the isolated forward phase (as k_bcr_eliminate_iso / k_bcr_reduce_iso, couplings between chains never
     read), then top-down Sigma_{i,i-1}, Sigma_{i,i+1}, Sigma_{i,i} of every odd node.  Returns (cov [n,15,15], the neighbour
-    blocks Sigma_{k,k+1} [n-1,15,15], exactly 0 across chains)."""
+    blocks Sigma_{k,k+1} [n-1,15,15], exactly 0 across chains).  far(stride, N) (None: N^T) is the block the walk reads as
+    Sigma_{i+1,i-1} from N = Sigma_{i-1,i+1}: a hook through which tests/test_marginals_precision.py injects a misread."""
     n = len(D)
     Z = np.zeros((15, 15))
     lv, Dl, El, stride, m = [], [np.asarray(d) for d in D], [np.asarray(e) for e in E], 1, n
@@ -60,7 +63,8 @@ def selinv_ref(D, E, cid):
             hl = cid[(i - 1) * stride] == cid[i * stride]
             hr = i + 1 < m and cid[(i + 1) * stride] == cid[i * stride]
             back = lambda B: scipy.linalg.solve_triangular(Lc[t].T, B, lower=False)
-            XL = -back(Za[t] @ cov[(i - 1) * stride] + (Zb[t] @ nin[t].T if hr else 0)) if hl else Z
+            N_t = (nin[t].T if far is None else far(stride, nin[t])) if hl and hr else None
+            XL = -back(Za[t] @ cov[(i - 1) * stride] + (Zb[t] @ N_t if hr else 0)) if hl else Z
             XR = -back((Za[t] @ nin[t] if hl else 0) + Zb[t] @ cov[(i + 1) * stride]) if hr else Z
             cov[i * stride] = back(np.linalg.inv(Lc[t]) - Za[t] @ XL.T - Zb[t] @ XR.T)
             nout[i - 1] = XL.T
