@@ -54,6 +54,7 @@ SYMBOLS = {
     "cpi_propagate_batch": (c_int, [c_int, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "cpi_propagate_batch_host": (c_int, [c_int, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "cpi_retract_batch": (c_int, [c_i64, c_vp, c_vp, c_vp, c_vp]),
+    "cpi_state_update_batch": (c_int, [c_i64] + [c_vp] * 10),
     "cpi_host_last_timing": (c_int, [c_vp, c_vp]),
     "cpi_host_register": (c_int, [c_vp, ctypes.c_size_t]),
     "cpi_host_unregister": (c_int, [c_vp]),

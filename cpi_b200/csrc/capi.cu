@@ -1023,4 +1023,25 @@ int cpi_retract_batch(int64_t n, const double* states, const double* xi, double*
     return CPI_OK;
 }
 
+int cpi_state_update_batch(int64_t n, const double* states, const double* cov, const double* meas_info, const double* meas_states,
+                           const double* gate, double* states_out, double* cov_out, double* nis, int32_t* applied, void* stream) {
+    if (n < 0) return fail(CPI_EINVAL, "negative count");
+    if (n == 0) return CPI_OK;
+    if (!states || !cov || !meas_info || !meas_states || !states_out || !cov_out) return fail(CPI_EINVAL, "null pointer argument");
+    const void* ins[5] = {states, cov, meas_info, meas_states, gate};
+    const void* outs[4] = {states_out, cov_out, nis, applied};
+    for (const void* o : outs)
+        for (const void* q : ins)
+            if (o && o == q) return fail(CPI_EINVAL, "outputs must not overlap inputs");
+    for (int a = 0; a < 4; a++)
+        for (int b = a + 1; b < 4; b++)
+            if (outs[a] && outs[a] == outs[b]) return fail(CPI_EINVAL, "outputs must not overlap each other");
+    DevInfo d;
+    int rc = device_info(d);
+    if (rc) return rc;
+    CU(cpi::state_update_launch(n, states, cov, meas_info, meas_states, gate, states_out, cov_out, nis, applied, (cudaStream_t)stream));
+    g_launches += 1;
+    return CPI_OK;
+}
+
 }  // extern "C"

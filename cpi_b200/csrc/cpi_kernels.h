@@ -104,6 +104,9 @@ cudaError_t state_priors_fold_launch(int64_t n_chains, const int64_t* offs, int6
 cudaError_t state_priors_robust_launch(int64_t n, const int32_t* loss, const double* loss_k, const double* info, const double* rhs,
                                        const double* f, double* info_out, double* rhs_out, double* f_out, cudaStream_t st);
 cudaError_t retract_launch(int64_t n, const double* states, const double* xi, double* out, cudaStream_t st);
+// update.cu: the filter's measurement update by direct state fixes, with chi-square gating (K10; gate, nis, applied may be NULL)
+cudaError_t state_update_launch(int64_t n, const double* states, const double* cov, const double* meas_info, const double* meas_states,
+                                const double* gate, double* states_out, double* cov_out, double* nis, int32_t* applied, cudaStream_t st);
 // relinearize.cu: selection, stable compaction, gather and scatter around the K1/K2 launch of cpi_imu_records_relinearize
 struct RelinWorkspace {
     double* crec;             // compact records [n][rd]

@@ -1,0 +1,175 @@
+// K10: EKF measurement update of many filters by direct state fixes, with chi-square gating (DESIGN.md section 3k).  Filter i has
+// the state x (16 doubles) and the error covariance Sigma (15x15, in the tangent space of retract); the fix is (W, x_bar) in the
+// convention of the state priors: d = local(x_bar, x), Jacobian taken as I.  In square-root form (Sigma^-1 is never formed):
+//   Sigma = L L^T,  C = chol(I + L^T W L),  u = L^T W d,  v = C^-1 u,  w = C^-T v,
+//   xi = -L w,  Sigma+ = M M^T with M = L C^-T,  gamma = (d + xi)^T W (d + xi) + w^T w,  x+ = retract(x, xi)
+// gamma > gate[i] skips the fix: x and Sigma are copied bit for bit.
+//
+// One warp per filter.  Sigma and W are staged in shared memory (row-major, pitch 16) with coalesced loads; d, u, v and w live in
+// the spare column 15 of the pitch-16 buffers.  Lane c < 15 forms column c of L^T W L from column c of L, lane 15 forms u from d in
+// the same pass.  After the warp's Cholesky of C, lane i < 15 solves row i of M while lane 15 solves for v; the warp solves for w
+// with shuffles (warp_bwd15).  Then lane i < 15 forms row i of Sigma+ left of the diagonal and mirrors it, so Sigma+ is exactly
+// symmetric, while lane 15 forms xi, gamma and the retraction.  No atomics: the same bits on every run.
+#include "chol15.cuh"
+#include "cpi_kernels.h"
+#include "local15.cuh"
+
+namespace cpi {
+
+constexpr int UWARPS = 4;                        // filters (warps) per CTA
+constexpr int UP = 240;                          // one 15x15 matrix, row-major with pitch 16
+
+// JPLNavState::retract: the arithmetic of k_retract (factor.cu), kept as a local copy so that k_retract's code is untouched
+CPI_DEV void retract_state(const double* x, const double* d, double* o) {
+    const double nrm = sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
+    double s, c;
+    sincos(nrm / 2.0, &s, &c);
+    double dq[4] = {(s / nrm) * d[0], (s / nrm) * d[1], (s / nrm) * d[2], c};
+    double nn = sqrt(dq[0] * dq[0] + dq[1] * dq[1] + dq[2] * dq[2] + dq[3] * dq[3]);
+#pragma unroll
+    for (int k = 0; k < 4; k++) dq[k] /= nn;
+    if (dq[3] < 0) { dq[0] = -dq[0]; dq[1] = -dq[1]; dq[2] = -dq[2]; dq[3] = -dq[3]; }
+    nn = sqrt(dq[0] * dq[0] + dq[1] * dq[1] + dq[2] * dq[2] + dq[3] * dq[3]);
+    if (isnan(nn)) { dq[0] = dq[1] = dq[2] = 0.0; dq[3] = 1.0; }
+    const double q[4] = {x[0], x[1], x[2], x[3]};
+    double qn[4];
+    quat_multiply(dq, q, qn);
+#pragma unroll
+    for (int k = 0; k < 4; k++) o[k] = qn[k];
+#pragma unroll
+    for (int k = 0; k < 12; k++) o[4 + k] = x[4 + k] + d[3 + k];
+}
+
+__global__ void __launch_bounds__(UWARPS * 32) k_state_update(int64_t n, const double* states, const double* cov, const double* meas_info,
+                                                             const double* meas_states, const double* gate, double* states_out,
+                                                             double* cov_out, double* nis, int32_t* applied) {
+    __shared__ double smem[UWARPS][4 * UP];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int64_t i = (int64_t)blockIdx.x * UWARPS + warp;
+    if (i >= n) return;
+    double* L = smem[warp];                       // Sigma, then its Cholesky factor (lower triangle)
+    double* W = L + UP;                           // the fix's information
+    double* C = W + UP;                           // I + L^T W L (column 15: u), its Cholesky factor, then Sigma+
+    double* M = C + UP;                           // L C^-T
+    const double* sg = cov + i * 225;
+    const double* wg = meas_info + i * 225;
+    for (int e = lane; e < 225; e += 32) {        // column-major (r, c) -> row-major pitch 16
+        const int r = e % 15, c = e / 15;
+        L[r * 16 + c] = __ldg(sg + e);
+        W[r * 16 + c] = __ldg(wg + e);
+    }
+    const double* x = states + i * CPI_STATE_DOUBLES;
+    if (lane == 15) {                             // d = local(x_bar, x) in the spare column 15 of W
+        double d[15];
+        local15(meas_states + i * CPI_STATE_DOUBLES, x, d);
+#pragma unroll
+        for (int r = 0; r < 15; r++) W[r * 16 + 15] = d[r];
+    }
+    __syncwarp();
+    warp_chol15(L, lane);
+
+    if (lane < 16) {                              // column lane of L^T W L (lane 15: u = L^T W d)
+        double y[15];                             // W a, a = column lane of L (lane 15: d), column by column
+#pragma unroll
+        for (int r = 0; r < 15; r++) y[r] = 0.0;
+#pragma unroll
+        for (int k = 0; k < 15; k++) {
+            const double a = lane == 15 ? W[k * 16 + 15] : (k >= lane ? L[k * 16 + lane] : 0.0);
+#pragma unroll
+            for (int r = 0; r < 15; r++) y[r] = fma(W[r * 16 + k], a, y[r]);
+        }
+#pragma unroll
+        for (int r = 0; r < 15; r++) {
+            double t = 0.0;
+#pragma unroll
+            for (int k = r; k < 15; k++) t = fma(L[k * 16 + r], y[k], t);
+            C[r * 16 + lane] = r == lane ? t + 1.0 : t;
+        }
+    }
+    __syncwarp();
+    warp_chol15(C, lane);                         // eigenvalues >= 1 for a PSD W; column 15 is not touched
+
+    if (lane < 15) {                              // row lane of M: (C^-1 L^T)(:, lane) = C^-1 L(lane, :)^T
+        double y[15];
+#pragma unroll
+        for (int k = 0; k < 15; k++) y[k] = k <= lane ? L[lane * 16 + k] : 0.0;
+        fwd15(C, y);
+#pragma unroll
+        for (int k = 0; k < 15; k++) M[lane * 16 + k] = y[k];
+    } else if (lane == 15) {                      // v = C^-1 u, in place of u
+        double v[15];
+#pragma unroll
+        for (int k = 0; k < 15; k++) v[k] = C[k * 16 + 15];
+        fwd15(C, v);
+#pragma unroll
+        for (int k = 0; k < 15; k++) C[k * 16 + 15] = v[k];
+    }
+    __syncwarp();
+    {                                             // w = C^-T v = -L^-1 xi, lane k holds w_k; into the spare column 15 of M
+        const double wk = warp_bwd15(C, lane < 15 ? C[lane * 16 + 15] : 0.0, lane);
+        if (lane < 15) M[lane * 16 + 15] = wk;
+    }
+    __syncwarp();
+    double g = 0.0;
+    if (lane < 15) {                              // Sigma+(lane, j) = M(lane, :) M(j, :)^T, j <= lane, mirrored
+        double y[15];
+#pragma unroll
+        for (int k = 0; k < 15; k++) y[k] = M[lane * 16 + k];
+        for (int j = 0; j <= lane; j++) {
+            double t = 0.0;
+#pragma unroll
+            for (int k = 0; k < 15; k++) t = fma(y[k], M[j * 16 + k], t);
+            C[lane * 16 + j] = t;
+            C[j * 16 + lane] = t;
+        }
+    } else if (lane == 15) {
+        double w[15], g2 = 0.0;
+#pragma unroll
+        for (int k = 0; k < 15; k++) { w[k] = M[k * 16 + 15]; g2 = fma(w[k], w[k], g2); }
+#pragma unroll
+        for (int r = 14; r >= 0; r--) {           // xi = -L w in place (row r reads w[0..r])
+            double t = 0.0;
+#pragma unroll
+            for (int k = 0; k <= r; k++) t = fma(L[r * 16 + k], w[k], t);
+            w[r] = -t;
+        }
+        double g1 = 0.0;
+#pragma unroll
+        for (int r = 0; r < 15; r++) {            // (d + xi)^T W (d + xi)
+            double t = 0.0;
+#pragma unroll
+            for (int k = 0; k < 15; k++) t = fma(W[r * 16 + k], W[k * 16 + 15] + w[k], t);
+            g1 = fma(W[r * 16 + 15] + w[r], t, g1);
+        }
+        g = g1 + g2;
+        const bool on = !(gate && g > __ldg(gate + i));
+        double xo[16];
+        if (on) retract_state(x, w, xo);
+        else
+#pragma unroll
+            for (int k = 0; k < 16; k++) xo[k] = x[k];
+        double* o = states_out + i * CPI_STATE_DOUBLES;
+#pragma unroll
+        for (int k = 0; k < 16; k++) o[k] = xo[k];
+        if (nis) nis[i] = g;
+        if (applied) applied[i] = on ? 1 : 0;
+    }
+    g = __shfl_sync(0xffffffffu, g, 15);
+    const bool on = !(gate && g > __ldg(gate + i));
+    __syncwarp();
+    double* co = cov_out + i * 225;
+    if (on)
+        for (int e = lane; e < 225; e += 32) co[e] = C[(e % 15) * 16 + e / 15];
+    else
+        for (int e = lane; e < 225; e += 32) co[e] = __ldg(sg + e);
+}
+
+cudaError_t state_update_launch(int64_t n, const double* states, const double* cov, const double* meas_info, const double* meas_states,
+                                const double* gate, double* states_out, double* cov_out, double* nis, int32_t* applied, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    const int64_t grid = (n + UWARPS - 1) / UWARPS;
+    k_state_update<<<(unsigned)grid, UWARPS * 32, 0, st>>>(n, states, cov, meas_info, meas_states, gate, states_out, cov_out, nis, applied);
+    return cudaGetLastError();
+}
+
+}  // namespace cpi

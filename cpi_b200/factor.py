@@ -4,7 +4,7 @@
     ImuFactorCPIv1 / ImuFactorCPIv2  gtsam/ImuFactorCPIv1.h:55, gtsam/ImuFactorCPIv2.h:55   (ctor argument order kept)
         .evaluateError(state_i, state_j, H1=False, H2=False)      gtsam/ImuFactorCPIv1.cpp:37, ImuFactorCPIv2.cpp:38
 
-and the batch entry points (``factor_eval``, ``predict_state``, ``retract``).  The residual and Jacobians are UNWHITENED,
+and the batch entry points (``factor_eval``, ``predict_state``, ``retract``, ``propagate``, ``update``).  The residual and Jacobians are UNWHITENED,
 exactly what evaluateError returns; GTSAM's Gaussian::Covariance(P_meas) whitening is outside the reference tree.
 All arithmetic happens in libcpi_b200.so on the GPU.
 """
@@ -983,6 +983,52 @@ def retract(states, xi, stream=None):
         _launch(lib.cpi_retract_batch, dev, stream, n, _tptr(states.contiguous()), _tptr(xi.contiguous()), _tptr(out))
         return out
     return _staged(run, states, xi)
+
+
+def update(states, cov, meas_info, meas_states, gate=None, stream=None):
+    """Measurement update of n filters by direct state fixes, with chi-square gating (cpi_state_update_batch, kernel K10; DESIGN.md
+    section 3k): the update step of the filter that ``propagate`` predicts.  DEVICE float64 tensors: states [n,16], cov [n,225] (SPD,
+    column-major, the tangent space of retract), meas_info [n,225] (W, PSD, zero outside the blocks it measures), meas_states [n,16]
+    (x_bar, the fix in the convention of the state priors: residual local(x_bar, x), Jacobian taken as I).  With d = local(x_bar, x):
+        xi = -(cov^-1 + W)^-1 W d,   cov+ = (cov^-1 + W)^-1,   x+ = retract(x, xi),   nis = (d+xi)^T W (d+xi) + xi^T cov^-1 xi
+    computed in square-root form.  gate: None (every fix applied), a float, or a float64 CUDA tensor [n]; the fix of filter i is
+    skipped when nis[i] > gate[i] (its state and cov are copied bit for bit).  NaN gates are rejected, +inf is allowed.  Enqueues on
+    ``stream`` (default: torch's current stream); a float gate is filled on that stream.  A tensor gate is checked for NaN with one
+    host read, which synchronises with ``stream``; a float gate or None does not synchronise.
+    Returns (states [n,16], cov [n,225] exactly symmetric, nis [n], applied [n] int32 0/1)."""
+    import torch
+
+    dev = states.device
+    for name, t in (("states", states), ("cov", cov), ("meas_info", meas_info), ("meas_states", meas_states)):
+        if not isinstance(t, torch.Tensor):
+            raise ValueError(f"{name} must be a tensor")
+    if not states.is_cuda:
+        raise ValueError("states must be a CUDA tensor")
+    _check_f64(dev, states=states, cov=cov, meas_info=meas_info, meas_states=meas_states)
+    n = states.numel() // 16
+    if states.numel() != 16 * n or cov.numel() != 225 * n or meas_info.numel() != 225 * n or meas_states.numel() != 16 * n:
+        raise ValueError("update needs states [n,16], cov [n,225], meas_info [n,225] and meas_states [n,16]")
+    if isinstance(gate, torch.Tensor):
+        _check_f64(dev, gate=gate)
+        if gate.numel() != n:
+            raise ValueError(f"gate needs one entry per filter ({n}), got {gate.numel()}")
+    elif gate is not None and math.isnan(float(gate)):
+        raise ValueError("gate must not be NaN (+inf applies every fix)")
+    f64 = dict(dtype=torch.float64, device=dev)
+    with torch.cuda.device(dev), torch.cuda.stream(stream):         # the gate's check and fill are ordered with the launch
+        if isinstance(gate, torch.Tensor):
+            gate = gate.contiguous()
+            if bool(torch.isnan(gate).any()):
+                raise ValueError("gate must not be NaN (+inf applies every fix)")
+        elif gate is not None:
+            gate = torch.full((n,), float(gate), **f64)
+        x1, c1, nis = torch.empty((n, 16), **f64), torch.empty((n, 225), **f64), torch.empty(n, **f64)
+        applied = torch.empty(n, dtype=torch.int32, device=dev)
+        if n:
+            _launch(capi.load().cpi_state_update_batch, dev, stream, n, _tptr(states.contiguous()), _tptr(cov.contiguous()),
+                    _tptr(meas_info.contiguous()), _tptr(meas_states.contiguous()), _tptr(gate), _tptr(x1), _tptr(c1), _tptr(nis),
+                    _tptr(applied))
+    return x1, c1, nis, applied
 
 
 class JPLNavState:

@@ -556,6 +556,39 @@ int cpi_propagate_batch_host(int model, int64_t n, int64_t n_anchors, const doub
 /* JPLNavState::retract (JPLNavState.cpp:37-71): states_out[i] = states[i] (+) xi[i], xi = 15 doubles each. */
 int cpi_retract_batch(int64_t n, const double* states, const double* xi, double* states_out, void* stream);
 
+/*
+ * Measurement update of n filters by direct state fixes, with chi-square gating (DESIGN.md section 3k): the update step of the filter
+ * that cpi_propagate_batch predicts.  fp64, DEVICE pointers, asynchronous on `stream`, one kernel launch, no allocation, no host
+ * synchronisation.  PARITY UNPINNED (there is no reference filter); tests/update_ref.py holds the numpy statement.
+ *
+ * Filter i has the state x = states[i] (CPI_STATE_DOUBLES) and the error covariance S = cov[i] (225, column-major, SPD; the tangent
+ * space of cpi_retract_batch, as cpi_propagate_batch).  The fix is (W = meas_info[i], x_bar = meas_states[i]) in the convention of the
+ * state priors above: W PSD column-major 15x15, zero outside the blocks it measures; residual delta = local(x_bar, x') at the updated
+ * state, Jacobian taken as I.  With d = local(x_bar, x) and x' = retract(x, xi) the update minimises xi^T S^-1 xi + (d+xi)^T W (d+xi):
+ *     xi = -(S^-1 + W)^-1 W d,   S+ = (S^-1 + W)^-1,   x+ = retract(x, xi),
+ *     gamma = (d+xi)^T W (d+xi) + xi^T S^-1 xi      (= d^T (S + W^-1)^-1 d for an invertible W: the normalised innovation squared)
+ * computed in square-root form, S^-1 never formed (S's blocks span about ten orders of magnitude):
+ *     S = L L^T,  C = chol(I + L^T W L),  u = L^T W d,  v = C^-1 u,  xi = -L C^-T v,  S+ = M M^T with M = L C^-T,
+ *     gamma = (d+xi)^T W (d+xi) + |C^-T v|^2.
+ *   gate      device double[n], or NULL (every fix applied).  The fix is SKIPPED when gamma > gate[i]: states_out[i] and cov_out[i] are
+ *             then bit-for-bit copies of the inputs, applied[i] = 0.  A NaN gamma is not > gate: it is applied, and its NaN shows in
+ *             that filter's outputs.  +inf applies every finite gamma: the outputs are bitwise those of a NULL gate.  gamma does not
+ *             depend on the gate: a chi-square quantile for the rank of W is the usual threshold.
+ *   states_out / cov_out   device, as states / cov; cov_out exactly symmetric (lower triangle computed and mirrored)
+ *   nis       device double[n] (gamma, also for a skipped fix), or NULL;   applied  device int32[n] 0/1, or NULL
+ * One fix per filter per call: fixes that arrive together on disjoint blocks (position and velocity) form one (W, x_bar); a second
+ * fix on the same block is a second call.  Position, velocity and bias fixes are exact under the identity Jacobian; an attitude fix
+ * carries the second-order limit of the state priors.  x_bar must be a finite state with a unit quaternion even where W is zero.
+ * Sharpness: I + L^T W L has the condition number 1 + lambda_max(W S); in fp64 its Cholesky loses digits as that grows, and a pivot
+ * that is not positive (NaN outputs) appears near 1e17, a fix some 3e8 times sharper than the prior in standard deviations.  The
+ * precision gate covers lambda_max(W S) <= 1e12.
+ * A cov that is not SPD, or a NaN in W, gives NaN outputs for that filter only (one warp per filter).  A NaN in x_bar or x gives a
+ * NaN state and gamma (cov_out does not depend on d).  CPI_EINVAL for n < 0, a NULL required pointer, or an output equal to an input
+ * or to another output; outputs must not overlap inputs.  n = 0 launches nothing.
+ */
+int cpi_state_update_batch(int64_t n, const double* states, const double* cov, const double* meas_info, const double* meas_states,
+                           const double* gate, double* states_out, double* cov_out, double* nis, int32_t* applied, void* stream);
+
 /* ---- window builder (host) ------------------------------------------------------------------------------------------------------ */
 
 /*
