@@ -55,6 +55,8 @@ SYMBOLS = {
     "cpi_propagate_batch_host": (c_int, [c_int, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "cpi_retract_batch": (c_int, [c_i64, c_vp, c_vp, c_vp, c_vp]),
     "cpi_state_update_batch": (c_int, [c_i64] + [c_vp] * 10),
+    "cpi_state_update_measurements_batch": (c_int, [c_i64] + [c_vp] * 13),
+    "cpi_imu_measurements_linearize": (c_int, [c_i64] + [c_vp] * 10),
     "cpi_host_last_timing": (c_int, [c_vp, c_vp]),
     "cpi_host_register": (c_int, [c_vp, ctypes.c_size_t]),
     "cpi_host_unregister": (c_int, [c_vp]),
@@ -81,6 +83,8 @@ REC_DOUBLES = {1: 290, 2: 308}
 LM_RUNNING, LM_CONVERGED, LM_MAX_ITERATIONS, LM_LAMBDA_EXHAUSTED, LM_NONFINITE = 0, 1, 2, 3, 4
 # robust losses on state priors (CPI_LOSS_*)
 LOSS_GAUSSIAN, LOSS_HUBER, LOSS_CAUCHY = 0, 1, 2
+# measurement kinds (CPI_MEAS_*): DESIGN.md section 3l
+MEAS_POSITION, MEAS_VELOCITY_BODY, MEAS_DIRECTION = 1, 2, 3
 
 
 class LMParams(ctypes.Structure):

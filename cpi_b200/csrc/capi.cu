@@ -1044,4 +1044,49 @@ int cpi_state_update_batch(int64_t n, const double* states, const double* cov, c
     return CPI_OK;
 }
 
+int cpi_state_update_measurements_batch(int64_t n, const double* states, const double* cov, const int64_t* meas_offsets, const int32_t* kind,
+                                        const double* z, const double* sqrt_info, const double* aux, const double* gate, double* states_out,
+                                        double* cov_out, double* nis, int32_t* applied, void* stream) {
+    if (n < 0) return fail(CPI_EINVAL, "negative count");
+    if (n == 0) return CPI_OK;
+    if (!states || !cov || !meas_offsets || !kind || !z || !sqrt_info || !aux || !states_out || !cov_out)
+        return fail(CPI_EINVAL, "null pointer argument");
+    const void* ins[8] = {states, cov, meas_offsets, kind, z, sqrt_info, aux, gate};
+    const void* outs[4] = {states_out, cov_out, nis, applied};
+    for (const void* o : outs)
+        for (const void* q : ins)
+            if (o && o == q) return fail(CPI_EINVAL, "outputs must not overlap inputs");
+    for (int a = 0; a < 4; a++)
+        for (int b = a + 1; b < 4; b++)
+            if (outs[a] && outs[a] == outs[b]) return fail(CPI_EINVAL, "outputs must not overlap each other");
+    DevInfo d;
+    int rc = device_info(d);
+    if (rc) return rc;
+    CU(cpi::state_update_meas_launch(n, states, cov, meas_offsets, kind, z, sqrt_info, aux, gate, states_out, cov_out, nis, applied,
+                                     (cudaStream_t)stream));
+    g_launches += 1;
+    return CPI_OK;
+}
+
+int cpi_imu_measurements_linearize(int64_t n, const int32_t* kind, const int64_t* state_idx, const double* states, const double* z,
+                                   const double* sqrt_info, const double* aux, double* info, double* rhs, double* f, void* stream) {
+    if (n < 0) return fail(CPI_EINVAL, "negative count");
+    if (n == 0) return CPI_OK;
+    if (n > ((int64_t)1 << 31)) return fail(CPI_EINVAL, "too many measurements (%lld; at most 2^31 per call)", (long long)n);
+    if (!kind || !state_idx || !states || !z || !sqrt_info || !aux || !f) return fail(CPI_EINVAL, "null pointer argument");
+    if ((info == nullptr) != (rhs == nullptr)) return fail(CPI_EINVAL, "info and rhs must both be given or both be null");
+    const void* ins[6] = {kind, state_idx, states, z, sqrt_info, aux};
+    const void* outs[3] = {info, rhs, f};
+    for (const void* o : outs)
+        for (const void* q : ins)
+            if (o && o == q) return fail(CPI_EINVAL, "outputs must not overlap inputs");
+    if (info == f || rhs == f || (info && info == rhs)) return fail(CPI_EINVAL, "outputs must not overlap each other");
+    DevInfo d;
+    int rc = device_info(d);
+    if (rc) return rc;
+    CU(cpi::measurements_linearize_launch(n, kind, state_idx, states, z, sqrt_info, aux, info, rhs, f, (cudaStream_t)stream));
+    g_launches += 1;
+    return CPI_OK;
+}
+
 }  // extern "C"

@@ -107,6 +107,13 @@ cudaError_t retract_launch(int64_t n, const double* states, const double* xi, do
 // update.cu: the filter's measurement update by direct state fixes, with chi-square gating (K10; gate, nis, applied may be NULL)
 cudaError_t state_update_launch(int64_t n, const double* states, const double* cov, const double* meas_info, const double* meas_states,
                                 const double* gate, double* states_out, double* cov_out, double* nis, int32_t* applied, cudaStream_t st);
+// update.cu: the same update by attitude-dependent measurements, a CSR list per filter (K11; gate, nis, applied may be NULL)
+cudaError_t state_update_meas_launch(int64_t n, const double* states, const double* cov, const int64_t* meas_offsets, const int32_t* kind,
+                                     const double* z, const double* sqrt_info, const double* aux, const double* gate, double* states_out,
+                                     double* cov_out, double* nis, int32_t* applied, cudaStream_t st);
+// measurements.cu: measurements linearised into moved prior blocks (K12; info, rhs NULL: the f-only pass)
+cudaError_t measurements_linearize_launch(int64_t n, const int32_t* kind, const int64_t* state_idx, const double* states, const double* z,
+                                          const double* sqrt_info, const double* aux, double* info, double* rhs, double* f, cudaStream_t st);
 // relinearize.cu: selection, stable compaction, gather and scatter around the K1/K2 launch of cpi_imu_records_relinearize
 struct RelinWorkspace {
     double* crec;             // compact records [n][rd]

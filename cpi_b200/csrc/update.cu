@@ -13,6 +13,7 @@
 #include "chol15.cuh"
 #include "cpi_kernels.h"
 #include "local15.cuh"
+#include "measurement.cuh"
 
 namespace cpi {
 
@@ -169,6 +170,163 @@ cudaError_t state_update_launch(int64_t n, const double* states, const double* c
     if (n == 0) return cudaSuccess;
     const int64_t grid = (n + UWARPS - 1) / UWARPS;
     k_state_update<<<(unsigned)grid, UWARPS * 32, 0, st>>>(n, states, cov, meas_info, meas_states, gate, states_out, cov_out, nis, applied);
+    return cudaGetLastError();
+}
+
+// K11: the same update by the measurements of DESIGN.md section 3l (measurement.cuh), filter i's being meas_offsets[i] ..
+// meas_offsets[i+1]-1, all linearised at x.  With B_j = A_j L, the accumulation replaces K10's L^T W L and u:
+//   C = chol(I + sum_j B_j^T B_j),  u = sum_j B_j^T b_j,  w = C^-T C^-1 u,  xi = -L w,  Sigma+ = M M^T with M = L C^-T,
+//   gamma = sum_j |b_j + A_j xi|^2 + |w|^2      (a sum of squares: no cancellation for sharp measurements)
+// Per measurement, lane 0 stages A_j and b_j in the (not yet used) M buffer, lane c < 15 forms column c of B_j and lane 15 copies
+// b_j beside it, then lane c < 16 adds column c of B_j^T [B_j b_j] to its registers: lane c's column of the Gram matrix and lane r's
+// row are the same fma chain of commuted products.  From the Cholesky of C on, K10's steps; lane 15 relinearises each measurement
+// at x for gamma.  A filter without measurements is copied bit for bit with gamma = 0 and applied = 1.
+__global__ void __launch_bounds__(UWARPS * 32) k_state_update_meas(int64_t n, const double* states, const double* cov, const int64_t* meas_offsets,
+                                                                  const int32_t* kind, const double* z, const double* sqrt_info, const double* aux,
+                                                                  const double* gate, double* states_out, double* cov_out, double* nis,
+                                                                  int32_t* applied) {
+    __shared__ double smem[UWARPS][3 * UP];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int64_t i = (int64_t)blockIdx.x * UWARPS + warp;
+    if (i >= n) return;
+    const double* sg = cov + i * 225;
+    const double* x = states + i * CPI_STATE_DOUBLES;
+    double* co = cov_out + i * 225;
+    const int64_t j0 = __ldg(meas_offsets + i), j1 = __ldg(meas_offsets + i + 1);
+    if (j0 >= j1) {                               // nothing to apply
+        for (int e = lane; e < 225; e += 32) co[e] = __ldg(sg + e);
+        if (lane < CPI_STATE_DOUBLES) states_out[i * CPI_STATE_DOUBLES + lane] = x[lane];
+        if (lane == 0) {
+            if (nis) nis[i] = 0.0;
+            if (applied) applied[i] = 1;
+        }
+        return;
+    }
+    double* L = smem[warp];                       // Sigma, then its Cholesky factor (lower triangle)
+    double* C = L + UP;                           // I + sum B^T B (column 15: u), its Cholesky factor, then Sigma+
+    double* M = C + UP;                           // A_j, b_j (row-major 3x15, then 3) and B_j | b_j (3 rows, pitch 16); then L C^-T
+    double* B = M + 48;
+    for (int e = lane; e < 225; e += 32) L[(e % 15) * 16 + e / 15] = __ldg(sg + e);
+    __syncwarp();
+    warp_chol15(L, lane);
+
+    double y[15];                                 // lane c < 15: column c of sum B^T B; lane 15: u
+#pragma unroll
+    for (int r = 0; r < 15; r++) y[r] = 0.0;
+    for (int64_t j = j0; j < j1; j++) {
+        if (lane == 0) meas_linearize(__ldg(kind + j), x, z + j * 3, sqrt_info + j * 9, aux + j * 3, M + 45, M);
+        __syncwarp();
+        if (lane < 15) {                          // B_j(k, lane) = sum_{m >= lane} A_j(k, m) L(m, lane)
+#pragma unroll
+            for (int k = 0; k < 3; k++) {
+                double t = 0.0;
+#pragma unroll
+                for (int m = 0; m < 15; m++) t = m >= lane ? fma(M[k * 15 + m], L[m * 16 + lane], t) : t;
+                B[k * 16 + lane] = t;
+            }
+        } else if (lane == 15) {
+#pragma unroll
+            for (int k = 0; k < 3; k++) B[k * 16 + 15] = M[45 + k];
+        }
+        __syncwarp();
+        if (lane < 16) {
+#pragma unroll
+            for (int r = 0; r < 15; r++) y[r] = fma(B[32 + r], B[32 + lane], fma(B[16 + r], B[16 + lane], fma(B[r], B[lane], y[r])));
+        }
+        __syncwarp();
+    }
+    if (lane < 16) {
+#pragma unroll
+        for (int r = 0; r < 15; r++) C[r * 16 + lane] = r == lane ? y[r] + 1.0 : y[r];
+    }
+    __syncwarp();
+    warp_chol15(C, lane);                         // eigenvalues >= 1; column 15 is not touched
+
+    if (lane < 15) {                              // row lane of M = L C^-T
+        double t[15];
+#pragma unroll
+        for (int k = 0; k < 15; k++) t[k] = k <= lane ? L[lane * 16 + k] : 0.0;
+        fwd15(C, t);
+#pragma unroll
+        for (int k = 0; k < 15; k++) M[lane * 16 + k] = t[k];
+    } else if (lane == 15) {                      // v = C^-1 u, in place of u
+        double v[15];
+#pragma unroll
+        for (int k = 0; k < 15; k++) v[k] = C[k * 16 + 15];
+        fwd15(C, v);
+#pragma unroll
+        for (int k = 0; k < 15; k++) C[k * 16 + 15] = v[k];
+    }
+    __syncwarp();
+    {                                             // w = C^-T v, lane k holds w_k; into the spare column 15 of M
+        const double wk = warp_bwd15(C, lane < 15 ? C[lane * 16 + 15] : 0.0, lane);
+        if (lane < 15) M[lane * 16 + 15] = wk;
+    }
+    __syncwarp();
+    double g = 0.0;
+    if (lane < 15) {                              // Sigma+(lane, j) = M(lane, :) M(j, :)^T, j <= lane, mirrored
+        double t[15];
+#pragma unroll
+        for (int k = 0; k < 15; k++) t[k] = M[lane * 16 + k];
+        for (int j = 0; j <= lane; j++) {
+            double s = 0.0;
+#pragma unroll
+            for (int k = 0; k < 15; k++) s = fma(t[k], M[j * 16 + k], s);
+            C[lane * 16 + j] = s;
+            C[j * 16 + lane] = s;
+        }
+    } else if (lane == 15) {
+        double w[15], g2 = 0.0;
+#pragma unroll
+        for (int k = 0; k < 15; k++) { w[k] = M[k * 16 + 15]; g2 = fma(w[k], w[k], g2); }
+#pragma unroll
+        for (int r = 14; r >= 0; r--) {           // xi = -L w in place (row r reads w[0..r])
+            double t = 0.0;
+#pragma unroll
+            for (int k = 0; k <= r; k++) t = fma(L[r * 16 + k], w[k], t);
+            w[r] = -t;
+        }
+        double g1 = 0.0;
+        for (int64_t j = j0; j < j1; j++) {       // |b_j + A_j xi|^2
+            double A[45], b[3];
+            meas_linearize(__ldg(kind + j), x, z + j * 3, sqrt_info + j * 9, aux + j * 3, b, A);
+#pragma unroll
+            for (int k = 0; k < 3; k++) {
+                double e = b[k];
+#pragma unroll
+                for (int c = 0; c < 15; c++) e = fma(A[k * 15 + c], w[c], e);
+                g1 = fma(e, e, g1);
+            }
+        }
+        g = g1 + g2;
+        const bool on = !(gate && g > __ldg(gate + i));
+        double xo[16];
+        if (on) retract_state(x, w, xo);
+        else
+#pragma unroll
+            for (int k = 0; k < 16; k++) xo[k] = x[k];
+        double* o = states_out + i * CPI_STATE_DOUBLES;
+#pragma unroll
+        for (int k = 0; k < 16; k++) o[k] = xo[k];
+        if (nis) nis[i] = g;
+        if (applied) applied[i] = on ? 1 : 0;
+    }
+    g = __shfl_sync(0xffffffffu, g, 15);
+    const bool on = !(gate && g > __ldg(gate + i));
+    __syncwarp();
+    if (on)
+        for (int e = lane; e < 225; e += 32) co[e] = C[(e % 15) * 16 + e / 15];
+    else
+        for (int e = lane; e < 225; e += 32) co[e] = __ldg(sg + e);
+}
+
+cudaError_t state_update_meas_launch(int64_t n, const double* states, const double* cov, const int64_t* meas_offsets, const int32_t* kind,
+                                     const double* z, const double* sqrt_info, const double* aux, const double* gate, double* states_out,
+                                     double* cov_out, double* nis, int32_t* applied, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    const int64_t grid = (n + UWARPS - 1) / UWARPS;
+    k_state_update_meas<<<(unsigned)grid, UWARPS * 32, 0, st>>>(n, states, cov, meas_offsets, kind, z, sqrt_info, aux, gate, states_out,
+                                                                cov_out, nis, applied);
     return cudaGetLastError();
 }
 

@@ -341,6 +341,75 @@ def _state_priors(state_priors, N, dev, offs=None, S=0, loss=None, measurement=T
             None if loss is None else (code.contiguous(), lk.contiguous()))
 
 
+def _measurements(measurements, N, dev, offs=None, S=0, loss=None):
+    """Validated measurements (state_idx [M] int64, kind [M] int32 capi.MEAS_*, z [M,3], sqrt_info [M,9], aux [M,3]; DESIGN.md
+    section 3l) on N states: returns (idx, kind, z, sqrt_info, aux, single, loss) as _state_priors does, or None for measurements None
+    or M = 0.  loss: measurement_loss, (code [M] int32, k [M] float64) with the semantics of state_prior_loss, or None.  Checks shapes
+    and dtypes, then 0 <= state_idx < N, the kind codes and the loss values (one host read), then the device."""
+    import torch
+
+    from .capi import MEAS_DIRECTION, MEAS_POSITION
+
+    if measurements is None:
+        if loss is not None:
+            raise ValueError("measurement_loss needs measurements")
+        return None
+    if not isinstance(measurements, (tuple, list)) or len(measurements) != 5:
+        raise ValueError("measurements is (state_idx [M] int64, kind [M] int32, z [M,3], sqrt_info [M,9], aux [M,3])")
+    idx, kind, z, si, aux = measurements
+    if not isinstance(idx, torch.Tensor) or idx.dtype != torch.int64 or idx.dim() != 1:
+        raise ValueError("measurements: state_idx must be a 1-d int64 tensor")
+    M = idx.numel()
+    if not isinstance(kind, torch.Tensor) or kind.dtype != torch.int32 or kind.dim() != 1 or kind.numel() != M:
+        raise ValueError(f"measurements: kind must be a 1-d int32 tensor with one code for each of the {M} measurements")
+    for name, t, k in (("z", z, 3), ("sqrt_info", si, 9), ("aux", aux, 3)):
+        if not isinstance(t, torch.Tensor) or t.dtype != torch.float64:
+            raise ValueError(f"measurements: {name} must be a float64 tensor")
+        if t.numel() != k * M or t.dim() < 1 or t.shape[0] != M:
+            raise ValueError(f"measurements: {name} needs {k} doubles for each of the {M} measurements")
+    if loss is not None:
+        if not isinstance(loss, (tuple, list)) or len(loss) != 2:
+            raise ValueError("measurement_loss is (loss [M] int32, loss_k [M] float64)")
+        code, lk = loss
+        if not isinstance(code, torch.Tensor) or code.dtype != torch.int32 or code.dim() != 1 or code.numel() != M:
+            raise ValueError(f"measurement_loss: loss must be a 1-d int32 tensor with one code for each of the {M} measurements")
+        if not isinstance(lk, torch.Tensor) or lk.dtype != torch.float64 or lk.dim() != 1 or lk.numel() != M:
+            raise ValueError(f"measurement_loss: loss_k must be a 1-d float64 tensor with one threshold for each of the {M} measurements")
+        if code.device != idx.device or lk.device != idx.device:
+            raise ValueError("measurement_loss: loss and loss_k must be on the device of state_idx")
+    if kind.device != idx.device:
+        raise ValueError("measurements: kind must be on the device of state_idx")
+    single = S == 1
+    if M:
+        flags = [((idx < 0) | (idx >= N)).any(), ((kind < MEAS_POSITION) | (kind > MEAS_DIRECTION)).any()]
+        if offs is not None and idx.device == offs.device:         # a chain of one state carrying a measurement
+            c = (torch.searchsorted(offs, idx.clamp(0, max(N - 1, 0)), right=True) - 1).clamp(0, offs.numel() - 2)
+            flags.append(((offs[c + 1] - offs[c]) == 1).any())
+        else:
+            flags.append(torch.zeros((), dtype=torch.bool, device=idx.device))
+        if loss is not None:
+            flags += _loss_flags(code, lk, None, None, False)
+        flags = torch.stack(flags).tolist()
+        if flags[0]:
+            raise IndexError(f"measurements: state_idx out of range [0, {N})")
+        if flags[1]:
+            raise ValueError("measurements: kind codes are 1 (position), 2 (body-frame velocity) and 3 (direction)")
+        if loss is not None:
+            if flags[3]:
+                raise ValueError("measurement_loss: loss codes are 0 (Gaussian), 1 (Huber) and 2 (Cauchy)")
+            if flags[4]:
+                raise ValueError("measurement_loss: a Huber or Cauchy measurement needs a threshold k with 0 < k^2 < inf")
+        if offs is not None:
+            single = bool(flags[2])
+    if not idx.is_cuda or idx.device != dev:
+        raise ValueError(f"measurements: state_idx must be a CUDA tensor on {dev}")
+    _check_f64(dev, z=z, sqrt_info=si, aux=aux)
+    if M == 0:
+        return None
+    return (idx, kind.contiguous(), z.reshape(M, 3), si.reshape(M, 9), aux.reshape(M, 3), single,
+            None if loss is None else (code.contiguous(), lk.contiguous()))
+
+
 def _state_prior_csr(key, N):
     """(order, sp_offsets [N+1]): the stable sort of the priors by key and the CSR of the keys below N (the priors of state k are
     order[sp_offsets[k] .. sp_offsets[k+1]-1])."""
@@ -358,16 +427,28 @@ class _StatePriors:
     def __init__(self, sp, N, layout, key=None):
         import torch
 
-        idx, info, rhs, f, lin, self.single, loss = sp
+        idx, info, rhs, f, lin, single, loss = sp
+        order = self._sorted(idx, N, layout, key, single, loss)
+        self.info, self.rhs, self.lin = info[order].contiguous(), rhs[order].contiguous(), lin[order].contiguous()
+        self.f = None if f is None else f[order].contiguous()
+        f64 = dict(dtype=torch.float64, device=idx.device)
+        self.x, self.r, self.fm = torch.empty((self.M, 16), **f64), torch.empty((self.M, 15), **f64), torch.empty(self.M, **f64)
+        self._weighted()
+
+    def _sorted(self, idx, N, layout, key, single, loss):
+        """What the fold reads of every source: the stable sort by key (default: the state) and its CSR, the layout, the count, the
+        single-state flag and the loss in that order.  Returns the order; sets idx sorted."""
         order, self.sp_off = _state_prior_csr(idx if key is None else key, N)
         self.C, self.offs, self.S = layout
-        self.M = M = idx.numel()
-        self.idx, self.info, self.rhs, self.lin = idx[order], info[order].contiguous(), rhs[order].contiguous(), lin[order].contiguous()
-        self.f = None if f is None else f[order].contiguous()
+        self.M, self.single, self.idx = idx.numel(), single, idx[order]
         self.loss = None if loss is None else (loss[0][order].contiguous(), loss[1][order].contiguous())
-        f64 = dict(dtype=torch.float64, device=idx.device)
-        self.x, self.r, self.fm = torch.empty((M, 16), **f64), torch.empty((M, 15), **f64), torch.empty(M, **f64)
-        self.iw = self.info if loss is None else torch.empty((M, 225), **f64)     # the info the fold reads: weighted under a loss
+        return order
+
+    def _weighted(self):
+        """The info the fold reads: self.info, or a buffer for the weighted info under a loss."""
+        import torch
+
+        self.iw = self.info if self.loss is None else torch.empty((self.M, 225), dtype=torch.float64, device=self.info.device)
 
     def fold(self, lib, sp, rhs, f, G11=None, G22=None, g1=None, g2=None, f_out=None, pi=None, pr=None, pf=None):
         """Reweight the priors (info, rhs, f) in place under their loss (s = f) and fold them into the targets; rhs None: f alone."""
@@ -387,6 +468,68 @@ class _StatePriors:
         torch.index_select(X, 0, self.idx, out=self.x)
         capi.check(lib.cpi_imu_prior_at(self.M, p(self.info), p(self.rhs), p(self.f), p(self.lin), p(self.x), p(self.r), p(self.fm), sp))
         self.fold(lib, sp, None if cost_only else self.r, self.fm, **targets)
+
+
+class _Measurements(_StatePriors):
+    """The measurements of one call (the tuple of _measurements) sorted stably by state, with their CSR, on the chain layout: the
+    state priors' fold, with the blocks linearised by cpi_imu_measurements_linearize at every call of `at` (DESIGN.md section 3l)."""
+
+    def __init__(self, ms, N, layout):
+        import torch
+
+        idx, kind, z, si, aux, single, loss = ms
+        order = self._sorted(idx, N, layout, None, single, loss)
+        self.idx, self.kind = self.idx.contiguous(), kind[order].contiguous()
+        self.z, self.si, self.aux = z[order].contiguous(), si[order].contiguous(), aux[order].contiguous()
+        M, f64 = self.M, dict(dtype=torch.float64, device=idx.device)
+        self.info, self.r, self.fm = torch.empty((M, 225), **f64), torch.empty((M, 15), **f64), torch.empty(M, **f64)
+        self._weighted()
+
+    def at(self, lib, sp, X, cost_only=False, **targets):
+        """Linearise the measurements at the states X [N,16] (the f-only pass for cost_only), reweight and fold them as state priors."""
+        p = _tptr
+        info, r = (None, None) if cost_only else (self.info, self.r)
+        capi.check(lib.cpi_imu_measurements_linearize(self.M, p(self.kind), p(self.idx), p(X), p(self.z), p(self.si), p(self.aux), p(info),
+                                                      p(r), p(self.fm), sp))
+        self.fold(lib, sp, r, self.fm, **targets)
+
+
+def _folds(sp, ms, N, layout):
+    """The fold sources of one call: the state priors, then the measurements (each None or validated); an empty list for neither.
+    Folded one after the other, the measurements of a state are added after its priors."""
+    return ([] if sp is None else [_StatePriors(sp, N, layout)]) + ([] if ms is None else [_Measurements(ms, N, layout)])
+
+
+def measurements_linearize(states, measurements, stream=None):
+    """The measurements (state_idx [M] int64, kind [M] int32 capi.MEAS_*, z [M,3], sqrt_info [M,9], aux [M,3]) linearised at the
+    states [N,16] (cpi_imu_measurements_linearize, kernel K12; DESIGN.md section 3l) into moved prior blocks: info = A^T A [M,225]
+    (exactly symmetric), rhs' = -A^T b [M,15], f' = b^T b [M].  Validated like state_priors (one host read).  Returns (info, rhs, f,
+    state_priors) with state_priors = (state_idx, info, rhs, f, states[state_idx]): what chain_marginalize takes, as given at the
+    blocks' linearisation point, to marginalise a lag window's measurements on eliminated states."""
+    import torch
+
+    if not isinstance(states, torch.Tensor):
+        raise ValueError("states must be a tensor")
+    if measurements is None:
+        raise ValueError("measurements_linearize needs measurements")
+    dev = states.device
+    N = states.numel() // 16
+    if states.numel() != 16 * N:
+        raise ValueError(f"states must hold 16 doubles per state (got {states.numel()} doubles)")
+    ms = _measurements(measurements, N, dev)
+    _check_f64(dev, states=states)
+    idx = measurements[0]
+    M = idx.numel()
+    f64 = dict(dtype=torch.float64, device=dev)
+    with torch.cuda.device(dev), torch.cuda.stream(stream):         # buffers, copies and the launch in the order of `stream`
+        info, rhs, f = torch.empty((M, 225), **f64), torch.empty((M, 15), **f64), torch.empty(M, **f64)
+        X = states.reshape(N, 16).contiguous()
+        if ms is not None:
+            kind, z, si, aux = (t.contiguous() for t in ms[1:5])
+            _launch(capi.load().cpi_imu_measurements_linearize, dev, stream, M, _tptr(kind), _tptr(idx.contiguous()), _tptr(X), _tptr(z),
+                    _tptr(si), _tptr(aux), _tptr(info), _tptr(rhs), _tptr(f))
+        lin = X.index_select(0, idx)
+    return info, rhs, f, (idx, info, rhs, f, lin)
 
 
 def state_priors_fold(chain_offsets, sp_offsets, sp_info, sp_rhs, sp_f, G11=None, G22=None, g1=None, g2=None, f=None, prior_info=None,
@@ -529,7 +672,7 @@ def _prior_at_checks(info, rhs, f, lin_states, states):
 
 
 def chains_lm_step(model, states, records, lin, chain_offsets, prior=None, lam=1e-5, diagonal_damping=True, stream=None, state_priors=None,
-                   state_prior_loss=None):
+                   state_prior_loss=None, measurements=None, measurement_loss=None):
     """One damped Gauss-Newton step of many independent IMU-only chains at once (a fixed-lag smoother's windows), on the device:
     evaluateError -> information blocks -> prior_at (every chain's prior moved to its current first state) -> chains_assemble ->
     ONE block-cyclic-reduction solve over all chains -> retract.  states [N,16]; records / lin: the N - n_chains factors, chain c's
@@ -541,11 +684,15 @@ def chains_lm_step(model, states, records, lin, chain_offsets, prior=None, lam=1
     state_prior_loss: (loss [M] int32 capi.LOSS_*, loss_k [M] float64) aligned with state_priors, or None (DESIGN.md section 3h): a
     Huber or Cauchy prior (a measurement prior: rhs and f None or zero) is reweighted at the states (state_priors_robust) before the
     fold and costs c(s).
-    Returns (new_states, delta [N,15], cost per chain before the step [n_chains] = sum of e^T P^-1 e + the moved priors' f')."""
+    measurements: (state_idx [M] int64, kind [M] int32 capi.MEAS_*, z [M,3], sqrt_info [M,9], aux [M,3]) or None (DESIGN.md section
+    3l): linearised at the states (measurements_linearize) and folded after the state priors; measurement_loss as state_prior_loss.
+    Returns (new_states, delta [N,15], cost per chain before the step [n_chains] = sum of e^T P^-1 e + the moved priors' f' + the
+    measurements' whitened squared residuals)."""
     import torch
 
     (C, offs, S), X, (G11, G12, G22, g1, g2, f), (pi_a, pr_c, pf_c) = _linearized(model, states, records, lin, chain_offsets, prior, stream,
-                                                                                  state_priors, state_prior_loss)
+                                                                                  state_priors, state_prior_loss, measurements,
+                                                                                  measurement_loss)
     D, E, rhs = chains_assemble(G11, G12, G22, g1, g2, chain_offsets, lam, pi_a, pr_c, diagonal_damping=diagonal_damping, n_chains=C, stream=stream)
     dx = chain_solve(D, E, rhs, stream=stream)
     dev, lib, f64 = X.device, capi.load(), dict(dtype=torch.float64, device=X.device)
@@ -561,7 +708,8 @@ def chains_lm_step(model, states, records, lin, chain_offsets, prior=None, lam=1
     return retract(X, dx, stream=stream), dx, cost
 
 
-def _linearized(model, states, records, lin, chain_offsets, prior, stream, state_priors, state_prior_loss):
+def _linearized(model, states, records, lin, chain_offsets, prior, stream, state_priors, state_prior_loss, measurements=None,
+                measurement_loss=None):
     """What chains_lm_step and chains_marginals do before the assembly: the layout and argument checks, the state priors (their one
     host read), the factors' state indices, the buffers and one _linearize at the states.  Returns ((C, offs, S), X [N,16], the
     blocks (G11, G12, G22, g1, g2, f) with the state priors folded in, and the chain prior as the assembly and the cost read it:
@@ -575,11 +723,12 @@ def _linearized(model, states, records, lin, chain_offsets, prior, stream, state
     if records.numel() != REC_DOUBLES[model] * nf:
         raise ValueError(f"{C} chains over {N} states hold {nf} factors: one record each")
     sp = _state_priors(state_priors, N, dev, offs, S, loss=state_prior_loss)
+    ms = _measurements(measurements, N, dev, offs, S, loss=measurement_loss)
     idx_i, idx_j = _factor_indices(nf, records.device, states, lin, *_chain_factor_states(C, offs, S, nf, dev))
     f64 = dict(dtype=torch.float64, device=dev)
     c = lambda t: None if t is None else t.contiguous()
     pi, pr, pf, lin0 = (None,) * 4 if prior is None else map(c, prior)
-    single = sp is not None and sp[5]
+    single = (sp is not None and sp[5]) or (ms is not None and ms[5])
     first, x0, pr_c, pf_c = None, None, pr, pf
     if lin0 is not None:
         first = offs[:-1] if offs is not None else torch.arange(C, dtype=torch.int64, device=dev) * S
@@ -595,19 +744,20 @@ def _linearized(model, states, records, lin, chain_offsets, prior, stream, state
     e, H1, H2 = torch.empty((nf, 15), **f64), torch.empty((nf, 225), **f64), torch.empty((nf, 225), **f64)
     G11, G12, G22 = (torch.empty((nf, 225), **f64) for _ in range(3))
     g1, g2, f = torch.empty((nf, 15), **f64), torch.empty((nf, 15), **f64), torch.empty(nf, **f64)
-    sps = None if sp is None else _StatePriors(sp, N, (C, offs, S))
+    folds = _folds(sp, ms, N, (C, offs, S))
     lib = capi.load()
     with torch.cuda.device(dev), torch.cuda.stream(stream):
         _linearize(lib, _stream(dev, stream), model, X, records.contiguous(), lin.contiguous(), idx_i, idx_j, (e, H1, H2, G11, G12, G22, g1, g2, f),
-                   (pi, pr, pf, lin0, first), (x0, pr_c, pf_c), sps, pi_r)
+                   (pi, pr, pf, lin0, first), (x0, pr_c, pf_c), folds, pi_r)
     return (C, offs, S), X, (G11, G12, G22, g1, g2, f), (pi_r if single else pi, pr_c, pf_c)
 
 
-def _linearize(lib, sp, model, X, records, lin, idx_i, idx_j, blocks, prior, moved, sps, pi_r):
+def _linearize(lib, sp, model, X, records, lin, idx_i, idx_j, blocks, prior, moved, folds, pi_r):
     """The linearisation at the states X [N,16] that chains_lm_step and every round of chains_lm share, on the stream handle sp:
     eval and the information blocks into blocks = (e, H1, H2, G11, G12, G22, g1, g2, f); the chain prior (pi, pr, pf, lin0, first)
-    moved to X[first] into moved = (x0, pr_c, pf_c) unless lin0 is None; the state priors sps (or None) moved to X, reweighted and
-    folded into the blocks and, on single-state chains, into pi_r (a copy of pi), pr_c and pf_c."""
+    moved to X[first] into moved = (x0, pr_c, pf_c) unless lin0 is None; the fold sources (_folds: state priors, measurements)
+    linearised or moved to X, reweighted and folded into the blocks and, on single-state chains, into pi_r (a copy of pi), pr_c and
+    pf_c."""
     import torch
 
     p = _tptr
@@ -621,10 +771,11 @@ def _linearize(lib, sp, model, X, records, lin, idx_i, idx_j, blocks, prior, mov
     if lin0 is not None:
         torch.index_select(X, 0, first, out=x0)
         capi.check(lib.cpi_imu_prior_at(x0.shape[0], p(pi), p(pr), p(pf), p(lin0), p(x0), p(pr_c), p(pf_c), sp))
-    if sps is not None:
-        if sps.single:
-            pi_r.copy_(pi)
-        sps.at(lib, sp, X, G11=G11, G22=G22, g1=g1, g2=g2, f_out=f, pi=pi_r, pr=pr_c if sps.single else None, pf=pf_c if sps.single else None)
+    single = any(s.single for s in folds)
+    if single:
+        pi_r.copy_(pi)
+    for s in folds:
+        s.at(lib, sp, X, G11=G11, G22=G22, g1=g1, g2=g2, f_out=f, pi=pi_r, pr=pr_c if single else None, pf=pf_c if single else None)
 
 
 _PRIOR = {}
@@ -729,7 +880,8 @@ def chains_covariance(D, E, chain_offsets, cross=False, n_chains=None, workspace
     return cov, cr
 
 
-def chains_marginals(model, states, records, lin, chain_offsets, prior=None, state_priors=None, state_prior_loss=None, cross=False, stream=None):
+def chains_marginals(model, states, records, lin, chain_offsets, prior=None, state_priors=None, state_prior_loss=None, cross=False, stream=None,
+                     measurements=None, measurement_loss=None):
     """Marginal covariances of every keyframe of many IMU chains at the states (GTSAM's Marginals / BatchFixedLagSmoother::
     marginalCovariance; DESIGN.md section 3j): the linearisation of chains_lm_step at `states` (the chain prior moved there by prior_at,
     the state priors folded in, robust weights frozen at `states` as GTSAM linearises a robust factor for Marginals), assembled with
@@ -737,13 +889,13 @@ def chains_marginals(model, states, records, lin, chain_offsets, prior=None, sta
     without priors on later states are numerically singular in fp64: their covariances are meaningless.  Returns (cov [N,225],
     cross [N - n_chains,225] or None) as chains_covariance, in the tangent space of retract at the states."""
     (C, _, _), _, (G11, G12, G22, g1, g2, _), (pi_a, pr_c, _) = _linearized(model, states, records, lin, chain_offsets, prior, stream,
-                                                                            state_priors, state_prior_loss)
+                                                                            state_priors, state_prior_loss, measurements, measurement_loss)
     D, E, _ = chains_assemble(G11, G12, G22, g1, g2, chain_offsets, 0.0, pi_a, pr_c, n_chains=C, stream=stream)
     return chains_covariance(D, E, chain_offsets, cross=cross, n_chains=C, stream=stream)
 
 
 def chains_lm(model, states, records, lin, chain_offsets, prior=None, lam=1e-5, diagonal_damping=True, params=None, max_rounds=200, check_every=8,
-              stream=None, state_priors=None, state_prior_loss=None):
+              stream=None, state_priors=None, state_prior_loss=None, measurements=None, measurement_loss=None):
     """Levenberg-Marquardt of many independent IMU-only chains at once, to convergence, on the device (GTSAM's
     LevenbergMarquardtOptimizer rule per chain: include/cpi_b200.h, DESIGN.md section 3f).  Arguments as chains_lm_step; lam: the
     initial lambda of every chain; params: capi.LMParams (None: GTSAM's defaults).  A prior without a linearisation point is taken as
@@ -753,7 +905,8 @@ def chains_lm(model, states, records, lin, chain_offsets, prior=None, lam=1e-5, 
     asynchronous).  state_priors as chains_lm_step: every round moves them to the current states after the information blocks and
     folds them in (state_priors_fold), and folds their f' at the candidate into its cost.  state_prior_loss as chains_lm_step: the
     robust priors are reweighted at every round's states before the fold (the weighted info goes to a buffer of the call; the given
-    info is constant), and their cost c(s) at the candidate goes into its cost.  Returns (states [N,16], cost [C] at them,
+    info is constant), and their cost c(s) at the candidate goes into its cost.  measurements / measurement_loss as chains_lm_step:
+    every round linearises them at its states after the state priors, and the candidate's cost takes their f-only pass there.  Returns (states [N,16], cost [C] at them,
     lam [C], status [C] int32 (capi.LM_*), iterations [C] (accepted steps), tries [C] (rounds the chain ran)), all int32 counters."""
     import torch
 
@@ -762,6 +915,7 @@ def chains_lm(model, states, records, lin, chain_offsets, prior=None, lam=1e-5, 
     N = states.numel() // 16
     C, offs, S = _chain_layout(chain_offsets, dev, n_states=N)
     sps = _state_priors(state_priors, N, dev, offs, S, loss=state_prior_loss)
+    ms = _measurements(measurements, N, dev, offs, S, loss=measurement_loss)
     _check_f64(dev, states=states, records=records, lin=lin)
     nf = N - C
     if records.numel() != REC_DOUBLES[model] * nf or lin.numel() != 13 * nf:
@@ -783,10 +937,10 @@ def chains_lm(model, states, records, lin, chain_offsets, prior=None, lam=1e-5, 
         pr = torch.zeros((C, 15), **f64) if pr is None else pr.contiguous()
         pf = torch.zeros(C, **f64) if pf is None else pf.contiguous()
         lin0 = X.index_select(0, first) if lin0 is None else lin0.contiguous()
-    use_prior, single = prior is not None, False
-    if sps is not None:
-        sps = _StatePriors(sps, N, (C, offs, S))
-        single = sps.single
+    use_prior = prior is not None
+    folds = _folds(sps, ms, N, (C, offs, S))
+    single = any(s.single for s in folds)
+    if folds:
         if single and not use_prior:                                 # a chain of one state carries priors: a zero chain prior receives them
             pi, pr, pf, lin0 = torch.zeros((C, 225), **f64), torch.zeros((C, 15), **f64), torch.zeros(C, **f64), X.index_select(0, first)
             use_prior = True
@@ -810,7 +964,7 @@ def chains_lm(model, states, records, lin, chain_offsets, prior=None, lam=1e-5, 
         sp = _stream(dev, stream)
         for r in range(max_rounds):
             check = check_every > 0 and (r + 1) % check_every == 0
-            _linearize(lib, sp, model, X, records, lin, idx_i, idx_j, blocks, chain_prior, moved, sps, pi_r)
+            _linearize(lib, sp, model, X, records, lin, idx_i, idx_j, blocks, chain_prior, moved, folds, pi_r)
             capi.check(lib.cpi_imu_chains_assemble_lm(C, p(offs), S, p(G11), p(G12), p(G22), p(g1), p(g2), p(lam_t), int(bool(diagonal_damping)),
                                                       p(pi_r if single else pi), p(pr_c if use_prior else None), p(D), p(E), p(rhs), p(damp), sp))
             capi.check(lib.cpi_imu_chains_solve(C, p(offs), S, N, p(D), p(E), p(rhs), p(dx), p(ws_solve), sp))
@@ -820,8 +974,8 @@ def chains_lm(model, states, records, lin, chain_offsets, prior=None, lam=1e-5, 
             if use_prior:
                 torch.index_select(Xn, 0, first, out=x0)
                 capi.check(lib.cpi_imu_prior_at(C, p(pi), p(pr), p(pf), p(lin0), p(x0), p(pr_n), p(pf_n), sp))
-            if sps is not None:                                      # the state priors' cost at the candidate
-                sps.at(lib, sp, Xn, cost_only=True, f_out=f_new, pf=pf_n if single else None)
+            for s in folds:                                          # the state priors' and measurements' cost at the candidate
+                s.at(lib, sp, Xn, cost_only=True, f_out=f_new, pf=pf_n if single else None)
             if check:
                 flag.zero_()
             capi.check(lib.cpi_imu_chains_lm_update(C, p(offs), S, N, ctypes.byref(params), p(f_cur), p(pf_c if use_prior else None),
@@ -1027,6 +1181,58 @@ def update(states, cov, meas_info, meas_states, gate=None, stream=None):
         if n:
             _launch(capi.load().cpi_state_update_batch, dev, stream, n, _tptr(states.contiguous()), _tptr(cov.contiguous()),
                     _tptr(meas_info.contiguous()), _tptr(meas_states.contiguous()), _tptr(gate), _tptr(x1), _tptr(c1), _tptr(nis),
+                    _tptr(applied))
+    return x1, c1, nis, applied
+
+
+def update_measurements(states, cov, measurements, gate=None, stream=None):
+    """Measurement update of n filters by the measurements of DESIGN.md section 3l (cpi_state_update_measurements_batch, kernel K11):
+    GNSS at a lever arm, body-frame velocity and known directions, linearised at the predicted states.  states [n,16], cov [n,225] as
+    ``update``; measurements as chains_lm_step's, (state_idx [M] int64, kind [M] int32 capi.MEAS_*, z [M,3], sqrt_info [M,9], aux
+    [M,3]), with state_idx indexing the FILTERS: every measurement of a filter is applied in one update, stably sorted by filter.  With
+    A_j, b_j the whitened rows at x, Sigma = L L^T, B_j = A_j L and C = chol(I + sum B_j^T B_j):
+        w = -C^-T C^-1 sum B_j^T b_j,  xi = L w,  cov+ = M M^T with M = L C^-T,  x+ = retract(x, xi),  nis = sum |b_j + A_j xi|^2 + |w|^2
+    A filter without measurements is copied bit for bit with nis = 0 and applied = 1.  gate as ``update``.  The measurements are
+    validated like state_priors (one host read for the filter indices and kind codes).
+    Returns (states [n,16], cov [n,225] exactly symmetric, nis [n], applied [n] int32 0/1)."""
+    import torch
+
+    for name, t in (("states", states), ("cov", cov)):
+        if not isinstance(t, torch.Tensor):
+            raise ValueError(f"{name} must be a tensor")
+    if not states.is_cuda:
+        raise ValueError("states must be a CUDA tensor")
+    dev = states.device
+    _check_f64(dev, states=states, cov=cov)
+    n = states.numel() // 16
+    if states.numel() != 16 * n or cov.numel() != 225 * n:
+        raise ValueError("update_measurements needs states [n,16] and cov [n,225]")
+    if isinstance(gate, torch.Tensor):
+        _check_f64(dev, gate=gate)
+        if gate.numel() != n:
+            raise ValueError(f"gate needs one entry per filter ({n}), got {gate.numel()}")
+    elif gate is not None and math.isnan(float(gate)):
+        raise ValueError("gate must not be NaN (+inf applies every measurement)")
+    ms = _measurements(measurements, n, dev)
+    f64 = dict(dtype=torch.float64, device=dev)
+    with torch.cuda.device(dev), torch.cuda.stream(stream):         # the gate's check and fill and the sort are ordered with the launch
+        if isinstance(gate, torch.Tensor):
+            gate = gate.contiguous()
+            if bool(torch.isnan(gate).any()):
+                raise ValueError("gate must not be NaN (+inf applies every measurement)")
+        elif gate is not None:
+            gate = torch.full((n,), float(gate), **f64)
+        if ms is None:                                              # no measurement: every filter is copied (one row keeps the pointers valid)
+            offsets = torch.zeros(n + 1, dtype=torch.int64, device=dev)
+            kind, z, si, aux = torch.zeros(1, dtype=torch.int32, device=dev), torch.zeros((1, 3), **f64), torch.zeros((1, 9), **f64), torch.zeros((1, 3), **f64)
+        else:
+            order, offsets = _state_prior_csr(ms[0], n)
+            kind, z, si, aux = (t[order].contiguous() for t in ms[1:5])
+        x1, c1, nis = torch.empty((n, 16), **f64), torch.empty((n, 225), **f64), torch.empty(n, **f64)
+        applied = torch.empty(n, dtype=torch.int32, device=dev)
+        if n:
+            _launch(capi.load().cpi_state_update_measurements_batch, dev, stream, n, _tptr(states.contiguous()), _tptr(cov.contiguous()),
+                    _tptr(offsets), _tptr(kind), _tptr(z), _tptr(si), _tptr(aux), _tptr(gate), _tptr(x1), _tptr(c1), _tptr(nis),
                     _tptr(applied))
     return x1, c1, nis, applied
 

@@ -449,6 +449,36 @@ int cpi_imu_state_priors_robust(int64_t n, const int32_t* loss, const double* lo
                                 double* info_out, double* rhs_out, double* f_out, void* stream);
 
 /*
+ * Measurements of one state that depend on its attitude (DESIGN.md section 3l): a GNSS antenna at a lever arm, body-frame velocity
+ * (odometer, DVL, non-holonomic constraint), a known global direction seen in the body frame (magnetometer, gravity at rest).  They
+ * enter the solver as moved state priors relinearised at every round, so their Jacobian is exact where a state prior's is taken as I.
+ * fp64, DEVICE pointers, asynchronous on `stream`, no allocation.  PARITY UNPINNED (GTSAM's GPSFactor with a lever arm and Pose3
+ * attitude factors are the nearest); tests/measurement_ref.py holds the numpy statement.
+ *
+ * Measurement i is (state_idx[i], kind[i], z[3i..], sqrt_info[9i..] the column-major S with Lambda = S^T S, aux[3i..]) on the state
+ * x = states[state_idx[i]] (JPL quaternion, C = C(q) global to IMU, tangent [dtheta, b_g, v, b_a, p] of cpi_retract_batch):
+ *     CPI_MEAS_POSITION       h = p + C^T aux    H_theta = -C^T [aux]x   H_p = I     aux: the lever arm in the IMU frame (0: position)
+ *     CPI_MEAS_VELOCITY_BODY  h = C v            H_theta = [C v]x        H_v = C     aux: not read
+ *     CPI_MEAS_DIRECTION      h = C aux          H_theta = [C aux]x                  aux: the known vector in the global frame
+ * r = h(x) - z, whitened A = S H (3x15) and b = S r.  S may be singular (a non-holonomic constraint weighs the lateral and vertical
+ * axes only).  An unknown kind gives NaN blocks for that measurement only (its chain ends CPI_LM_NONFINITE in LM).
+ *
+ *   cpi_imu_measurements_linearize   (info, rhs', f') per measurement in the convention of the state priors (cost f - 2 rhs^T xi +
+ *       xi^T info xi at xi = 0 the given state): info = A^T A (device double[n*225], column-major, exactly symmetric), rhs' = -A^T b
+ *       (double[n*15]), f' = b^T b (double[n]), the whitened squared residual s that cpi_imu_state_priors_robust reads.  info and rhs:
+ *       both or neither; neither is the f-only pass (LM's candidate cost), whose f is bitwise the full pass's.  Then
+ *       cpi_imu_state_priors_robust and cpi_imu_state_priors_fold take the blocks unchanged.  Lane-parallel stores, no atomics: the
+ *       same bits on every run.  state_idx (device int64) is not checked: indices must lie in the states array.
+ *   CPI_EINVAL for n < 0, n > 2^31, a NULL required pointer, or an output equal to an input or another output.  n = 0 launches nothing.
+ */
+#define CPI_MEAS_POSITION        1
+#define CPI_MEAS_VELOCITY_BODY   2
+#define CPI_MEAS_DIRECTION       3
+int cpi_imu_measurements_linearize(int64_t n, const int32_t* kind, const int64_t* state_idx, const double* states, const double* z,
+                                   const double* sqrt_info, const double* aux, double* info /* or NULL */, double* rhs /* or NULL */,
+                                   double* f, void* stream);
+
+/*
  * Marginal covariances of many chains (DESIGN.md section 3j): what GTSAM's Marginals / BatchFixedLagSmoother::marginalCovariance give
  * for every keyframe of a window, for every chain at once.  fp64, DEVICE pointers, asynchronous on `stream`, no allocation.  PARITY
  * UNPINNED; tests/test_chain_marginals.py holds the numpy statement of the level walk.
@@ -588,6 +618,29 @@ int cpi_retract_batch(int64_t n, const double* states, const double* xi, double*
  */
 int cpi_state_update_batch(int64_t n, const double* states, const double* cov, const double* meas_info, const double* meas_states,
                            const double* gate, double* states_out, double* cov_out, double* nis, int32_t* applied, void* stream);
+
+/*
+ * The same update by the measurements of cpi_imu_measurements_linearize (DESIGN.md section 3l; kinds CPI_MEAS_*): the filter's
+ * update by GNSS at a lever arm, body-frame velocity and known directions.  fp64, DEVICE pointers, asynchronous on `stream`, one
+ * kernel launch, no allocation, no host synchronisation.  PARITY UNPINNED; tests/measurement_ref.py holds the numpy statement.
+ *
+ * Filter i (states[i], cov[i] as cpi_state_update_batch) takes measurements meas_offsets[i] .. meas_offsets[i+1]-1 (device int64
+ * [n+1], CSR, non-decreasing, not checked) of kind / z / sqrt_info / aux (as cpi_imu_measurements_linearize, without state_idx), all
+ * linearised at x = states[i] (one EKF step).  With A_j, b_j their whitened rows at x, in square-root form:
+ *     Sigma = L L^T,  B_j = A_j L,  C = chol(I + sum_j B_j^T B_j),  w = -C^-T C^-1 sum_j B_j^T b_j,  xi = L w,
+ *     Sigma+ = M M^T with M = L C^-T (exactly symmetric),  x+ = retract(x, xi),  gamma = sum_j |b_j + A_j xi|^2 + |w|^2
+ * gamma is the normalised innovation squared r^T (H Sigma H^T + Lambda^-1)^-1 r for invertible Lambda, summed as squares.
+ *   gate      as cpi_state_update_batch: gamma > gate[i] skips the update (bit-for-bit copies, applied[i] = 0)
+ *   nis, applied   as cpi_state_update_batch
+ * A filter without measurements is copied bit for bit with gamma = 0 and applied = 1.  Sharpness: I + sum B^T B has the condition
+ * number 1 + lambda_max(W Sigma), W = sum_j A_j^T A_j, with K10's limit (pivots fail near 1e17).  A cov that is not SPD, or a NaN in a
+ * measurement's S or kind, gives NaN outputs for that filter only; a NaN in z a NaN state and gamma (cov_out does not depend on z).
+ * CPI_EINVAL for n < 0, a NULL required pointer, or an output equal to an input or another output.  n = 0 launches nothing.
+ */
+int cpi_state_update_measurements_batch(int64_t n, const double* states, const double* cov, const int64_t* meas_offsets,
+                                        const int32_t* kind, const double* z, const double* sqrt_info, const double* aux,
+                                        const double* gate, double* states_out, double* cov_out, double* nis, int32_t* applied,
+                                        void* stream);
 
 /* ---- window builder (host) ------------------------------------------------------------------------------------------------------ */
 
