@@ -56,6 +56,7 @@ SYMBOLS = {
     "cpi_retract_batch": (c_int, [c_i64, c_vp, c_vp, c_vp, c_vp]),
     "cpi_state_update_batch": (c_int, [c_i64] + [c_vp] * 10),
     "cpi_state_update_measurements_batch": (c_int, [c_i64] + [c_vp] * 13),
+    "cpi_state_update_measurements_iterated_batch": (c_int, [c_i64] + [c_vp] * 10 + [c_int, ctypes.c_double] + [c_vp] * 6),
     "cpi_imu_measurements_linearize": (c_int, [c_i64] + [c_vp] * 10),
     "cpi_host_last_timing": (c_int, [c_vp, c_vp]),
     "cpi_host_register": (c_int, [c_vp, ctypes.c_size_t]),

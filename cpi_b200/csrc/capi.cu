@@ -1068,6 +1068,35 @@ int cpi_state_update_measurements_batch(int64_t n, const double* states, const d
     return CPI_OK;
 }
 
+int cpi_state_update_measurements_iterated_batch(int64_t n, const double* states, const double* cov, const int64_t* meas_offsets,
+                                                 const int32_t* kind, const double* z, const double* sqrt_info, const double* aux,
+                                                 const int32_t* loss, const double* loss_k, const double* gate, int max_iterations, double tol,
+                                                 double* states_out, double* cov_out, double* nis, int32_t* status, int32_t* iterations,
+                                                 void* stream) {
+    if (n < 0) return fail(CPI_EINVAL, "negative count");
+    if (max_iterations < 1) return fail(CPI_EINVAL, "max_iterations must be >= 1 (got %d)", max_iterations);
+    if (!(tol >= 0.0)) return fail(CPI_EINVAL, "tol must be >= 0 (+inf: one iteration; got %g)", tol);
+    if ((loss == nullptr) != (loss_k == nullptr)) return fail(CPI_EINVAL, "loss and loss_k must both be given or both be null");
+    if (n == 0) return CPI_OK;
+    if (!states || !cov || !meas_offsets || !kind || !z || !sqrt_info || !aux || !states_out || !cov_out)
+        return fail(CPI_EINVAL, "null pointer argument");
+    const void* ins[10] = {states, cov, meas_offsets, kind, z, sqrt_info, aux, loss, loss_k, gate};
+    const void* outs[5] = {states_out, cov_out, nis, status, iterations};
+    for (const void* o : outs)
+        for (const void* q : ins)
+            if (o && o == q) return fail(CPI_EINVAL, "outputs must not overlap inputs");
+    for (int a = 0; a < 5; a++)
+        for (int b = a + 1; b < 5; b++)
+            if (outs[a] && outs[a] == outs[b]) return fail(CPI_EINVAL, "outputs must not overlap each other");
+    DevInfo d;
+    int rc = device_info(d);
+    if (rc) return rc;
+    CU(cpi::state_update_meas_iter_launch(n, states, cov, meas_offsets, kind, z, sqrt_info, aux, loss, loss_k, gate, max_iterations, tol,
+                                          states_out, cov_out, nis, status, iterations, (cudaStream_t)stream));
+    g_launches += 1;
+    return CPI_OK;
+}
+
 int cpi_imu_measurements_linearize(int64_t n, const int32_t* kind, const int64_t* state_idx, const double* states, const double* z,
                                    const double* sqrt_info, const double* aux, double* info, double* rhs, double* f, void* stream) {
     if (n < 0) return fail(CPI_EINVAL, "negative count");

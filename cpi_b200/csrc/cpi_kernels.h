@@ -111,6 +111,11 @@ cudaError_t state_update_launch(int64_t n, const double* states, const double* c
 cudaError_t state_update_meas_launch(int64_t n, const double* states, const double* cov, const int64_t* meas_offsets, const int32_t* kind,
                                      const double* z, const double* sqrt_info, const double* aux, const double* gate, double* states_out,
                                      double* cov_out, double* nis, int32_t* applied, cudaStream_t st);
+// update.cu: the iterated update by the same measurements, with robust losses (K13; loss / loss_k, gate, nis, status, iterations may be NULL)
+cudaError_t state_update_meas_iter_launch(int64_t n, const double* states, const double* cov, const int64_t* meas_offsets, const int32_t* kind,
+                                          const double* z, const double* sqrt_info, const double* aux, const int32_t* loss, const double* loss_k,
+                                          const double* gate, int max_iter, double tol, double* states_out, double* cov_out, double* nis,
+                                          int32_t* status, int32_t* iterations, cudaStream_t st);
 // measurements.cu: measurements linearised into moved prior blocks (K12; info, rhs NULL: the f-only pass)
 cudaError_t measurements_linearize_launch(int64_t n, const int32_t* kind, const int64_t* state_idx, const double* states, const double* z,
                                           const double* sqrt_info, const double* aux, double* info, double* rhs, double* f, cudaStream_t st);

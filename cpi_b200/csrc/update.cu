@@ -14,6 +14,7 @@
 #include "cpi_kernels.h"
 #include "local15.cuh"
 #include "measurement.cuh"
+#include "robust_loss.cuh"
 
 namespace cpi {
 
@@ -327,6 +328,224 @@ cudaError_t state_update_meas_launch(int64_t n, const double* states, const doub
     const int64_t grid = (n + UWARPS - 1) / UWARPS;
     k_state_update_meas<<<(unsigned)grid, UWARPS * 32, 0, st>>>(n, states, cov, meas_offsets, kind, z, sqrt_info, aux, gate, states_out,
                                                                 cov_out, nis, applied);
+    return cudaGetLastError();
+}
+
+// K13: the iterated update (DESIGN.md section 3m): Gauss-Newton on the one-step MAP problem
+//   |L^-1 local(x_hat, x)|^2 + sum_j rho_j(|b_j(x)|^2)        (the prior's Jacobian taken as I, section 3g's convention)
+// from x_0 = x_hat, relinearising the measurements at every iterate x_t and reweighting them by IRLS (robust_loss, section 3h):
+//   d_t = local(x_hat, x_t),  A_j, b_j at x_t,  om_j = omega(|b_j|^2),  B_j = sqrt(om_j) A_j L,  b'_j = sqrt(om_j) (b_j - A_j d_t),
+//   C = chol(I + sum_j B_j^T B_j),  w = C^-T C^-1 sum_j B_j^T b'_j,  eps = -L w,  delta = eps - d_t,  x_{t+1} = retract(x_t, delta)
+// until max_k |delta_k| <= tol sqrt(Sigma_kk) (status 1) or max_iter linearisations (status 2).  Sigma+ = M M^T, M = L C^-T, from the
+// last C; gamma = sum_j om_j |b_j + A_j eps_0|^2 + |w_0|^2 of the first linearisation is gated before the first step is taken
+// (gamma > gate[i]: bit-for-bit copies, status 0, one linearisation).  At t = 0 (d_0 = 0 exactly, weights 1 without a loss) K13
+// performs K11's operations in K11's order: Sigma+ and gamma are bitwise K11's, the state to rounding (ptxas contracts the
+// retraction's unfused products differently in the two kernels; DESIGN.md section 3m).
+// K11's buffers and steps: L is factored once; x_t, d_t and w live in 48 extra doubles per warp.  Lane 0 stages the weighted A_j and
+// b'_j (folding -A_j d_t into column 15); lane 15 takes the step, the stopping test and the retraction, and broadcasts the decision.
+// M and Sigma+ are formed once, after the loop.  No atomics: the same bits on every run.
+__global__ void __launch_bounds__(UWARPS * 32) k_state_update_meas_iter(int64_t n, const double* states, const double* cov,
+                                                                       const int64_t* meas_offsets, const int32_t* kind, const double* z,
+                                                                       const double* sqrt_info, const double* aux, const int32_t* loss,
+                                                                       const double* loss_k, const double* gate, int max_iter, double tol,
+                                                                       double* states_out, double* cov_out, double* nis, int32_t* status,
+                                                                       int32_t* iterations) {
+    __shared__ double smem[UWARPS][3 * UP + 48];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int64_t i = (int64_t)blockIdx.x * UWARPS + warp;
+    if (i >= n) return;
+    const double* sg = cov + i * 225;
+    const double* x = states + i * CPI_STATE_DOUBLES;                // x_hat
+    double* co = cov_out + i * 225;
+    const int64_t j0 = __ldg(meas_offsets + i), j1 = __ldg(meas_offsets + i + 1);
+    if (j0 >= j1) {                               // nothing to apply
+        for (int e = lane; e < 225; e += 32) co[e] = __ldg(sg + e);
+        if (lane < CPI_STATE_DOUBLES) states_out[i * CPI_STATE_DOUBLES + lane] = x[lane];
+        if (lane == 0) {
+            if (nis) nis[i] = 0.0;
+            if (status) status[i] = 1;
+            if (iterations) iterations[i] = 0;
+        }
+        return;
+    }
+    double* L = smem[warp];                       // Sigma, then its Cholesky factor (lower triangle)
+    double* C = L + UP;                           // I + sum B^T B (column 15: u), its Cholesky factor; after the loop Sigma+
+    double* M = C + UP;                           // weighted A_j, b'_j (row-major 3x15, then 3) and B_j | b'_j (3 rows, pitch 16); then L C^-T
+    double* B = M + 48;
+    double* X = M + UP;                           // x_t
+    double* D = X + 16;                           // d_t
+    double* W = D + 16;                           // w
+    for (int e = lane; e < 225; e += 32) L[(e % 15) * 16 + e / 15] = __ldg(sg + e);
+    if (lane < CPI_STATE_DOUBLES) X[lane] = x[lane];
+    __syncwarp();
+    warp_chol15(L, lane);
+
+    double g = 0.0;
+    int t = 0, st;                                // st: -1 go on, 0 gated, 1 converged, 2 stopped at max_iter
+    do {
+        if (lane == 15 && t > 0) {
+            double d[15];
+            local15(x, X, d);
+#pragma unroll
+            for (int r = 0; r < 15; r++) D[r] = d[r];
+        }
+        __syncwarp();
+        double y[15];                             // lane c < 15: column c of sum B^T B; lane 15: u
+#pragma unroll
+        for (int r = 0; r < 15; r++) y[r] = 0.0;
+        for (int64_t j = j0; j < j1; j++) {
+            if (lane == 0) {
+                meas_linearize(__ldg(kind + j), X, z + j * 3, sqrt_info + j * 9, aux + j * 3, M + 45, M);
+                double om, c;
+                robust_loss(loss ? __ldg(loss + j) : CPI_LOSS_GAUSSIAN, loss ? __ldg(loss_k + j) : 0.0,
+                            fma(M[47], M[47], fma(M[46], M[46], M[45] * M[45])), om, c);
+                if (t > 0)                        // b_j - A_j d_t (d_0 = 0)
+#pragma unroll
+                    for (int k = 0; k < 3; k++) {
+                        double e = M[45 + k];
+#pragma unroll
+                        for (int m = 0; m < 15; m++) e = fma(-M[k * 15 + m], D[m], e);
+                        M[45 + k] = e;
+                    }
+                if (om != 1.0) {
+                    const double sw = sqrt(om);
+#pragma unroll
+                    for (int k = 0; k < 48; k++) M[k] *= sw;
+                }
+            }
+            __syncwarp();
+            if (lane < 15) {                      // B_j(k, lane) = sum_{m >= lane} A_j(k, m) L(m, lane)
+#pragma unroll
+                for (int k = 0; k < 3; k++) {
+                    double s = 0.0;
+#pragma unroll
+                    for (int m = 0; m < 15; m++) s = m >= lane ? fma(M[k * 15 + m], L[m * 16 + lane], s) : s;
+                    B[k * 16 + lane] = s;
+                }
+            } else if (lane == 15) {
+#pragma unroll
+                for (int k = 0; k < 3; k++) B[k * 16 + 15] = M[45 + k];
+            }
+            __syncwarp();
+            if (lane < 16) {
+#pragma unroll
+                for (int r = 0; r < 15; r++) y[r] = fma(B[32 + r], B[32 + lane], fma(B[16 + r], B[16 + lane], fma(B[r], B[lane], y[r])));
+            }
+            __syncwarp();
+        }
+        if (lane < 16) {
+#pragma unroll
+            for (int r = 0; r < 15; r++) C[r * 16 + lane] = r == lane ? y[r] + 1.0 : y[r];
+        }
+        __syncwarp();
+        warp_chol15(C, lane);                     // eigenvalues >= 1; column 15 is not touched
+        if (lane == 15) {                         // v = C^-1 u, in place of u
+            double v[15];
+#pragma unroll
+            for (int k = 0; k < 15; k++) v[k] = C[k * 16 + 15];
+            fwd15(C, v);
+#pragma unroll
+            for (int k = 0; k < 15; k++) C[k * 16 + 15] = v[k];
+        }
+        __syncwarp();
+        {                                         // w = C^-T v, lane k holds w_k
+            const double wk = warp_bwd15(C, lane < 15 ? C[lane * 16 + 15] : 0.0, lane);
+            if (lane < 15) W[lane] = wk;
+        }
+        __syncwarp();
+        st = -1;
+        if (lane == 15) {
+            double w[15], g2 = 0.0;
+#pragma unroll
+            for (int k = 0; k < 15; k++) { w[k] = W[k]; g2 = fma(w[k], w[k], g2); }
+#pragma unroll
+            for (int r = 14; r >= 0; r--) {       // eps = -L w in place (row r reads w[0..r])
+                double s = 0.0;
+#pragma unroll
+                for (int k = 0; k <= r; k++) s = fma(L[r * 16 + k], w[k], s);
+                w[r] = -s;
+            }
+            if (t == 0) {                         // gamma: sum om_j |b_j + A_j eps_0|^2 + |w_0|^2 at x_hat
+                double g1 = 0.0;
+                for (int64_t j = j0; j < j1; j++) {
+                    double A[45], b[3], om, c;
+                    meas_linearize(__ldg(kind + j), x, z + j * 3, sqrt_info + j * 9, aux + j * 3, b, A);
+                    robust_loss(loss ? __ldg(loss + j) : CPI_LOSS_GAUSSIAN, loss ? __ldg(loss_k + j) : 0.0,
+                                fma(b[2], b[2], fma(b[1], b[1], b[0] * b[0])), om, c);
+#pragma unroll
+                    for (int k = 0; k < 3; k++) {
+                        double e = b[k];
+#pragma unroll
+                        for (int q = 0; q < 15; q++) e = fma(A[k * 15 + q], w[q], e);
+                        g1 = fma(om * e, e, g1);
+                    }
+                }
+                g = g1 + g2;
+                if (gate && g > __ldg(gate + i)) st = 0;
+            } else {                              // delta = eps - d_t
+#pragma unroll
+                for (int k = 0; k < 15; k++) w[k] -= D[k];
+            }
+            if (st != 0) {
+                bool conv = true;
+#pragma unroll
+                for (int k = 0; k < 15; k++) conv = conv && fabs(w[k]) <= tol * sqrt(__ldg(sg + k * 16));
+                double xo[16];
+                retract_state(X, w, xo);
+#pragma unroll
+                for (int k = 0; k < 16; k++) X[k] = xo[k];
+                st = conv ? 1 : (t + 1 >= max_iter ? 2 : -1);
+            }
+        }
+        st = __shfl_sync(0xffffffffu, st, 15);
+        t++;
+        __syncwarp();
+    } while (st < 0);
+
+    if (st == 0) {                                // gated: the inputs
+        for (int e = lane; e < 225; e += 32) co[e] = __ldg(sg + e);
+        if (lane < CPI_STATE_DOUBLES) states_out[i * CPI_STATE_DOUBLES + lane] = x[lane];
+    } else {
+        if (lane < 15) {                          // row lane of M = L C^-T, from the last C
+            double r[15];
+#pragma unroll
+            for (int k = 0; k < 15; k++) r[k] = k <= lane ? L[lane * 16 + k] : 0.0;
+            fwd15(C, r);
+#pragma unroll
+            for (int k = 0; k < 15; k++) M[lane * 16 + k] = r[k];
+        }
+        __syncwarp();
+        if (lane < 15) {                          // Sigma+(lane, j) = M(lane, :) M(j, :)^T, j <= lane, mirrored
+            double r[15];
+#pragma unroll
+            for (int k = 0; k < 15; k++) r[k] = M[lane * 16 + k];
+            for (int j = 0; j <= lane; j++) {
+                double s = 0.0;
+#pragma unroll
+                for (int k = 0; k < 15; k++) s = fma(r[k], M[j * 16 + k], s);
+                C[lane * 16 + j] = s;
+                C[j * 16 + lane] = s;
+            }
+        }
+        __syncwarp();
+        for (int e = lane; e < 225; e += 32) co[e] = C[(e % 15) * 16 + e / 15];
+        if (lane < CPI_STATE_DOUBLES) states_out[i * CPI_STATE_DOUBLES + lane] = X[lane];
+    }
+    if (lane == 15) {
+        if (nis) nis[i] = g;
+        if (status) status[i] = st;
+        if (iterations) iterations[i] = t;
+    }
+}
+
+cudaError_t state_update_meas_iter_launch(int64_t n, const double* states, const double* cov, const int64_t* meas_offsets, const int32_t* kind,
+                                          const double* z, const double* sqrt_info, const double* aux, const int32_t* loss, const double* loss_k,
+                                          const double* gate, int max_iter, double tol, double* states_out, double* cov_out, double* nis,
+                                          int32_t* status, int32_t* iterations, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    const int64_t grid = (n + UWARPS - 1) / UWARPS;
+    k_state_update_meas_iter<<<(unsigned)grid, UWARPS * 32, 0, st>>>(n, states, cov, meas_offsets, kind, z, sqrt_info, aux, loss, loss_k, gate,
+                                                                     max_iter, tol, states_out, cov_out, nis, status, iterations);
     return cudaGetLastError();
 }
 

@@ -1197,37 +1197,12 @@ def update_measurements(states, cov, measurements, gate=None, stream=None):
     Returns (states [n,16], cov [n,225] exactly symmetric, nis [n], applied [n] int32 0/1)."""
     import torch
 
-    for name, t in (("states", states), ("cov", cov)):
-        if not isinstance(t, torch.Tensor):
-            raise ValueError(f"{name} must be a tensor")
-    if not states.is_cuda:
-        raise ValueError("states must be a CUDA tensor")
-    dev = states.device
-    _check_f64(dev, states=states, cov=cov)
-    n = states.numel() // 16
-    if states.numel() != 16 * n or cov.numel() != 225 * n:
-        raise ValueError("update_measurements needs states [n,16] and cov [n,225]")
-    if isinstance(gate, torch.Tensor):
-        _check_f64(dev, gate=gate)
-        if gate.numel() != n:
-            raise ValueError(f"gate needs one entry per filter ({n}), got {gate.numel()}")
-    elif gate is not None and math.isnan(float(gate)):
-        raise ValueError("gate must not be NaN (+inf applies every measurement)")
+    dev, n = _filter_checks(states, cov, gate, "update_measurements")
     ms = _measurements(measurements, n, dev)
     f64 = dict(dtype=torch.float64, device=dev)
     with torch.cuda.device(dev), torch.cuda.stream(stream):         # the gate's check and fill and the sort are ordered with the launch
-        if isinstance(gate, torch.Tensor):
-            gate = gate.contiguous()
-            if bool(torch.isnan(gate).any()):
-                raise ValueError("gate must not be NaN (+inf applies every measurement)")
-        elif gate is not None:
-            gate = torch.full((n,), float(gate), **f64)
-        if ms is None:                                              # no measurement: every filter is copied (one row keeps the pointers valid)
-            offsets = torch.zeros(n + 1, dtype=torch.int64, device=dev)
-            kind, z, si, aux = torch.zeros(1, dtype=torch.int32, device=dev), torch.zeros((1, 3), **f64), torch.zeros((1, 9), **f64), torch.zeros((1, 3), **f64)
-        else:
-            order, offsets = _state_prior_csr(ms[0], n)
-            kind, z, si, aux = (t[order].contiguous() for t in ms[1:5])
+        gate = _filter_gate(gate, n, f64)
+        offsets, kind, z, si, aux, _ = _filter_csr(ms, n, f64)
         x1, c1, nis = torch.empty((n, 16), **f64), torch.empty((n, 225), **f64), torch.empty(n, **f64)
         applied = torch.empty(n, dtype=torch.int32, device=dev)
         if n:
@@ -1235,6 +1210,98 @@ def update_measurements(states, cov, measurements, gate=None, stream=None):
                     _tptr(offsets), _tptr(kind), _tptr(z), _tptr(si), _tptr(aux), _tptr(gate), _tptr(x1), _tptr(c1), _tptr(nis),
                     _tptr(applied))
     return x1, c1, nis, applied
+
+
+def update_measurements_iterated(states, cov, measurements, gate=None, measurement_loss=None, max_iterations=10, tol=1e-9, stream=None):
+    """The iterated EKF update of n filters by the measurements of ``update_measurements``, with Huber and Cauchy losses
+    (cpi_state_update_measurements_iterated_batch, kernel K13; DESIGN.md section 3m): Gauss-Newton on the one-step MAP problem
+    |L^-1 local(x, x')|^2 + sum_j rho_j(|b_j(x')|^2) (Sigma = cov = L L^T, the prior's Jacobian taken as I), relinearising every
+    measurement at each iterate and reweighting it by IRLS.  From x_0 = x, with d_t = local(x, x_t), A_j, b_j at x_t and om_j the
+    IRLS weight of |b_j|^2:
+        B_j = sqrt(om_j) A_j L,  b'_j = sqrt(om_j) (b_j - A_j d_t),  C = chol(I + sum B_j^T B_j),  w = C^-T C^-1 sum B_j^T b'_j,
+        delta = -L w - d_t,  x_{t+1} = retract(x_t, delta)
+    until max_k |delta_k| <= tol sqrt(cov_kk) (status 1) or max_iterations linearisations (status 2).  cov+ = M M^T with M = L C^-T of
+    the last linearisation (exactly symmetric); nis is gamma of the first linearisation, sum_j om_j |b_j + A_j eps_0|^2 + |w_0|^2 with
+    eps_0 = -L w_0 (K11's gamma without a loss), and the gate compares it before iterating: a gated filter is copied bit for bit with
+    status 0.  A filter without measurements is copied bit for bit with nis 0, status 1 and 0 iterations.  tol = +inf takes one
+    iteration (update_measurements without a loss, to rounding); tol = 0 takes max_iterations unless a step is exactly zero.
+    states, cov, measurements and gate as ``update_measurements``; measurement_loss as chains_lm_step's, (loss [M] int32 capi.LOSS_*,
+    loss_k [M] float64) or None (every measurement Gaussian), validated with the measurements' one host read.  max_iterations: int
+    >= 1; tol: float >= 0 (+inf allowed), in the prior's standard deviations.
+    Returns (states [n,16], cov [n,225], nis [n], status [n] int32 0 gated / 1 converged / 2 stopped at max_iterations,
+    iterations [n] int32 linearisations)."""
+    import torch
+
+    if isinstance(max_iterations, bool) or not isinstance(max_iterations, (int, np.integer)) or not 1 <= max_iterations < 2 ** 31:
+        raise ValueError(f"max_iterations must be an int >= 1 (got {max_iterations!r})")
+    if not isinstance(tol, (int, float, np.floating)) or isinstance(tol, bool) or not float(tol) >= 0.0:
+        raise ValueError(f"tol must be a float >= 0 (+inf: one iteration; got {tol!r})")
+    dev, n = _filter_checks(states, cov, gate, "update_measurements_iterated")
+    ms = _measurements(measurements, n, dev, loss=measurement_loss)
+    f64 = dict(dtype=torch.float64, device=dev)
+    with torch.cuda.device(dev), torch.cuda.stream(stream):         # the gate's check and fill and the sort are ordered with the launch
+        gate = _filter_gate(gate, n, f64)
+        offsets, kind, z, si, aux, loss = _filter_csr(ms, n, f64)
+        x1, c1, nis = torch.empty((n, 16), **f64), torch.empty((n, 225), **f64), torch.empty(n, **f64)
+        status, iters = torch.empty(n, dtype=torch.int32, device=dev), torch.empty(n, dtype=torch.int32, device=dev)
+        if n:
+            _launch(capi.load().cpi_state_update_measurements_iterated_batch, dev, stream, n, _tptr(states.contiguous()),
+                    _tptr(cov.contiguous()), _tptr(offsets), _tptr(kind), _tptr(z), _tptr(si), _tptr(aux), _tptr(loss[0]), _tptr(loss[1]),
+                    _tptr(gate), int(max_iterations), float(tol), _tptr(x1), _tptr(c1), _tptr(nis), _tptr(status), _tptr(iters))
+    return x1, c1, nis, status, iters
+
+
+def _filter_checks(states, cov, gate, name):
+    """The host checks of the filter updates by measurements: states [n,16] and cov [n,225] float64 CUDA tensors on one device, and a
+    gate that is None, a number other than NaN, or a float64 tensor [n] on that device.  Returns (device, n)."""
+    import torch
+
+    for what, t in (("states", states), ("cov", cov)):
+        if not isinstance(t, torch.Tensor):
+            raise ValueError(f"{what} must be a tensor")
+    if not states.is_cuda:
+        raise ValueError("states must be a CUDA tensor")
+    dev = states.device
+    _check_f64(dev, states=states, cov=cov)
+    n = states.numel() // 16
+    if states.numel() != 16 * n or cov.numel() != 225 * n:
+        raise ValueError(f"{name} needs states [n,16] and cov [n,225]")
+    if isinstance(gate, torch.Tensor):
+        _check_f64(dev, gate=gate)
+        if gate.numel() != n:
+            raise ValueError(f"gate needs one entry per filter ({n}), got {gate.numel()}")
+    elif gate is not None and math.isnan(float(gate)):
+        raise ValueError("gate must not be NaN (+inf applies every measurement)")
+    return dev, n
+
+
+def _filter_gate(gate, n, f64):
+    """The gate as the kernels read it, on the current stream: a tensor gate checked for NaN (one host read), a number filled in."""
+    import torch
+
+    if isinstance(gate, torch.Tensor):
+        gate = gate.contiguous()
+        if bool(torch.isnan(gate).any()):
+            raise ValueError("gate must not be NaN (+inf applies every measurement)")
+    elif gate is not None:
+        gate = torch.full((n,), float(gate), **f64)
+    return gate
+
+
+def _filter_csr(ms, n, f64):
+    """The validated measurements ms (_measurements) of n filters as the kernels read them, on the current stream: (offsets [n+1],
+    kind, z, sqrt_info, aux, (loss, loss_k)) sorted stably by filter, the loss permuted alike ((None, None) without one).  Without
+    measurements every filter is copied: offsets are zero and one row keeps the pointers valid."""
+    import torch
+
+    if ms is None:
+        dev = f64["device"]
+        return (torch.zeros(n + 1, dtype=torch.int64, device=dev), torch.zeros(1, dtype=torch.int32, device=dev), torch.zeros((1, 3), **f64),
+                torch.zeros((1, 9), **f64), torch.zeros((1, 3), **f64), (None, None))
+    order, offsets = _state_prior_csr(ms[0], n)
+    kind, z, si, aux = (t[order].contiguous() for t in ms[1:5])
+    loss = (None, None) if ms[6] is None else tuple(t[order].contiguous() for t in ms[6])
+    return offsets, kind, z, si, aux, loss
 
 
 class JPLNavState:

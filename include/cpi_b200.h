@@ -642,6 +642,39 @@ int cpi_state_update_measurements_batch(int64_t n, const double* states, const d
                                         const double* gate, double* states_out, double* cov_out, double* nis, int32_t* applied,
                                         void* stream);
 
+/*
+ * The iterated update by the same measurements, with robust losses (DESIGN.md section 3m): the iterated EKF, for filters that start
+ * or recover with a poor attitude, where the single linearisation of cpi_state_update_measurements_batch lands away from the posterior
+ * mode and reports a covariance taken at the wrong attitude.  fp64, DEVICE pointers, asynchronous on `stream`, one kernel launch, no
+ * allocation, no host synchronisation.  PARITY UNPINNED; tests/update_iter_ref.py holds the numpy statement.
+ *
+ * Filter i (states[i] = x_hat, cov[i] = Sigma = L L^T, measurements meas_offsets[i] .. meas_offsets[i+1]-1 as
+ * cpi_state_update_measurements_batch) runs undamped Gauss-Newton on  |L^-1 local(x_hat, x)|^2 + sum_j rho_j(|b_j(x)|^2)  with the
+ * prior's Jacobian taken as I (the state priors' convention): the iterates of cpi_imu_chains_* on a single-state chain at lambda = 0.
+ * rho_j is measurement j's loss (loss[j], loss_k[j] as cpi_imu_state_priors_robust) and om_j its IRLS weight at |b_j|^2.  From
+ * x_0 = x_hat, for t = 0, 1, ...:
+ *     d_t = local(x_hat, x_t) (0 at t = 0),  A_j, b_j at x_t,  B_j = sqrt(om_j) A_j L,  b'_j = sqrt(om_j) (b_j - A_j d_t),
+ *     C = chol(I + sum_j B_j^T B_j),  w = C^-T C^-1 sum_j B_j^T b'_j,  eps = -L w,  delta = eps - d_t,  x_{t+1} = retract(x_t, delta)
+ * stopping when max_k |delta_k| <= tol sqrt(Sigma_kk) (the step in prior standard deviations) or after max_iterations linearisations.
+ *   states_out  x_T, the last iterate;   cov_out  M M^T with M = L C^-T of the last linearisation, its weights frozen (exactly symmetric)
+ *   nis       gamma = sum_j om_j |b_j + A_j eps_0|^2 + |w_0|^2 of the FIRST linearisation (weights at x_hat); K11's gamma without a loss
+ *   gate      device double[n] or NULL: gamma > gate[i] is decided before iterating and skips the update (bit-for-bit copies, status 0);
+ *             a NaN gamma is not gated
+ *   status    device int32[n] or NULL: 0 gated, 1 converged, 2 stopped at max_iterations without meeting tol
+ *   iterations  device int32[n] or NULL: the linearisations taken (1 for a gated filter)
+ *   loss, loss_k  device int32[M] CPI_LOSS_* and double[M] thresholds, both or neither (neither: every measurement Gaussian)
+ * A filter without measurements is copied bit for bit with gamma = 0, status 1 and 0 iterations.  tol = +inf takes exactly one
+ * iteration, cpi_state_update_measurements_batch without a loss (to rounding); tol = 0 takes exactly max_iterations unless a step is exactly
+ * zero.  A cov that is not SPD, or a NaN in a measurement, gives NaN outputs for that filter only (it stops with status 2).
+ * CPI_EINVAL for n < 0, max_iterations < 1, a NaN or negative tol, only one of loss / loss_k, a NULL required pointer, or an output
+ * equal to an input or another output.  n = 0 launches nothing.
+ */
+int cpi_state_update_measurements_iterated_batch(int64_t n, const double* states, const double* cov, const int64_t* meas_offsets,
+                                                 const int32_t* kind, const double* z, const double* sqrt_info, const double* aux,
+                                                 const int32_t* loss /* or NULL */, const double* loss_k /* or NULL */,
+                                                 const double* gate, int max_iterations, double tol, double* states_out, double* cov_out,
+                                                 double* nis, int32_t* status, int32_t* iterations, void* stream);
+
 /* ---- window builder (host) ------------------------------------------------------------------------------------------------------ */
 
 /*
