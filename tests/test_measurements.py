@@ -199,7 +199,8 @@ def _ms_dev(torch, ms):
 @pytest.mark.gpu
 def test_kernel_is_the_statement(cuda):
     """K12 against linearize_ref for every kind (and an unknown one, NaN) at random states: every field within 1e-13 of the scale it
-    is formed at; info exactly symmetric; the f-only pass bitwise the full pass's f; two runs give the same bits."""
+    is formed at; info exactly symmetric; the f-only pass bitwise the full pass's f; two runs give the same bits.  K12's
+    extended-precision gate on the measurement stress batch is tests/test_measurements_precision.py."""
     from cpi_b200 import factor
     torch = cuda
     rng = np.random.default_rng(20)

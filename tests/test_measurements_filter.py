@@ -31,7 +31,8 @@ def _run(torch, x, cov, owner, kind, z, si, aux, gate=None):
 def test_kernel_is_the_statement(cuda):
     """0 to 4 measurements of every kind per filter (owners shuffled: the wrapper sorts them): every field within 20x the distance
     between the square-root and the information statements (floor 1e-13); cov+ exactly symmetric; a filter without measurements
-    bitwise its inputs with gamma = 0 and applied = 1; two runs give the same bits."""
+    bitwise its inputs with gamma = 0 and applied = 1; two runs give the same bits.  K11's extended-precision gate on the measurement
+    stress batch is tests/test_measurements_precision.py."""
     torch = cuda
     rng = np.random.default_rng(70)
     counts = rng.integers(0, 5, size=400)

@@ -11,6 +11,7 @@ import numpy as np
 import pytest
 
 from cpi_b200 import capi, synth
+from robust_loss_ref import np_loss
 from test_chains_lm import DEFAULTS, dev_prior, make_problem, np_cost, well_posed
 from test_marginalize import _dense_truth, _np_hessian, local, marginalize_ref, mat, prior_at_ref, random_prior, vec
 from test_state_priors import (_chain_idx, _dev, _meas_priors, _np_system, _per_chain_sps, _sp_dev, csr, dense_chain, fold_ref,
@@ -23,31 +24,6 @@ HUBER_K, CAUCHY_K = 1.345, 2.3849          # GTSAM's 95 %-efficiency thresholds
 # ------------------------------------------------------------------------------------------------------------------
 # numpy statements
 # ------------------------------------------------------------------------------------------------------------------
-
-def np_loss(code, k, s):
-    """(w, c) of whitened squared residuals s under loss codes `code` with thresholds k (arrays, broadcast): the header's table.
-    An unknown code or k outside 0 < k^2 < inf gives NaN."""
-    code, k, s = (np.asarray(a) for a in np.broadcast_arrays(code, k, s))
-    s = s.astype(np.float64)
-    w, c = np.full(s.shape, np.nan), np.full(s.shape, np.nan)
-    with np.errstate(all="ignore"):
-        k2 = k * k
-        ok = (k > 0) & (k2 > 0) & np.isfinite(k2)
-        g = code == capi.LOSS_GAUSSIAN
-        w[g], c[g] = 1.0, s[g]
-        hi = (code == capi.LOSS_HUBER) & ok & (s <= k2)
-        w[hi], c[hi] = 1.0, s[hi]
-        ho = (code == capi.LOSS_HUBER) & ok & ~(s <= k2)
-        r = np.sqrt(s[ho])
-        w[ho], c[ho] = k[ho] / r, 2.0 * k[ho] * r - k2[ho]
-        ca = (code == capi.LOSS_CAUCHY) & ok
-        u = s[ca] / k2[ca]
-        w[ca], c[ca] = 1.0 / (1.0 + u), k2[ca] * np.log1p(u)
-        big = np.zeros(s.shape, bool)
-        big[ca] = np.isinf(u)                                      # k < 1 and finite s above k^2 DBL_MAX: u overflows
-        w[big], c[big] = k2[big] / s[big], k2[big] * (np.log(s[big]) - np.log(k2[big]))
-    return w, c
-
 
 def robust_ref(code, k, info, rhs, f):
     """The kernel's statement: (w info, w rhs, c(f)) per prior; a weight of 1 copies."""

@@ -146,7 +146,8 @@ def test_kernel_is_the_statement(cuda):
     """400 filters, 0 to 4 measurements of every kind, Gaussian, Huber and Cauchy losses, owners shuffled.  tol = 0 with 1, 3 and 8
     iterations: every field within 20x the distance between the square-root and the information statements (floor 1e-13), and the
     same iteration counts.  tol = 1e-9: status and iterations equal the statement's on every filter whose stopping tests all lie
-    further than 1e-6 (relative) from the threshold."""
+    further than 1e-6 (relative) from the threshold.  K13's extended-precision gate on the measurement stress batch is
+    tests/test_measurements_precision.py."""
     torch = cuda
     rng, counts, x, cov, off, owner, kind, z, si, aux, loss = _mixed(40)
     perm = rng.permutation(len(owner))

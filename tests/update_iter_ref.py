@@ -6,6 +6,7 @@ from __future__ import annotations
 import numpy as np
 
 import measurement_ref as mr
+from robust_loss_ref import np_loss
 from test_marginalize import local, mat, vec
 from update_ref import retract
 
@@ -13,15 +14,9 @@ GAUSSIAN, HUBER, CAUCHY = 0, 1, 2
 
 
 def weight(code, k, s):
-    """The IRLS weight omega(s) of robust_loss (robust_loss.cuh) for whitened squared residuals s [M]."""
-    code, k, s = np.broadcast_arrays(np.asarray(code), np.asarray(k, dtype=float), np.asarray(s, dtype=float))
-    w = np.ones(s.shape)
-    with np.errstate(divide="ignore", invalid="ignore"):
-        h = (code == HUBER) & (s > k * k)
-        w[h] = k[h] / np.sqrt(s[h])
-        c = code == CAUCHY
-        w[c] = 1.0 / (1.0 + s[c] / (k[c] * k[c]))
-    return w
+    """The IRLS weight omega(s) of robust_loss (robust_loss.cuh) for whitened squared residuals s [M]: robust_loss_ref.np_loss's,
+    with the Cauchy branch where u = s/k^2 overflows (omega = k^2/s there, not 1/(1 + inf) = 0)."""
+    return np_loss(code, k, s)[0]
 
 
 def _weighted(kind, x, z, si, aux, code, k):

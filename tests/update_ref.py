@@ -6,6 +6,7 @@ from __future__ import annotations
 import atexit
 import ctypes
 import os
+import platform
 import shutil
 import subprocess
 import tempfile
@@ -81,20 +82,40 @@ def update_kalman(x, cov, W, xb, rows):
 _LIBS = {}
 
 
-def oracle(long_double=False):
-    """The plain-C statement (tests/update_oracle.c) in fp64 or long double, compiled on first use with oracle/Makefile's flags."""
-    key = bool(long_double)
+def _host_fma():
+    """Whether this x86-64 host executes FMA instructions (its CPU flags list fma); elsewhere gcc fuses with the target's own fma."""
+    if platform.machine() not in ("x86_64", "AMD64"):
+        return False
+    try:
+        with open("/proc/cpuinfo") as f:
+            return any(line.startswith("flags") and " fma " in line + " " for line in f)
+    except OSError:
+        return False
+
+
+def oracle(long_double=False, contract=False):
+    """The plain-C statement (tests/update_oracle.c) in fp64 or long double, compiled on first use with oracle/Makefile's flags;
+    contract (fp64 only): built with -ffp-contract=fast (and -mfma on x86-64), so that products fuse into fma as the kernels' do."""
+    key = (bool(long_double), bool(contract))
     if key not in _LIBS:
         tmp = tempfile.mkdtemp(prefix="cpi_update_oracle_")
         atexit.register(shutil.rmtree, tmp, True)
-        out = os.path.join(tmp, f"libupdate{'_ld' if key else ''}.so")
-        cmd = [os.environ.get("CC", "gcc"), "-std=c11", "-O2", "-fPIC", "-shared", "-fno-fast-math", "-ffp-contract=off", "-o", out,
-               os.path.join(_HERE, "update_oracle.c"), "-lm"] + (["-DCPI_ORACLE_LONG_DOUBLE"] if key else [])
+        out = os.path.join(tmp, f"libupdate{'_ld' if long_double else ''}{'_fma' if contract else ''}.so")
+        fp = ["-ffp-contract=fast"] + (["-mfma"] if _host_fma() else []) if contract else ["-ffp-contract=off"]
+        cmd = [os.environ.get("CC", "gcc"), "-std=c11", "-O2", "-fPIC", "-shared", "-fno-fast-math", *fp, "-o", out,
+               os.path.join(_HERE, "update_oracle.c"), "-lm"] + (["-DCPI_ORACLE_LONG_DOUBLE"] if long_double else [])
         subprocess.run(cmd, check=True)
         lib = ctypes.CDLL(out)
         P = ctypes.POINTER(ctypes.c_double)
         lib.oracle_state_update.argtypes = [ctypes.c_int64, P, P, P, P, ctypes.c_int, P, P, P, P]
         lib.oracle_state_update.restype = ctypes.c_int
+        I32, I64, c_int, c_dbl = ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int64), ctypes.c_int, ctypes.c_double
+        lib.oracle_measurements_linearize.argtypes = [ctypes.c_int64, I32, I64, P, P, P, P, c_int, P, P, P]
+        lib.oracle_state_update_measurements.argtypes = [ctypes.c_int64, P, P, I64, I32, P, P, P, c_int, P, P, P, P]
+        lib.oracle_state_update_measurements_iterated.argtypes = [ctypes.c_int64, P, P, I64, I32, P, P, P, I32, P, P, c_int, c_dbl,
+                                                                  I32, c_int, P, P, P, I32, I32, P, P, P]
+        for f in (lib.oracle_measurements_linearize, lib.oracle_state_update_measurements, lib.oracle_state_update_measurements_iterated):
+            f.restype = ctypes.c_int
         _LIBS[key] = lib
     return _LIBS[key]
 
@@ -107,6 +128,55 @@ def oracle_update(x, cov, W, xb, order, long_double=False):
     P = lambda v: v.ctypes.data_as(ctypes.POINTER(ctypes.c_double))
     assert oracle(long_double).oracle_state_update(n, *[P(v) for v in a], int(order), P(xo), P(co), P(xi), P(g)) == 0
     return xo, co, xi, g
+
+
+def _c(a, dtype):
+    """A C-contiguous copy-if-needed of a in dtype and its ctypes pointer (None stays NULL)."""
+    if a is None:
+        return None, None
+    a = np.ascontiguousarray(a, dtype=dtype)
+    return a, a.ctypes.data_as(ctypes.POINTER(np.ctypeslib.as_ctypes_type(dtype)))
+
+
+def oracle_linearize(kind, state_idx, states, z, si, aux, order, long_double=False):
+    """oracle_measurements_linearize (K12): order 0 A^T A, -A^T b, b^T b; order 1 H^T (S^T S) H, -H^T S^T (S r), |S r|^2.
+    Returns (info [M,225], rhs [M,15], f [M])."""
+    M = len(kind)
+    keep = [_c(kind, np.int32), _c(state_idx, np.int64), _c(states, np.float64), _c(z, np.float64), _c(si, np.float64), _c(aux, np.float64)]
+    info, rhs, f = np.zeros((M, 225)), np.zeros((M, 15)), np.zeros(M)
+    assert oracle(long_double).oracle_measurements_linearize(M, *[p for _, p in keep], int(order), *[_c(v, np.float64)[1]
+                                                                                                      for v in (info, rhs, f)]) == 0
+    return info, rhs, f
+
+
+def oracle_update_iter(x, cov, offsets, kind, z, si, aux, order, loss=None, loss_k=None, gate=None, max_iterations=10, tol=1e-9,
+                       force=None, long_double=False, contract=False):
+    """oracle_state_update_measurements_iterated (K13).  Returns (x+ [n,16], cov+ [n,225], gamma [n], status [n], iterations [n],
+    x_lin [n,16] the last linearisation point, margin [n], sharp [n] the largest lambda_max(L^T sum om A^T A L) it met)."""
+    n = len(x)
+    keep = [_c(x, np.float64), _c(cov, np.float64), _c(offsets, np.int64), _c(kind, np.int32), _c(z, np.float64), _c(si, np.float64),
+            _c(aux, np.float64), _c(loss, np.int32), _c(loss_k, np.float64), _c(gate, np.float64)]
+    fo = _c(force, np.int32)
+    out = [np.zeros((n, 16)), np.zeros((n, 225)), np.zeros(n), np.zeros(n, np.int32), np.zeros(n, np.int32), np.zeros(n),
+           np.zeros((n, 16)), np.zeros(n)]
+    ptrs = [_c(v, v.dtype)[1] for v in out]
+    assert oracle(long_double, contract).oracle_state_update_measurements_iterated(
+        n, *[p for _, p in keep], int(max_iterations), float(tol), fo[1], int(order), ptrs[0], ptrs[1], ptrs[2], ptrs[3], ptrs[4], ptrs[5],
+        ptrs[6], ptrs[7]) == 0
+    xo, co, g, st, it, mg, xl, sh = out
+    return xo, co, g, st, it, xl, mg, sh
+
+
+def oracle_update_meas(x, cov, offsets, kind, z, si, aux, order, long_double=False, contract=False):
+    """oracle_state_update_measurements (K11): order 0 the square-root form, 1 the information form.  Returns (x+ [n,16],
+    cov+ [n,225], gamma [n], sharp [n] = lambda_max(L^T sum A^T A L))."""
+    n = len(x)
+    keep = [_c(x, np.float64), _c(cov, np.float64), _c(offsets, np.int64), _c(kind, np.int32), _c(z, np.float64), _c(si, np.float64),
+            _c(aux, np.float64)]
+    out = [np.zeros((n, 16)), np.zeros((n, 225)), np.zeros(n), np.zeros(n)]
+    assert oracle(long_double, contract).oracle_state_update_measurements(n, *[p for _, p in keep], int(order), *[_c(v, np.float64)[1]
+                                                                                                           for v in out]) == 0
+    return tuple(out)
 
 
 # ---------------------------------------------------------------------------------------------- inputs
