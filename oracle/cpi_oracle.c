@@ -490,10 +490,11 @@ static void quat_mat(const real* q, real sign, real* M) {
 }
 
 /* ImuFactorCPIv1::evaluateError (ImuFactorCPIv1.cpp:37-208); model 2: ImuFactorCPIv2.cpp:38-212 */
-static void factor_eval(int model, const double* xi_in, const double* xj_in, const double* r_in, const double* l_in,
-                        double* err_out, double* H1, double* H2) {
-    real xi[CPI_STATE_DOUBLES], xj[CPI_STATE_DOUBLES], r[CPI_REC_V2_DOUBLES], l[CPI_LIN_DOUBLES], err[15];
-    load(xi, xi_in, CPI_STATE_DOUBLES); load(xj, xj_in, CPI_STATE_DOUBLES); load(l, l_in, CPI_LIN_DOUBLES);
+/* on states held in `real` (propagate_one keeps x_k1 unrounded); the entry below loads double states */
+static void factor_eval_r(int model, const real* xi, const real* xj, const double* r_in, const double* l_in,
+                          real* err, real* Hi, real* Hj) {
+    real r[CPI_REC_V2_DOUBLES], l[CPI_LIN_DOUBLES];
+    load(l, l_in, CPI_LIN_DOUBLES);
     load(r, r_in, model == 1 ? CPI_REC_V1_DOUBLES : CPI_REC_V2_DOUBLES);
     const real *q_GtoK = xi, *bg_K = xi + 4, *v_K = xi + 7, *ba_K = xi + 10, *p_K = xi + 13;
     const real *q_GtoK1 = xj, *bg_K1 = xj + 4, *v_K1 = xj + 7, *ba_K1 = xj + 10, *p_K1 = xj + 13;
@@ -544,8 +545,8 @@ static void factor_eval(int model, const double* xi_in, const double* xj_in, con
         err[12 + i] = alphahat[i] - alpha[i];
     }
     real eye[9]; mat_eye(eye, 3);
-    if (H1) {                                                                 /* :98-154 */
-        real Hi[225], A[9], Bm[9], AB[9], blk[9], sk[9], v3[3];
+    if (Hi) {                                                                 /* :98-154 */
+        real A[9], Bm[9], AB[9], blk[9], sk[9], v3[3];
         mat_zero(Hi, 225);
         quat_mat(q_n, -1.0, A); quat_mat(q_m, -1.0, Bm); gemm(3, 3, 3, A, Bm, AB);
         for (int j = 0; j < 3; j++) for (int i = 0; i < 3; i++) E(blk, 3, i, j) = -(E(AB, 3, i, j) + q_n[i] * q_m[j]);
@@ -567,25 +568,32 @@ static void factor_eval(int model, const double* xi_in, const double* xj_in, con
         set_block(Hi, 15, 9, 9, 3, 3, eye, -1.0);                             /* :137 */
         set_block(Hi, 15, 12, 9, 3, 3, H_alpha, -1.0);                        /* :139 */
         set_block(Hi, 15, 12, 12, 3, 3, Rk, -1.0);                            /* :143 */
-        store(H1, Hi, 225);
     }
-    if (H2) {                                                                 /* :158-198 */
-        real Hj[225], A[9];
+    if (Hj) {                                                                 /* :158-198 */
+        real A[9];
         mat_zero(Hj, 225);
         quat_mat(q_r, +1.0, A); set_block(Hj, 15, 0, 0, 3, 3, A, 1.0);        /* :169 */
         set_block(Hj, 15, 3, 3, 3, 3, eye, 1.0);
         set_block(Hj, 15, 6, 6, 3, 3, Rk, 1.0);
         set_block(Hj, 15, 9, 9, 3, 3, eye, 1.0);
         set_block(Hj, 15, 12, 12, 3, 3, Rk, 1.0);
-        store(H2, Hj, 225);
     }
+}
+
+static void factor_eval(int model, const double* xi_in, const double* xj_in, const double* r_in, const double* l_in,
+                        double* err_out, double* H1, double* H2) {
+    real xi[CPI_STATE_DOUBLES], xj[CPI_STATE_DOUBLES], err[15], Hi[225], Hj[225];
+    load(xi, xi_in, CPI_STATE_DOUBLES); load(xj, xj_in, CPI_STATE_DOUBLES);
+    factor_eval_r(model, xi, xj, r_in, l_in, err, H1 ? Hi : 0, H2 ? Hj : 0);
+    if (H1) store(H1, Hi, 225);
+    if (H2) store(H2, Hj, 225);
     store(err_out, err, 15);
 }
 
 /* getpredictedstate_v1 / _v2, solvers/GraphSolver_IMU.cpp:263-307 */
-static void predict_state(int model, const double* x_in, const double* r_in, const double* l_in, double* o_out) {
-    real x[CPI_STATE_DOUBLES], r[CPI_REC_V2_DOUBLES], l[CPI_LIN_DOUBLES], o[CPI_STATE_DOUBLES];
-    load(x, x_in, CPI_STATE_DOUBLES); load(l, l_in, CPI_LIN_DOUBLES); load(r, r_in, model == 1 ? CPI_REC_V1_DOUBLES : CPI_REC_V2_DOUBLES);
+static void predict_state_r(int model, const real* x, const double* r_in, const double* l_in, real* o) {
+    real r[CPI_REC_V2_DOUBLES], l[CPI_LIN_DOUBLES];
+    load(l, l_in, CPI_LIN_DOUBLES); load(r, r_in, model == 1 ? CPI_REC_V1_DOUBLES : CPI_REC_V2_DOUBLES);
     const real *q_GtoK = x, *bg_K = x + 4, *v_K = x + 7, *ba_K = x + 10, *p_K = x + 13, *grav = l + 10;
     real dt = r[CPI_REC_DT], qi[4], Rinv[9], rb[3], ra[3];
     quat_multiply(r + CPI_REC_Q, q_GtoK, o);
@@ -601,6 +609,12 @@ static void predict_state(int model, const double* x_in, const double* r_in, con
             o[13 + i] = p_K[i] + v_K[i] * dt + ra[i];
         }
     }
+}
+
+static void predict_state(int model, const double* x_in, const double* r_in, const double* l_in, double* o_out) {
+    real x[CPI_STATE_DOUBLES], o[CPI_STATE_DOUBLES];
+    load(x, x_in, CPI_STATE_DOUBLES);
+    predict_state_r(model, x, r_in, l_in, o);
     store(o_out, o, CPI_STATE_DOUBLES);
 }
 
@@ -618,6 +632,202 @@ static void retract(const double* x_in, const double* xi_in, double* o_out) {
     quat_multiply(dq, x, o);
     for (int i = 0; i < 12; i++) o[4 + i] = x[4 + i] + xi[3 + i];
     store(o_out, o, CPI_STATE_DOUBLES);
+}
+
+/* ------------------------------------------------------------------ K7: covariance propagation (DESIGN.md 3d) ----- */
+/* Not a reference routine: a statement of cpi_propagate_batch, x_k1 = predict_state(x_k), H1 / H2 the dense Jacobians of
+ * factor_eval at (x_k, x_k1), A = -H2^-1 H1, B = H2^-1, Sigma_k1 = A Sigma_k A^T + B P_meas B^T, C = Sigma_k A^T.  x_k1 stays in
+ * `real`, so the long-double build forms the Jacobians at the unrounded prediction.  order 0 is independent of the kernel's algebra:
+ * B by a pivoted Gauss-Jordan inverse of the dense H2 and every product a dense 15x15 one.  order 1 restates propagate.cu: the
+ * closed-form Q^-1 and Rk^T, the sparse theta / v / p rows of A with their exact I and DT I blocks, N = A Sigma_k column by column,
+ * Sigma_k1 row by row from N with its upper triangle mirrored, C = N^T. */
+
+/* Inv = M^-1 (n x n, column-major) by Gauss-Jordan elimination with partial pivoting; 0 where a pivot is exactly zero */
+static int gj_inverse(int n, const real* M, real* Inv) {
+    real A[225];
+    memcpy(A, M, sizeof *A * (size_t)(n * n));
+    mat_eye(Inv, n);
+    for (int c = 0; c < n; c++) {
+        int p = c;
+        for (int i = c + 1; i < n; i++) if (fabs(E(A, n, i, c)) > fabs(E(A, n, p, c))) p = i;
+        if (E(A, n, p, c) == 0) return 0;
+        if (p != c)
+            for (int j = 0; j < n; j++) {
+                real t = E(A, n, p, j); E(A, n, p, j) = E(A, n, c, j); E(A, n, c, j) = t;
+                t = E(Inv, n, p, j); E(Inv, n, p, j) = E(Inv, n, c, j); E(Inv, n, c, j) = t;
+            }
+        const real d = E(A, n, c, c);
+        for (int j = 0; j < n; j++) { E(A, n, c, j) /= d; E(Inv, n, c, j) /= d; }
+        for (int i = 0; i < n; i++) {
+            const real f = E(A, n, i, c);
+            if (i == c || f == 0) continue;
+            for (int j = 0; j < n; j++) { E(A, n, i, j) -= f * E(A, n, c, j); E(Inv, n, i, j) -= f * E(Inv, n, c, j); }
+        }
+    }
+    return 1;
+}
+
+/* the 3x3 coefficient blocks of A's theta, v and p rows (propagate.cu's cf), (i, j) = E(blk, 3, i, j) */
+typedef struct { real tt[9], tb[9], vt[9], vb[9], va[9], pt[9], pb[9], pa[9], dt; } arows_t;
+
+/* x <- A x in place, propagate.cu a_apply's order: p rows first (they read v), then v, theta last */
+static void a_apply_r(real* x, const arows_t* a) {
+    for (int i = 0; i < 3; i++) {
+        real tp = x[12 + i] + a->dt * x[6 + i];
+        for (int j = 0; j < 3; j++) tp += E(a->pt, 3, i, j) * x[j] + E(a->pb, 3, i, j) * x[3 + j] + E(a->pa, 3, i, j) * x[9 + j];
+        x[12 + i] = tp;
+    }
+    for (int i = 0; i < 3; i++) {
+        real tv = x[6 + i];
+        for (int j = 0; j < 3; j++) tv += E(a->vt, 3, i, j) * x[j] + E(a->vb, 3, i, j) * x[3 + j] + E(a->va, 3, i, j) * x[9 + j];
+        x[6 + i] = tv;
+    }
+    real t0[3];
+    for (int i = 0; i < 3; i++) {
+        t0[i] = 0;
+        for (int j = 0; j < 3; j++) t0[i] += E(a->tt, 3, i, j) * x[j] + E(a->tb, 3, i, j) * x[3 + j];
+    }
+    x[0] = t0[0]; x[1] = t0[1]; x[2] = t0[2];
+}
+
+/* one window: x (16) and S (225, column-major) in, x1, S1 and C (may be NULL) out, all in `real` */
+static void propagate_one(int model, const real* x, const real* S, const double* r_in, const double* l_in, int order, real* x1,
+                          real* S1, real* C) {
+    real e[15], H1[225], H2[225], Pm[225], B[225], A[225], T[225], U[225];
+    predict_state_r(model, x, r_in, l_in, x1);
+    factor_eval_r(model, x, x1, r_in, l_in, e, H1, H2);
+    load(Pm, r_in + CPI_REC_P, 225);
+    if (order == 0) {
+        if (!gj_inverse(15, H2, B)) for (int k = 0; k < 225; k++) B[k] = NAN;
+        gemm(15, 15, 15, B, H1, A);
+        for (int k = 0; k < 225; k++) A[k] = -A[k];
+        gemm(15, 15, 15, A, S, T);
+        gemm_nt(15, 15, 15, T, A, S1);
+        gemm(15, 15, 15, B, Pm, T);
+        gemm_nt(15, 15, 15, T, B, U);
+        for (int k = 0; k < 225; k++) S1[k] += U[k];
+        if (C) gemm_nt(15, 15, 15, S, A, C);
+        return;
+    }
+    /* Q = w I + [v x] is H2's (theta, theta) block: Q^-1 = (w^2 I - w [v x] + v v^T) / (w |q_r|^2); Rk its (v, v) block */
+    const real w = E(H2, 15, 0, 0), v[3] = {E(H2, 15, 2, 1), E(H2, 15, 0, 2), E(H2, 15, 1, 0)};
+    const real d = 1 / (w * (w * w + v[0] * v[0] + v[1] * v[1] + v[2] * v[2]));
+    real K[9], Qi[9], Rt[9], Rk[9], blk[9];
+    skew_x(v, K);
+    for (int c = 0; c < 3; c++) for (int u = 0; u < 3; u++) E(Qi, 3, u, c) = ((u == c ? w * w : 0) - w * E(K, 3, u, c) + v[u] * v[c]) * d;
+    get_block(H2, 15, 6, 6, 3, 3, Rk);
+    transpose(3, 3, Rk, Rt);
+    arows_t a;
+    a.dt = r_in[CPI_REC_DT];
+    /* -H2_II^-1 H1_IJ: the theta row through Q^-1, the v and p rows through Rk^T */
+    struct { real* dst; const real* L; int r0, c0; } rows[8] = {
+        {a.tt, Qi, 0, 0}, {a.tb, Qi, 0, 1}, {a.vt, Rt, 2, 0}, {a.vb, Rt, 2, 1}, {a.va, Rt, 2, 3},
+        {a.pt, Rt, 4, 0}, {a.pb, Rt, 4, 1}, {a.pa, Rt, 4, 3}};
+    for (int k = 0; k < 8; k++) {
+        get_block(H1, 15, 3 * rows[k].r0, 3 * rows[k].c0, 3, 3, blk);
+        m3_mul(rows[k].L, blk, rows[k].dst);
+        for (int q = 0; q < 9; q++) rows[k].dst[q] = -rows[k].dst[q];
+    }
+    real N[225], col[15];
+    for (int j = 0; j < 15; j++) {                                           /* N(:, j) = A S(:, j) */
+        for (int k = 0; k < 15; k++) col[k] = E(S, 15, k, j);
+        a_apply_r(col, &a);
+        for (int k = 0; k < 15; k++) E(N, 15, k, j) = col[k];
+    }
+    for (int i = 0; i < 15; i++) {                                           /* S1(i, j >= i) = (A N(i, :)^T)_j + (B P B^T)(i, j) */
+        const int bI = i / 3, ii = i - 3 * bI;
+        for (int k = 0; k < 15; k++) col[k] = E(N, 15, i, k);
+        a_apply_r(col, &a);
+        real bi[3];                                                          /* row ii of B_I: Q^-1, I or Rk^T */
+        for (int c = 0; c < 3; c++) bi[c] = bI == 0 ? E(Qi, 3, ii, c) : (bI == 2 || bI == 4) ? E(Rt, 3, ii, c) : (c == ii ? 1 : 0);
+        for (int bJ = 0; bJ < 5; bJ++) {
+            real t[3], s[3];
+            for (int m = 0; m < 3; m++) {
+                const int k = 3 * bJ + m;
+                t[m] = bi[0] * E(Pm, 15, 3 * bI, k) + bi[1] * E(Pm, 15, 3 * bI + 1, k) + bi[2] * E(Pm, 15, 3 * bI + 2, k);
+            }
+            for (int m = 0; m < 3; m++) {                                    /* ... B_J^T on the right */
+                if (bJ == 0) s[m] = t[0] * E(Qi, 3, m, 0) + t[1] * E(Qi, 3, m, 1) + t[2] * E(Qi, 3, m, 2);
+                else if (bJ == 2 || bJ == 4) s[m] = t[0] * E(Rt, 3, m, 0) + t[1] * E(Rt, 3, m, 1) + t[2] * E(Rt, 3, m, 2);
+                else s[m] = t[m];
+            }
+            for (int m = 0; m < 3; m++) {
+                const int j = 3 * bJ + m;
+                if (j >= i) { const real y = col[j] + s[m]; E(S1, 15, i, j) = y; E(S1, 15, j, i) = y; }
+            }
+        }
+    }
+    if (C) transpose(15, 15, N, C);
+}
+
+/* the two entries below: windows (chains) [lo, hi) of one job per thread */
+typedef struct {
+    int model, order, t, nt; int64_t n, steps;
+    const double *states, *cov, *path, *records, *lin; const int64_t* anchor;
+    double *states_out, *cov_out, *cross;
+} pjob_t;
+
+static void* pworker(void* arg) {
+    const pjob_t* j = (const pjob_t*)arg;
+    const int rd = j->model == 1 ? CPI_REC_V1_DOUBLES : CPI_REC_V2_DOUBLES;
+    const int64_t lo = j->n * j->t / j->nt, hi = j->n * (j->t + 1) / j->nt;
+    for (int64_t i = lo; i < hi; i++) {
+        real x[CPI_STATE_DOUBLES], S[225], x1[CPI_STATE_DOUBLES], S1[225], C[225];
+        if (j->steps == 0) {                                                 /* oracle_propagate: window i */
+            const int64_t a = j->anchor ? j->anchor[i] : i;
+            load(x, j->states + a * CPI_STATE_DOUBLES, CPI_STATE_DOUBLES);
+            load(S, j->cov + a * 225, 225);
+            propagate_one(j->model, x, S, j->records + i * (int64_t)rd, j->lin + i * CPI_LIN_DOUBLES, j->order, x1, S1, j->cross ? C : 0);
+            store(j->states_out + i * CPI_STATE_DOUBLES, x1, CPI_STATE_DOUBLES);
+            store(j->cov_out + i * 225, S1, 225);
+            if (j->cross) store(j->cross + i * 225, C, 225);
+            continue;
+        }
+        load(x, j->states + i * CPI_STATE_DOUBLES, CPI_STATE_DOUBLES);       /* oracle_propagate_chain: chain i */
+        load(S, j->cov + i * 225, 225);
+        for (int64_t k = 0; k < j->steps; k++) {
+            const int64_t w = i * j->steps + k;
+            if (j->path) load(x, j->path + (i * (j->steps + 1) + k) * CPI_STATE_DOUBLES, CPI_STATE_DOUBLES);
+            propagate_one(j->model, x, S, j->records + w * (int64_t)rd, j->lin + w * CPI_LIN_DOUBLES, j->order, x1, S1, 0);
+            memcpy(x, x1, sizeof x); memcpy(S, S1, sizeof S);
+        }
+        store(j->states_out + i * CPI_STATE_DOUBLES, x, CPI_STATE_DOUBLES);
+        store(j->cov_out + i * 225, S, 225);
+    }
+    return 0;
+}
+
+static void prun(pjob_t* proto, int nthreads) {
+    if (nthreads < 1) nthreads = 1;
+    if (nthreads > 256) nthreads = 256;
+    pjob_t jobs[256]; pthread_t th[256];
+    for (int t = 0; t < nthreads; t++) { jobs[t] = *proto; jobs[t].t = t; jobs[t].nt = nthreads; }
+    if (nthreads == 1) { pworker(&jobs[0]); return; }
+    for (int t = 0; t < nthreads; t++) pthread_create(&th[t], 0, pworker, &jobs[t]);
+    for (int t = 0; t < nthreads; t++) pthread_join(th[t], 0);
+}
+
+int oracle_propagate(int model, int64_t n, const double* states_k, const double* cov_k, const int64_t* anchor, const double* records,
+                     const double* lin, int order, double* states_k1, double* cov_k1, double* cross, int nthreads) {
+    if ((model != 1 && model != 2) || (order != 0 && order != 1)) return -1;
+    pjob_t j; memset(&j, 0, sizeof j);
+    j.model = model; j.order = order; j.n = n; j.states = states_k; j.cov = cov_k; j.anchor = anchor; j.records = records; j.lin = lin;
+    j.states_out = states_k1; j.cov_out = cov_k1; j.cross = cross;
+    prun(&j, nthreads);
+    return 0;
+}
+
+/* `steps` windows of K7 per chain (records and lin chain-major, [n_chains * steps]), the state and covariance held in `real`
+ * between steps.  path (may be NULL) [n_chains * (steps + 1), 16]: step k starts from path's state k of the chain instead of the
+ * statement's own prediction, so that the covariance recursion can follow a given (the device's) trajectory. */
+int oracle_propagate_chain(int model, int64_t n_chains, int64_t steps, const double* states0, const double* cov0, const double* path,
+                           const double* records, const double* lin, int order, double* states_out, double* cov_out, int nthreads) {
+    if ((model != 1 && model != 2) || (order != 0 && order != 1) || steps < 1) return -1;
+    pjob_t j; memset(&j, 0, sizeof j);
+    j.model = model; j.order = order; j.n = n_chains; j.steps = steps; j.states = states0; j.cov = cov0; j.path = path;
+    j.records = records; j.lin = lin; j.states_out = states_out; j.cov_out = cov_out;
+    prun(&j, nthreads);
+    return 0;
 }
 
 /* ------------------------------------------------------------------ merging model-1 records (DESIGN.md 3b, 3c) ---- */

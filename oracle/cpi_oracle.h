@@ -55,6 +55,15 @@ int oracle_local(int64_t n, const double* lin, const double* x, double* delta);
 int oracle_prior_at(int64_t n, const double* info, const double* rhs, const double* f, const double* lin, const double* x, double* rhs_out,
                     double* f_out);
 
+/* K7 (DESIGN.md 3d): x_k1, Sigma_k1 = A Sigma_k A^T + B P_meas B^T and cross = Sigma_k A^T (may be NULL) of window i from the state
+ * and covariance of anchor[i] (anchor NULL: i); order 0 dense (a pivoted inverse of H2), 1 propagate.cu's sparse route.
+ * propagate_chain: `steps` windows per chain, state and covariance held in working precision between steps; path (may be NULL)
+ * [n_chains * (steps + 1), 16] the states each step starts from.  Both split their windows (chains) over nthreads threads. */
+int oracle_propagate(int model, int64_t n, const double* states_k, const double* cov_k, const int64_t* anchor, const double* records,
+                     const double* lin, int order, double* states_k1, double* cov_k1, double* cross, int nthreads);
+int oracle_propagate_chain(int model, int64_t n_chains, int64_t steps, const double* states0, const double* cov0, const double* path,
+                           const double* records, const double* lin, int order, double* states_out, double* cov_out, int nthreads);
+
 /* quat_ops.h helpers (col-major 3x3) */
 void oracle_rot_2_quat(const double* R, double* q);
 void oracle_quat_2_Rot(const double* q, double* R);

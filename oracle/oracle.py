@@ -267,6 +267,42 @@ class Oracle(_Base):
         assert fn(C, _i(offs), u, *[_d(x) for x in a], dp(pc), _d(fnw), dp(pn), _d(out), int(nthreads)) == 0
         return out
 
+    # ---- K7, the covariance propagation (DESIGN.md 3d)
+    def propagate(self, model, states_k, cov_k, records, lin, order=0, anchor=None, want_cross=True, nthreads=1):
+        """(x_k1 [n,16], cov_k1 [n,225], cross [n,225] or None) of cpi_propagate_batch_host: order 0 the dense statement (a pivoted
+        inverse of H2, dense products), 1 the sparse route of propagate.cu."""
+        fn = self._rec_fn("oracle_propagate", [ctypes.c_int, ctypes.c_int64, _P, _P, _PI, _P, _P, ctypes.c_int, _P, _P, _P, ctypes.c_int])
+        X = np.ascontiguousarray(states_k, dtype=np.float64).reshape(-1, 16)
+        S = np.ascontiguousarray(cov_k, dtype=np.float64).reshape(-1, 225)
+        rec = np.ascontiguousarray(records, dtype=np.float64).reshape(-1, REC_DOUBLES[model])
+        lin = np.ascontiguousarray(lin, dtype=np.float64).reshape(-1, 13)
+        n = rec.shape[0]
+        an = np.arange(n, dtype=np.int64) if anchor is None else np.ascontiguousarray(anchor, dtype=np.int64)
+        assert an.shape == (n,) and lin.shape[0] == n and (n == 0 or (an.min() >= 0 and an.max() < len(X) and len(S) == len(X)))
+        x1, c1 = np.zeros((n, 16)), np.zeros((n, 225))
+        cr = np.zeros((n, 225)) if want_cross else None
+
+        assert fn(model, n, _d(X), _d(S), _i(an), _d(rec), _d(lin), int(order), _d(x1), _d(c1), None if cr is None else _d(cr),
+                  int(nthreads)) == 0
+        return x1, c1, cr
+
+    def propagate_chain(self, model, states0, cov0, records, lin, steps, order=0, path=None, nthreads=1):
+        """(x [C,16], cov [C,225]) after `steps` windows of K7 per chain (records / lin chain-major [C * steps]), held in working
+        precision between steps; path [C * (steps + 1), 16]: the states each step starts from (default: the statement's own)."""
+        fn = self._rec_fn("oracle_propagate_chain", [ctypes.c_int, ctypes.c_int64, ctypes.c_int64, _P, _P, _P, _P, _P, ctypes.c_int,
+                                                      _P, _P, ctypes.c_int])
+        X = np.ascontiguousarray(states0, dtype=np.float64).reshape(-1, 16)
+        S = np.ascontiguousarray(cov0, dtype=np.float64).reshape(-1, 225)
+        C = X.shape[0]
+        rec = np.ascontiguousarray(records, dtype=np.float64).reshape(C, steps, REC_DOUBLES[model])
+        lin = np.ascontiguousarray(lin, dtype=np.float64).reshape(C, steps, 13)
+        pth = None if path is None else np.ascontiguousarray(path, dtype=np.float64).reshape(C, steps + 1, 16)
+        xo, co = np.zeros((C, 16)), np.zeros((C, 225))
+
+        assert fn(model, C, int(steps), _d(X), _d(S), None if pth is None else _d(pth), _d(rec), _d(lin), int(order), _d(xo), _d(co),
+                  int(nthreads)) == 0
+        return xo, co
+
     def local(self, lin, x):
         """local(x_lin, x) [n,15], the inverse of retract."""
         fn = self._rec_fn("oracle_local", [ctypes.c_int64, _P, _P, _P])
