@@ -99,7 +99,15 @@ class LMParams(ctypes.Structure):
                  relative_error_tol=1e-5, max_iterations=100):
         super().__init__(lambda_factor, lambda_lower, lambda_upper, min_model_fidelity, absolute_error_tol, relative_error_tol, max_iterations)
 SAMPLE_DOUBLES, LIN_DOUBLES, STATE_DOUBLES = 7, 13, 16
-FLAG_IMU_AVG, FLAG_ANALYTIC_JACOBIANS = 1, 2
+FLAG_IMU_AVG, FLAG_ANALYTIC_JACOBIANS, FLAG_DISCRETE = 1, 2, 4
+
+
+def check_discrete(model, dtype_bits, flags):
+    """FLAG_DISCRETE produces model-1 records in fp64 only (include/cpi_b200.h); raise before anything reaches the device."""
+    if flags & FLAG_DISCRETE and model != 1:
+        raise ValueError(f"FLAG_DISCRETE produces model-1 records: model must be 1 (got {model})")
+    if flags & FLAG_DISCRETE and dtype_bits != 64:
+        raise ValueError("FLAG_DISCRETE is fp64 only")
 # record field slices (include/cpi_b200.h)
 REC = dict(q=(0, 4), R=(4, 13), alpha=(13, 16), beta=(16, 19), DT=(19, 20), J_q=(20, 29), J_a=(29, 38), J_b=(38, 47),
            H_a=(47, 56), H_b=(56, 65), P=(65, 290), O_a=(290, 299), O_b=(299, 308))

@@ -104,11 +104,20 @@ int dev_buf(int slot, size_t bytes, void** out) {
     return CPI_OK;
 }
 
+// CPI_FLAG_DISCRETE produces model-1 records in fp64 only
+int check_discrete(int model, int dtype, int flags) {
+    if (!(flags & CPI_FLAG_DISCRETE)) return CPI_OK;
+    if (model != 1) return fail(CPI_EINVAL, "CPI_FLAG_DISCRETE produces model-1 records: model must be 1 (got %d)", model);
+    if (dtype != 64) return fail(CPI_EINVAL, "CPI_FLAG_DISCRETE is fp64 only: dtype must be 64 (got %d)", dtype);
+    return CPI_OK;
+}
+
 int preintegrate_dev(int model, int dtype, int64_t n_windows, const int64_t* sample_offsets, int64_t ns_uniform,
                             const void* samples, const void* lin, const double* sigmas, int flags, void* out_records, void* stream, int wpb,
                             const void* init_records = nullptr) {
     if (model != 1 && model != 2) return fail(CPI_EINVAL, "model must be 1 or 2 (got %d)", model);
     if (dtype != 64 && dtype != 32) return fail(CPI_EINVAL, "dtype must be 64 or 32 (got %d)", dtype);
+    if (int rc = check_discrete(model, dtype, flags)) return rc;
     if (n_windows < 0 || (!sample_offsets && ns_uniform < 0)) return fail(CPI_EINVAL, "negative count");
     if (n_windows >= 2147483647) return fail(CPI_EINVAL, "too many windows (%lld; at most 2^31 - 2 per call)", (long long)n_windows);
     if (n_windows == 0) return CPI_OK;
@@ -123,8 +132,9 @@ int preintegrate_dev(int model, int dtype, int64_t n_windows, const int64_t* sam
     cpi::PreintParams p;
     p.n_windows = n_windows; p.offsets = sample_offsets; p.ns_uniform = ns_uniform;
     p.samples = samples; p.lin = lin; p.out = out_records; p.init = init_records;
-    if (init_records && !cpi::preint_tri_supported(model, flags))
-        return fail(CPI_EINVAL, "continuation is implemented for the default modes only (no imu_avg, model 2 with state_transition_jacobians)");
+    if (init_records && !cpi::preint_tri_supported(model, flags) && (flags & (CPI_FLAG_DISCRETE | CPI_FLAG_IMU_AVG)) != CPI_FLAG_DISCRETE)
+        return fail(CPI_EINVAL, "continuation is implemented for the default modes and the discrete mode only (no imu_avg, model 2 with "
+                                "state_transition_jacobians)");
     p.q_w = sigmas[0] * sigmas[0]; p.q_wb = sigmas[1] * sigmas[1]; p.q_a = sigmas[2] * sigmas[2]; p.q_ab = sigmas[3] * sigmas[3];
     p.wpb = wpb;
     int launches = 0;
@@ -138,7 +148,7 @@ int preintegrate_dev(int model, int dtype, int64_t n_windows, const int64_t* sam
 extern "C" {
 
 const char* cpi_last_error(void) { return g_err.c_str(); }
-const char* cpi_version(void) { return "cpi_b200 0.2 (sm_90a)"; }
+const char* cpi_version(void) { return "cpi_b200 0.3 (sm_90a)"; }
 int cpi_record_doubles(int model) { return model == 1 ? CPI_REC_V1_DOUBLES : (model == 2 ? CPI_REC_V2_DOUBLES : CPI_EINVAL); }
 int64_t cpi_launch_count(void) { return g_launches.load(); }
 
@@ -178,6 +188,7 @@ int cpi_imu_records_relinearize(int model, int64_t n_factors, const double* stat
                                 void* workspace, void* stream) {
     if (n_relinearized) *n_relinearized = 0;
     if (model != 1 && model != 2) return fail(CPI_EINVAL, "model must be 1 or 2 (got %d)", model);
+    if (int rc = check_discrete(model, 64, flags)) return rc;
     if (n_factors < 0 || (!sample_offsets && ns_uniform < 0)) return fail(CPI_EINVAL, "negative count");
     if (n_factors >= 2147483647) return fail(CPI_EINVAL, "too many factors (%lld; at most 2^31 - 2 per call)", (long long)n_factors);
     const double tols[3] = {tol_bw, tol_ba, tol_theta};
@@ -218,6 +229,7 @@ int cpi_preintegrate_batch_host(int model, int dtype, int64_t n_windows, const i
                                 const void* samples, const void* lin, const double* sigmas, int flags, void* out_records) {
     if (model != 1 && model != 2) return fail(CPI_EINVAL, "model must be 1 or 2 (got %d)", model);
     if (dtype != 64 && dtype != 32) return fail(CPI_EINVAL, "dtype must be 64 or 32 (got %d)", dtype);
+    if (int rc = check_discrete(model, dtype, flags)) return rc;
     if (n_windows < 0) return fail(CPI_EINVAL, "negative count");
     if (n_windows == 0) return CPI_OK;
     if (!lin || !sigmas || !out_records) return fail(CPI_EINVAL, "null pointer argument");

@@ -26,7 +26,7 @@ struct PreintParams {
     const void* samples;      // device, double (dtype 64) or float (dtype 32)
     const void* lin;          // device
     void* out;                // device
-    const void* init;         // device, may be null: records holding the state to CONTINUE from (may alias `out`); tri-lane kernels only
+    const void* init;         // device, may be null: records holding the state to CONTINUE from (may alias `out`); tri-lane and discrete kernels only
     double q_w, q_wb, q_a, q_ab;   // sigma^2  (CpiBase.h:54-57)
     int wpb;                  // windows per block; 0 on entry = let preint_launch choose (one wave if possible)
 };
@@ -49,6 +49,9 @@ int preint_cap(int model, int dtype, int flags, int num_sms);
 bool preint_tri_supported(int model, int flags);
 int preint_tri_cap(int model, int dtype);
 cudaError_t preint_launch_tri(int model, int dtype, const PreintParams& p, int num_sms, cudaStream_t st);
+// discrete (Forster) kernel, model 1 fp64 (preintegrate_discrete.cu)
+int preint_discrete_cap();
+cudaError_t preint_launch_discrete(int flags, const PreintParams& p, int num_sms, cudaStream_t st);
 cudaError_t preint_launch(int model, int dtype, int flags, const PreintParams& p0, int num_sms, int max_smem_bytes, cudaStream_t st, int* launches);
 cudaError_t factor_launch(int model, const FactorParams& p, cudaStream_t st);
 cudaError_t predict_launch(int model, int64_t n, const double* states, const double* records, const double* lin, double* out, cudaStream_t st);

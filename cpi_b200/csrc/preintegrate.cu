@@ -1040,6 +1040,7 @@ int preint_pick_wpb(int model, int dtype, int64_t n_windows, int num_sms) {
 }
 
 int preint_cap(int model, int dtype, int flags, int num_sms) {
+    if (flags & CPI_FLAG_DISCRETE) return preint_discrete_cap();
     if (preint_tri_supported(model, flags)) return preint_tri_cap(model, dtype);
     return preint_pick_wpb(model, dtype, (int64_t)1 << 40, num_sms);
 }
@@ -1057,6 +1058,10 @@ cudaError_t preint_launch(int model, int dtype, int flags, const PreintParams& p
     PreintParams p = p0;
     if (p.n_windows == 0) return cudaSuccess;
     if (max_smem_bytes < 232448) return cudaErrorInvalidConfiguration;
+    if (flags & CPI_FLAG_DISCRETE) {
+        if (launches) *launches = 1;
+        return preint_launch_discrete(flags, p, num_sms, st);
+    }
     if (preint_tri_supported(model, flags)) {
         if (launches) *launches = 1;
         return preint_launch_tri(model, dtype, p, num_sms, st);

@@ -797,7 +797,7 @@ int preint_tri_cap(int model, int dtype) {
     return dtype == 32 ? TriSmem<2, float>::WPB : TriSmem<2, double>::WPB;
 }
 bool preint_tri_supported(int model, int flags) {
-    if (flags & CPI_FLAG_IMU_AVG) return false;
+    if (flags & (CPI_FLAG_IMU_AVG | CPI_FLAG_DISCRETE)) return false;
     return model == 1 || (model == 2 && !(flags & CPI_FLAG_ANALYTIC_JACOBIANS));
 }
 

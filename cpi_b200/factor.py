@@ -1051,6 +1051,7 @@ def relinearize_records(model, states, records, lin, chain_offsets, samples, sig
     lib = capi.load()
     if model not in (1, 2):
         raise ValueError(f"model must be 1 or 2 (got {model})")
+    capi.check_discrete(model, 64, flags)
     for name, t in (("tol_bw", tol_bw), ("tol_ba", tol_ba), ("tol_theta", tol_theta)):
         if not float(t) >= 0.0:
             raise ValueError(f"{name} must be >= 0 (math.inf disables the test; got {t})")

@@ -49,6 +49,7 @@ def preintegrate_host(model, samples, lin, sigmas, flags=0, offsets=None, ns=Non
     dtype = np.dtype(dtype)
     if dtype not in (np.dtype(np.float64), np.dtype(np.float32)):
         raise ValueError("dtype must be float64 or float32")
+    capi.check_discrete(model, 8 * dtype.itemsize, flags)
     samples = np.ascontiguousarray(samples, dtype=dtype).reshape(-1, 7)
     lin = np.ascontiguousarray(lin, dtype=dtype).reshape(-1, 13)
     sig = np.ascontiguousarray(sigmas, dtype=np.float64)
@@ -86,6 +87,7 @@ def preintegrate(model, samples, lin, sigmas, flags=0, offsets=None, ns=None, ou
         raise ValueError("samples and lin must both be float64 or both float32")
     tdt = samples.dtype
     dev = samples.device
+    capi.check_discrete(model, 64 if tdt == torch.float64 else 32, flags)
     if continue_records is not None:
         if out is not None:
             raise ValueError("give either out or continue_records")

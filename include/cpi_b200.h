@@ -74,6 +74,10 @@ extern "C" {
                                            trailing entry whose (w,a) are the "_1" arguments of the last step */
 #define CPI_FLAG_ANALYTIC_JACOBIANS  2  /* model 2 only: state_transition_jacobians = false (CpiV2.h:58); default
                                            (flag clear) is the reference's default/true path (GraphSolver_IMU.cpp:100) */
+#define CPI_FLAG_DISCRETE            4  /* model 1, fp64 only: discrete (Forster) preintegration instead of CpiV1's closed
+                                           forms -- first-order means and bias Jacobians and P' = Phi P Phi^T + Q per step, written
+                                           as a model-1 record that every consumer of model-1 records takes (DESIGN.md section 3n).
+                                           Model 2 or dtype 32 with this flag: CPI_EINVAL.  Until version 0.3 this bit was ignored. */
 
 /* error codes */
 #define CPI_OK          0
@@ -115,8 +119,10 @@ int cpi_preintegrate_batch(int model, int dtype, int64_t n_windows,
  * CpiV2 objects (feed_IMU accumulates into the object's fields, CpiBase.h:86, 99-124; every one of them is in the record).
  * `samples` / `sample_offsets` / `ns_uniform` describe the NEW samples only; lin, sigmas, flags must be those of the first call.
  * fp64: agrees with the one-shot call to rounding (~1e-15 relative; P_pp is re-split symmetrically).  dtype 32 continues from the
- * float-rounded record (the one-shot call carries the covariance state in fp64).  Default modes only (no CPI_FLAG_IMU_AVG, model 2
- * without CPI_FLAG_ANALYTIC_JACOBIANS): CPI_EINVAL otherwise.
+ * float-rounded record (the one-shot call carries the covariance state in fp64).  Default modes and CPI_FLAG_DISCRETE only (no
+ * CPI_FLAG_IMU_AVG, model 2 without CPI_FLAG_ANALYTIC_JACOBIANS): CPI_EINVAL otherwise.  With CPI_FLAG_DISCRETE the record is the whole
+ * state of the recursion, so splitting a window at any sample gives the one-shot record bit for bit.  `records` must have been made
+ * with the same flags: continuing a closed-form record discretely (or the reverse) is undefined, and the call cannot detect it.
  */
 int cpi_preintegrate_batch_continue(int model, int dtype, int64_t n_windows,
                                     const int64_t* sample_offsets, int64_t ns_uniform,
