@@ -1109,6 +1109,29 @@ int cpi_state_update_measurements_iterated_batch(int64_t n, const double* states
     return CPI_OK;
 }
 
+int cpi_rts_smooth_batch(int64_t n_runs, const int64_t* run_offsets, int64_t run_uniform, int64_t n_states, const double* states,
+                         const double* cov, const double* pred_states, const double* pred_cov, const double* cross, double* states_out,
+                         double* cov_out, double* cross_out, void* stream) {
+    int rc = chain_layout_check(n_runs, run_offsets, run_uniform, n_states);
+    if (rc || n_runs == 0) return rc;
+    const bool any_step = n_states > n_runs;                       // a transition exists
+    if (!states || !cov || !states_out || !cov_out || (any_step && (!pred_states || !pred_cov || !cross)))
+        return fail(CPI_EINVAL, "null pointer argument");
+    const void* ins[6] = {run_offsets, states, cov, pred_states, pred_cov, cross};
+    const void* outs[3] = {states_out, cov_out, cross_out};
+    for (const void* o : outs)
+        for (const void* q : ins)
+            if (o && o == q) return fail(CPI_EINVAL, "outputs must not overlap inputs");
+    if (states_out == cov_out || (cross_out && (cross_out == states_out || cross_out == cov_out)))
+        return fail(CPI_EINVAL, "outputs must not overlap each other");
+    DevInfo d;
+    if ((rc = device_info(d))) return rc;
+    CU(cpi::rts_smooth_launch(n_runs, run_offsets, run_offsets ? 0 : run_uniform, states, cov, pred_states, pred_cov, cross, states_out, cov_out,
+                              cross_out, (cudaStream_t)stream));
+    g_launches += 1;
+    return CPI_OK;
+}
+
 int cpi_imu_measurements_linearize(int64_t n, const int32_t* kind, const int64_t* state_idx, const double* states, const double* z,
                                    const double* sqrt_info, const double* aux, double* info, double* rhs, double* f, void* stream) {
     if (n < 0) return fail(CPI_EINVAL, "negative count");

@@ -119,6 +119,10 @@ cudaError_t state_update_meas_iter_launch(int64_t n, const double* states, const
                                           const double* z, const double* sqrt_info, const double* aux, const int32_t* loss, const double* loss_k,
                                           const double* gate, int max_iter, double tol, double* states_out, double* cov_out, double* nis,
                                           int32_t* status, int32_t* iterations, cudaStream_t st);
+// update.cu: Rauch-Tung-Striebel smoothing of filter runs from their posteriors and K7's predictions and cross (K15; cross_out may be NULL)
+cudaError_t rts_smooth_launch(int64_t n_runs, const int64_t* offs, int64_t uniform, const double* states, const double* cov,
+                              const double* pred_states, const double* pred_cov, const double* cross, double* states_out, double* cov_out,
+                              double* cross_out, cudaStream_t st);
 // measurements.cu: measurements linearised into moved prior blocks (K12; info, rhs NULL: the f-only pass)
 cudaError_t measurements_linearize_launch(int64_t n, const int32_t* kind, const int64_t* state_idx, const double* states, const double* z,
                                           const double* sqrt_info, const double* aux, double* info, double* rhs, double* f, cudaStream_t st);

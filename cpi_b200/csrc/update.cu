@@ -549,4 +549,156 @@ cudaError_t state_update_meas_iter_launch(int64_t n, const double* states, const
     return cudaGetLastError();
 }
 
+// K15: Rauch-Tung-Striebel smoothing of filter runs (DESIGN.md section 3o).  Run c holds keyframes o[c] .. o[c+1]-1 with the
+// filter's posteriors (x_k, P_k); its transitions are stored from o[c] - c, transition k carrying K7's prediction (xb_{k+1},
+// Pb_{k+1}) and cross C_k = P_k A_k^T from (x_k, P_k).  From the last keyframe (copied bit for bit) backwards:
+//   G = C_k Pb^-1 (Pb = L L^T),  d = local(xb_{k+1}, xs_{k+1}),  xs_k = retract(x_k, G d),
+//   Ps_k = P_k + G (Ps_{k+1} - Pb) G^T,  Xs_k = G Ps_{k+1}  (the smoothed (x_k, x_{k+1}) block)
+// One warp per run, sequential over its keyframes; xs_{k+1} and Ps_{k+1} are carried in shared memory.  Lane i < 15 solves row i
+// of G from row i of C_k with L (two per-lane triangular solves) while lane 15 forms d, then row i of T = G (Ps_{k+1} - Pb), row i
+// of Xs_k and (G d)_i; after a sync it forms row i of Ps_k left of the diagonal and mirrors it, so Ps_k is exactly symmetric, while
+// lane 15 retracts.  A Pb that is not SPD gives NaN from that keyframe back, in that run only.  No atomics: the same bits on every run.
+constexpr int RP = 240;                          // one 15x15 matrix, row-major with pitch 16
+
+__global__ void __launch_bounds__(UWARPS * 32) k_rts_smooth(int64_t n_runs, const int64_t* offs, int64_t uniform, const double* states,
+                                                           const double* cov, const double* pred_states, const double* pred_cov,
+                                                           const double* cross, double* states_out, double* cov_out, double* cross_out) {
+    __shared__ double smem[UWARPS][5 * RP + 64];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int64_t c = (int64_t)blockIdx.x * UWARPS + warp;
+    if (c >= n_runs) return;
+    double* Pb = smem[warp];                      // Pb_{k+1}
+    double* L = Pb + RP;                          // its Cholesky factor (lower triangle)
+    double* G = L + RP;                           // C_k, then G row by row
+    double* Ps = G + RP;                          // Ps_{k+1}, then Ps_k
+    double* Pk = Ps + RP;                         // P_k
+    double* XS = Pk + RP;                         // xs_{k+1}, then xs_k
+    double* XK = XS + 16;                         // x_k
+    double* XB = XK + 16;                         // xb_{k+1}
+    double* GD = XB + 16;                         // G d
+    const int64_t o0 = offs ? __ldg(offs + c) : c * uniform;
+    const int64_t o1 = offs ? __ldg(offs + c + 1) : o0 + uniform;
+    const int64_t last = o1 - 1, t0 = o0 - c;     // the run's last keyframe and its first transition
+    {                                             // the last keyframe: copied, and carried
+        const double* sg = cov + last * 225;
+        double* co = cov_out + last * 225;
+        for (int e = lane; e < 225; e += 32) {
+            const double v = __ldg(sg + e);
+            co[e] = v;
+            Ps[(e % 15) * 16 + e / 15] = v;
+        }
+        if (lane < CPI_STATE_DOUBLES) {
+            const double v = __ldg(states + last * CPI_STATE_DOUBLES + lane);
+            states_out[last * CPI_STATE_DOUBLES + lane] = v;
+            XS[lane] = v;
+        }
+    }
+    for (int64_t s = last - 1; s >= o0; s--) {
+        const int64_t t = t0 + (s - o0);
+        const double* pg = pred_cov + t * 225;
+        const double* cg = cross + t * 225;
+        const double* sg = cov + s * 225;
+        for (int e = lane; e < 225; e += 32) {    // column-major (r, c) -> row-major pitch 16
+            const int r = e % 15, q = e / 15;
+            const double p = __ldg(pg + e);
+            Pb[r * 16 + q] = p;
+            L[r * 16 + q] = p;
+            G[r * 16 + q] = __ldg(cg + e);
+            Pk[r * 16 + q] = __ldg(sg + e);
+        }
+        if (lane < CPI_STATE_DOUBLES) {
+            XK[lane] = __ldg(states + s * CPI_STATE_DOUBLES + lane);
+            XB[lane] = __ldg(pred_states + t * CPI_STATE_DOUBLES + lane);
+        }
+        __syncwarp();
+        warp_chol15(L, lane);
+
+        if (lane < 15) {                          // row lane of G: Pb^-1 C_k(lane, :)^T (Pb symmetric)
+            double g[15];
+#pragma unroll
+            for (int k = 0; k < 15; k++) g[k] = G[lane * 16 + k];
+            fwd15(L, g);
+#pragma unroll
+            for (int k = 0; k < 15; k++) G[lane * 16 + k] = g[k];
+        }
+        __syncwarp();                             // L reloaded for the backward solve: the two solves do not hold it in registers
+        if (lane < 15) {
+            double g[15];
+#pragma unroll
+            for (int k = 0; k < 15; k++) g[k] = G[lane * 16 + k];
+            bwd15(L, g);
+#pragma unroll
+            for (int k = 0; k < 15; k++) G[lane * 16 + k] = g[k];
+        } else if (lane == 15) {                  // d = local(xb_{k+1}, xs_{k+1}) in the spare column 15 of G
+            double d[15];
+            local15(XB, XS, d);
+#pragma unroll
+            for (int r = 0; r < 15; r++) G[r * 16 + 15] = d[r];
+        }
+        __syncwarp();
+        if (lane < 15) {                          // row lane of T = G (Ps_{k+1} - Pb) into L (free after the solves), of Xs_k, and (G d)_lane
+            const double* g = G + lane * 16;
+            double gd = 0.0;
+#pragma unroll
+            for (int m = 0; m < 15; m++) gd = fma(g[m], G[m * 16 + 15], gd);
+            GD[lane] = gd;
+            double tr[15];
+#pragma unroll
+            for (int j = 0; j < 15; j++) tr[j] = 0.0;
+#pragma unroll 1
+            for (int m = 0; m < 15; m++) {
+                const double gm = g[m];
+#pragma unroll
+                for (int j = 0; j < 15; j++) tr[j] = fma(gm, Ps[m * 16 + j] - Pb[m * 16 + j], tr[j]);
+            }
+#pragma unroll
+            for (int j = 0; j < 15; j++) L[lane * 16 + j] = tr[j];
+            if (cross_out) {                      // Xs_k(lane, j) = G(lane, :) Ps_{k+1}(:, j), column-major: coalesced over lanes
+                double* xo = cross_out + t * 225;
+#pragma unroll 1
+                for (int j = 0; j < 15; j++) {
+                    double x = 0.0;
+#pragma unroll
+                    for (int m = 0; m < 15; m++) x = fma(g[m], Ps[m * 16 + j], x);
+                    xo[lane + 15 * j] = x;
+                }
+            }
+        }
+        __syncwarp();
+        if (lane < 15) {                          // Ps_k(lane, j) = P_k(lane, j) + T(lane, :) G(j, :)^T, j <= lane, mirrored
+            double tr[15];
+#pragma unroll
+            for (int m = 0; m < 15; m++) tr[m] = L[lane * 16 + m];
+            for (int j = 0; j <= lane; j++) {
+                double v = 0.0;
+#pragma unroll
+                for (int m = 0; m < 15; m++) v = fma(tr[m], G[j * 16 + m], v);
+                v += Pk[lane * 16 + j];
+                Ps[lane * 16 + j] = v;
+                Ps[j * 16 + lane] = v;
+            }
+        } else if (lane == 15) {                  // xs_k = retract(x_k, G d)
+            double xo[16];
+            retract_state(XK, GD, xo);
+            double* o = states_out + s * CPI_STATE_DOUBLES;
+#pragma unroll
+            for (int k = 0; k < 16; k++) { XS[k] = xo[k]; o[k] = xo[k]; }
+        }
+        __syncwarp();
+        double* co = cov_out + s * 225;
+        for (int e = lane; e < 225; e += 32) co[e] = Ps[(e % 15) * 16 + e / 15];
+        __syncwarp();
+    }
+}
+
+cudaError_t rts_smooth_launch(int64_t n_runs, const int64_t* offs, int64_t uniform, const double* states, const double* cov,
+                              const double* pred_states, const double* pred_cov, const double* cross, double* states_out, double* cov_out,
+                              double* cross_out, cudaStream_t st) {
+    if (n_runs == 0) return cudaSuccess;
+    const int64_t grid = (n_runs + UWARPS - 1) / UWARPS;
+    k_rts_smooth<<<(unsigned)grid, UWARPS * 32, 0, st>>>(n_runs, offs, uniform, states, cov, pred_states, pred_cov, cross, states_out,
+                                                        cov_out, cross_out);
+    return cudaGetLastError();
+}
+
 }  // namespace cpi

@@ -1303,6 +1303,61 @@ def update_measurements_iterated(states, cov, measurements, gate=None, measureme
     return x1, c1, nis, status, iters
 
 
+def rts_smooth(model, states, cov, records, lin, run_offsets, cross=False, n_runs=None, stream=None):
+    """Fixed-interval (Rauch-Tung-Striebel) smoothing of many filter runs from the filter's own posteriors (cpi_rts_smooth_batch,
+    kernel K15; DESIGN.md section 3o).  Runs use the chain layout of chains_marginals: run_offsets is a device int64 tensor [n_runs+1]
+    of keyframe offsets or an int, the keyframes per run (n_runs as chains_covariance's n_chains); run c's transitions are stored back
+    to back from index offsets[c] - c.  DEVICE float64 tensors: states [N,16] and cov [N,225] (column-major) the filter's posterior
+    (x_k, P_k) at every keyframe, the prediction itself where no update was applied; records [N - n_runs, RD] and lin
+    [N - n_runs, 13] per transition.  The records and lin must be the ones the filter propagated with.  One propagate(...,
+    want_cross=True) call over every transition recomputes the predictions (xb_{k+1}, Pb_{k+1}) and the cross C_k = P_k A_k^T; K7 is
+    deterministic, so they are bitwise the forward pass's own.  That pass allocates 3 728 B per transition (16 + 225 + 225 doubles).
+    Then, per run from its last keyframe (copied bit for bit) backwards:
+        G = C_k Pb_{k+1}^-1,  xs_k = retract(x_k, G local(xb_{k+1}, xs_{k+1})),  Ps_k = P_k + G (Ps_{k+1} - Pb_{k+1}) G^T,
+        Xs_k = G Ps_{k+1}
+    A Pb_{k+1} that is not SPD gives NaN for that run only.  Enqueues on ``stream`` (default: torch's current stream) without
+    synchronising.  Returns (states_s [N,16], cov_s [N,225] exactly symmetric, cross_s [N - n_runs,225] with Xs_k in transition k's
+    slot, the slots and orientation of chains_covariance's cross, or None)."""
+    import torch
+
+    if model not in (1, 2):
+        raise ValueError(f"model must be 1 or 2 (got {model!r})")
+    for name, t in (("states", states), ("cov", cov), ("records", records), ("lin", lin)):
+        if not isinstance(t, torch.Tensor):
+            raise ValueError(f"{name} must be a tensor")
+    if not states.is_cuda:
+        raise ValueError("states must be a CUDA tensor")
+    dev = states.device
+    _check_f64(dev, states=states, cov=cov, records=records, lin=lin)
+    N = states.numel() // 16
+    if N < 1 or states.numel() != 16 * N or cov.numel() != 225 * N:
+        raise ValueError("rts_smooth needs states [N,16] and cov [N,225] with at least one keyframe")
+    if isinstance(run_offsets, torch.Tensor):
+        if run_offsets.numel() - 1 > N:
+            raise ValueError(f"run_offsets has {run_offsets.numel()} entries: more runs than the {N} keyframes")
+        if n_runs is not None and n_runs != run_offsets.numel() - 1:
+            raise ValueError(f"run_offsets has {run_offsets.numel()} entries, not n_runs + 1 = {n_runs + 1}")
+    with _on(dev, stream):
+        C, offs, S = _chain_layout(run_offsets, dev, n_states=N, n_chains=n_runs)
+        nt = N - C
+        if C < 1 or nt < 0:
+            raise ValueError(f"{C} runs over {N} keyframes: every run holds a keyframe")
+        if records.numel() != nt * REC_DOUBLES[model] or lin.numel() != 13 * nt:
+            raise ValueError(f"{N - C} transitions need records [{nt},{REC_DOUBLES[model]}] and lin [{nt},13]")
+        states, cov = states.contiguous(), cov.contiguous()
+        if nt:
+            idx_i, _ = _chain_factor_states(C, offs, S, nt, dev)
+            xp, cp, cr = propagate(model, states, cov, records, lin, anchor=idx_i, want_cross=True, stream=stream)
+        else:
+            xp = cp = cr = None
+        f64 = dict(dtype=torch.float64, device=dev)
+        xs, cs = torch.empty((N, 16), **f64), torch.empty((N, 225), **f64)
+        xc = torch.empty((nt, 225), **f64) if cross else None
+        _launch(capi.load().cpi_rts_smooth_batch, dev, stream, C, _tptr(offs), S, N, _tptr(states), _tptr(cov), _tptr(xp), _tptr(cp),
+                _tptr(cr), _tptr(xs), _tptr(cs), _tptr(xc))
+    return xs, cs, xc
+
+
 def _filter_checks(states, cov, gate, name):
     """The host checks of the filter updates by measurements: states [n,16] and cov [n,225] float64 CUDA tensors on one device, and a
     gate that is None, a number other than NaN, or a float64 tensor [n] on that device.  Returns (device, n)."""

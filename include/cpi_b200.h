@@ -681,6 +681,37 @@ int cpi_state_update_measurements_iterated_batch(int64_t n, const double* states
                                                  const double* gate, int max_iterations, double tol, double* states_out, double* cov_out,
                                                  double* nis, int32_t* status, int32_t* iterations, void* stream);
 
+/*
+ * Fixed-interval (Rauch-Tung-Striebel) smoothing of many filter runs from the filter's own posteriors (DESIGN.md section 3o): the
+ * smoothed estimates of logged runs and Monte-Carlo batches without re-solving them.  fp64, DEVICE pointers, asynchronous on
+ * `stream`, one kernel launch, no allocation, no host synchronisation.  tests/rts_ref.py holds the numpy statement.
+ *
+ * Runs use the chain layout of cpi_imu_chains_marginals: run c holds keyframes o[c] .. o[c+1]-1 (run_offsets: device int64
+ * [n_runs+1], offsets[0] = 0, every run non-empty, not checked; or NULL and run_uniform keyframes per run), n_states keyframes in all;
+ * its transitions are stored back to back from index o[c] - c, transition j going from keyframe o[c]+j to o[c]+j+1.
+ *   states, cov   the filter's posterior (x_k, P_k) at every keyframe ([n_states] x CPI_STATE_DOUBLES, [n_states] x 225 column-major,
+ *                 the tangent space of cpi_retract_batch); at a keyframe without an update, or with a gated one, the prediction
+ *   pred_states, pred_cov, cross   per transition, what cpi_propagate_batch writes from (x_k, P_k) with the record and linearisation
+ *                 point the filter propagated with: (xb_{k+1}, Pb_{k+1}) and C_k = P_k A_k^T ([n_states - n_runs] entries each)
+ * Per run, from the last keyframe backwards:
+ *     xs_{S-1} = x_{S-1},  Ps_{S-1} = P_{S-1}                                     (bit-for-bit copies)
+ *     G_k = C_k Pb_{k+1}^-1            (Cholesky of Pb_{k+1}, never an explicit inverse)
+ *     d = local(xb_{k+1}, xs_{k+1}),   xs_k = retract(x_k, G_k d)
+ *     Ps_k = P_k + G_k (Ps_{k+1} - Pb_{k+1}) G_k^T                                (exactly symmetric: one triangle computed, mirrored)
+ *     Xs_k = G_k Ps_{k+1}                                                         (the smoothed (x_k, x_{k+1}) block)
+ *   states_out, cov_out   as states, cov;   cross_out   [n_states - n_runs] x 225, or NULL: Xs_k in transition k's slot, the slots
+ *                 and orientation of cpi_imu_chains_marginals' cross
+ * A one-keyframe run is copied.  P_k = 0 (an exact anchor) gives G_k = 0, Ps_k = 0 and xs_k = retract(x_k, 0): the 12 linear entries
+ * copied bit for bit, the quaternion renormalised within an ulp (as cpi_state_update_batch for W = 0).  xs_{k+1} == xb_{k+1} gives d = 0
+ * exactly.  A Pb_{k+1} that is not SPD (P_k = 0 with a zero-step record) gives NaN for that run only (one warp per run).
+ * CPI_EINVAL for n_runs < 0, a NULL required pointer (pred_states, pred_cov and cross may be NULL when n_states = n_runs), an output
+ * equal to an input or another output, or a layout that does not match n_states (n_states < n_runs, or != n_runs x run_uniform without
+ * run_offsets); outputs must not overlap inputs.  n_runs = 0 launches nothing.
+ */
+int cpi_rts_smooth_batch(int64_t n_runs, const int64_t* run_offsets, int64_t run_uniform, int64_t n_states, const double* states,
+                         const double* cov, const double* pred_states, const double* pred_cov, const double* cross, double* states_out,
+                         double* cov_out, double* cross_out /* or NULL */, void* stream);
+
 /* ---- window builder (host) ------------------------------------------------------------------------------------------------------ */
 
 /*
