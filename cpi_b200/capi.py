@@ -59,6 +59,8 @@ SYMBOLS = {
     "cpi_state_update_measurements_iterated_batch": (c_int, [c_i64] + [c_vp] * 10 + [c_int, ctypes.c_double] + [c_vp] * 6),
     "cpi_imu_measurements_linearize": (c_int, [c_i64] + [c_vp] * 10),
     "cpi_rts_smooth_batch": (c_int, [c_i64, c_vp, c_i64, c_i64] + [c_vp] * 9),
+    "cpi_rts_smooth_scan_workspace": (c_i64, [c_i64, c_i64]),
+    "cpi_rts_smooth_scan_batch": (c_int, [c_i64, c_vp, c_i64, c_i64] + [c_vp] * 10),
     "cpi_host_last_timing": (c_int, [c_vp, c_vp]),
     "cpi_host_register": (c_int, [c_vp, ctypes.c_size_t]),
     "cpi_host_unregister": (c_int, [c_vp]),

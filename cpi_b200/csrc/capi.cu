@@ -1132,6 +1132,40 @@ int cpi_rts_smooth_batch(int64_t n_runs, const int64_t* run_offsets, int64_t run
     return CPI_OK;
 }
 
+int64_t cpi_rts_smooth_scan_workspace(int64_t n_runs, int64_t n_states) {
+    if (n_runs < 0 || n_states < 0) return fail(CPI_EINVAL, "negative count");
+    if (n_states < n_runs) return fail(CPI_EINVAL, "n_states (%lld) < n_runs (%lld): every run holds a keyframe", (long long)n_states,
+                                       (long long)n_runs);
+    return n_states > n_runs ? cpi::rts_scan_workspace_bytes(n_states) : 0;
+}
+
+int cpi_rts_smooth_scan_batch(int64_t n_runs, const int64_t* run_offsets, int64_t run_uniform, int64_t n_states, const double* states,
+                              const double* cov, const double* pred_states, const double* pred_cov, const double* cross, double* states_out,
+                              double* cov_out, double* cross_out, void* workspace, void* stream) {
+    int rc = chain_layout_check(n_runs, run_offsets, run_uniform, n_states);
+    if (rc || n_runs == 0) return rc;
+    const bool any_step = n_states > n_runs;                       // a transition exists
+    if (!states || !cov || !states_out || !cov_out || (any_step && (!pred_states || !pred_cov || !cross)))
+        return fail(CPI_EINVAL, "null pointer argument");
+    if (any_step && !workspace) return fail(CPI_EINVAL, "null pointer argument (workspace: cpi_rts_smooth_scan_workspace bytes)");
+    const void* ins[6] = {run_offsets, states, cov, pred_states, pred_cov, cross};
+    const void* outs[4] = {states_out, cov_out, cross_out, workspace};
+    for (const void* o : outs)
+        for (const void* q : ins)
+            if (o && o == q) return fail(CPI_EINVAL, "outputs must not overlap inputs");
+    for (int i = 0; i < 4; i++)
+        for (int j = i + 1; j < 4; j++)
+            if (outs[i] && outs[i] == outs[j]) return fail(CPI_EINVAL, "outputs must not overlap each other");
+    DevInfo d;
+    if ((rc = device_info(d))) return rc;
+    int launches = 0;
+    cudaError_t e = cpi::rts_scan_launch(n_runs, run_offsets, run_offsets ? 0 : run_uniform, n_states, states, cov, pred_states, pred_cov,
+                                         cross, states_out, cov_out, cross_out, workspace, d.sms, (cudaStream_t)stream, &launches);
+    g_launches += launches;
+    CU(e);
+    return CPI_OK;
+}
+
 int cpi_imu_measurements_linearize(int64_t n, const int32_t* kind, const int64_t* state_idx, const double* states, const double* z,
                                    const double* sqrt_info, const double* aux, double* info, double* rhs, double* f, void* stream) {
     if (n < 0) return fail(CPI_EINVAL, "negative count");

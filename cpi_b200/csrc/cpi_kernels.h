@@ -123,6 +123,12 @@ cudaError_t state_update_meas_iter_launch(int64_t n, const double* states, const
 cudaError_t rts_smooth_launch(int64_t n_runs, const int64_t* offs, int64_t uniform, const double* states, const double* cov,
                               const double* pred_states, const double* pred_cov, const double* cross, double* states_out, double* cov_out,
                               double* cross_out, cudaStream_t st);
+// rts_scan.cu: the same smoothing by a segmented parallel scan over every keyframe (K16; cross_out may be NULL; workspace
+// rts_scan_workspace_bytes(n), unused when no run has a transition)
+int64_t rts_scan_workspace_bytes(int64_t n_states);
+cudaError_t rts_scan_launch(int64_t n_runs, const int64_t* offs, int64_t uniform, int64_t n, const double* states, const double* cov,
+                            const double* pred_states, const double* pred_cov, const double* cross, double* states_out, double* cov_out,
+                            double* cross_out, void* workspace, int sms, cudaStream_t st, int* launches);
 // measurements.cu: measurements linearised into moved prior blocks (K12; info, rhs NULL: the f-only pass)
 cudaError_t measurements_linearize_launch(int64_t n, const int32_t* kind, const int64_t* state_idx, const double* states, const double* z,
                                           const double* sqrt_info, const double* aux, double* info, double* rhs, double* f, cudaStream_t st);

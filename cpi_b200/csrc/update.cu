@@ -15,32 +15,12 @@
 #include "local15.cuh"
 #include "measurement.cuh"
 #include "robust_loss.cuh"
+#include "rts.cuh"
 
 namespace cpi {
 
 constexpr int UWARPS = 4;                        // filters (warps) per CTA
 constexpr int UP = 240;                          // one 15x15 matrix, row-major with pitch 16
-
-// JPLNavState::retract: the arithmetic of k_retract (factor.cu), kept as a local copy so that k_retract's code is untouched
-CPI_DEV void retract_state(const double* x, const double* d, double* o) {
-    const double nrm = sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
-    double s, c;
-    sincos(nrm / 2.0, &s, &c);
-    double dq[4] = {(s / nrm) * d[0], (s / nrm) * d[1], (s / nrm) * d[2], c};
-    double nn = sqrt(dq[0] * dq[0] + dq[1] * dq[1] + dq[2] * dq[2] + dq[3] * dq[3]);
-#pragma unroll
-    for (int k = 0; k < 4; k++) dq[k] /= nn;
-    if (dq[3] < 0) { dq[0] = -dq[0]; dq[1] = -dq[1]; dq[2] = -dq[2]; dq[3] = -dq[3]; }
-    nn = sqrt(dq[0] * dq[0] + dq[1] * dq[1] + dq[2] * dq[2] + dq[3] * dq[3]);
-    if (isnan(nn)) { dq[0] = dq[1] = dq[2] = 0.0; dq[3] = 1.0; }
-    const double q[4] = {x[0], x[1], x[2], x[3]};
-    double qn[4];
-    quat_multiply(dq, q, qn);
-#pragma unroll
-    for (int k = 0; k < 4; k++) o[k] = qn[k];
-#pragma unroll
-    for (int k = 0; k < 12; k++) o[4 + k] = x[4 + k] + d[3 + k];
-}
 
 __global__ void __launch_bounds__(UWARPS * 32) k_state_update(int64_t n, const double* states, const double* cov, const double* meas_info,
                                                              const double* meas_states, const double* gate, double* states_out,
@@ -611,30 +591,12 @@ __global__ void __launch_bounds__(UWARPS * 32) k_rts_smooth(int64_t n_runs, cons
             XB[lane] = __ldg(pred_states + t * CPI_STATE_DOUBLES + lane);
         }
         __syncwarp();
-        warp_chol15(L, lane);
-
-        if (lane < 15) {                          // row lane of G: Pb^-1 C_k(lane, :)^T (Pb symmetric)
-            double g[15];
-#pragma unroll
-            for (int k = 0; k < 15; k++) g[k] = G[lane * 16 + k];
-            fwd15(L, g);
-#pragma unroll
-            for (int k = 0; k < 15; k++) G[lane * 16 + k] = g[k];
-        }
-        __syncwarp();                             // L reloaded for the backward solve: the two solves do not hold it in registers
-        if (lane < 15) {
-            double g[15];
-#pragma unroll
-            for (int k = 0; k < 15; k++) g[k] = G[lane * 16 + k];
-            bwd15(L, g);
-#pragma unroll
-            for (int k = 0; k < 15; k++) G[lane * 16 + k] = g[k];
-        } else if (lane == 15) {                  // d = local(xb_{k+1}, xs_{k+1}) in the spare column 15 of G
+        rts_gain(L, G, lane, [&] {                // d = local(xb_{k+1}, xs_{k+1}) in the spare column 15 of G
             double d[15];
             local15(XB, XS, d);
 #pragma unroll
             for (int r = 0; r < 15; r++) G[r * 16 + 15] = d[r];
-        }
+        });
         __syncwarp();
         if (lane < 15) {                          // row lane of T = G (Ps_{k+1} - Pb) into L (free after the solves), of Xs_k, and (G d)_lane
             const double* g = G + lane * 16;

@@ -1358,6 +1358,59 @@ def rts_smooth(model, states, cov, records, lin, run_offsets, cross=False, n_run
     return xs, cs, xc
 
 
+def rts_smooth_scan(model, states, cov, records, lin, run_offsets, cross=False, n_runs=None, stream=None):
+    """rts_smooth's smoothing, parallel in time (cpi_rts_smooth_scan_batch, kernel K16; DESIGN.md section 3p): the same arguments,
+    checks, K7 pass and return values, then a segmented associative scan over every keyframe of every run instead of one warp
+    walking each run, so that one long run spreads over the whole device.  Covariances and cross are rts_smooth's up to
+    reassociation; the means follow the backward recursion linearised at the filtered states,
+        xs_k = retract(x_k, delta_k),  delta_k = G_k d0_k + G_k J_k delta_{k+1},  d0_k = local(xb_{k+1}, x_{k+1}),
+    which agrees with rts_smooth's to second order in delta (the parallel extended RTS smoother of Sarkka and Garcia-Fernandez).
+    Faster than rts_smooth on few long runs, slower on many short ones (DESIGN.md section 3p has the crossover).  Allocates the
+    workspace (cpi_rts_smooth_scan_workspace bytes: about 5.5 KB per keyframe) on the stream's device.  Enqueues on ``stream``
+    (default: torch's current stream) without synchronising.  Returns (states_s [N,16], cov_s [N,225] exactly symmetric, cross_s
+    [N - n_runs,225] or None)."""
+    import torch
+
+    if model not in (1, 2):
+        raise ValueError(f"model must be 1 or 2 (got {model!r})")
+    for name, t in (("states", states), ("cov", cov), ("records", records), ("lin", lin)):
+        if not isinstance(t, torch.Tensor):
+            raise ValueError(f"{name} must be a tensor")
+    if not states.is_cuda:
+        raise ValueError("states must be a CUDA tensor")
+    dev = states.device
+    _check_f64(dev, states=states, cov=cov, records=records, lin=lin)
+    N = states.numel() // 16
+    if N < 1 or states.numel() != 16 * N or cov.numel() != 225 * N:
+        raise ValueError("rts_smooth_scan needs states [N,16] and cov [N,225] with at least one keyframe")
+    if isinstance(run_offsets, torch.Tensor):
+        if run_offsets.numel() - 1 > N:
+            raise ValueError(f"run_offsets has {run_offsets.numel()} entries: more runs than the {N} keyframes")
+        if n_runs is not None and n_runs != run_offsets.numel() - 1:
+            raise ValueError(f"run_offsets has {run_offsets.numel()} entries, not n_runs + 1 = {n_runs + 1}")
+    with _on(dev, stream):
+        C, offs, S = _chain_layout(run_offsets, dev, n_states=N, n_chains=n_runs)
+        nt = N - C
+        if C < 1 or nt < 0:
+            raise ValueError(f"{C} runs over {N} keyframes: every run holds a keyframe")
+        if records.numel() != nt * REC_DOUBLES[model] or lin.numel() != 13 * nt:
+            raise ValueError(f"{N - C} transitions need records [{nt},{REC_DOUBLES[model]}] and lin [{nt},13]")
+        states, cov = states.contiguous(), cov.contiguous()
+        lib = capi.load()
+        if nt:
+            idx_i, _ = _chain_factor_states(C, offs, S, nt, dev)
+            xp, cp, cr = propagate(model, states, cov, records, lin, anchor=idx_i, want_cross=True, stream=stream)
+            ws = torch.empty(int(lib.cpi_rts_smooth_scan_workspace(C, N)), dtype=torch.uint8, device=dev)
+        else:
+            xp = cp = cr = ws = None
+        f64 = dict(dtype=torch.float64, device=dev)
+        xs, cs = torch.empty((N, 16), **f64), torch.empty((N, 225), **f64)
+        xc = torch.empty((nt, 225), **f64) if cross else None
+        _launch(lib.cpi_rts_smooth_scan_batch, dev, stream, C, _tptr(offs), S, N, _tptr(states), _tptr(cov), _tptr(xp), _tptr(cp),
+                _tptr(cr), _tptr(xs), _tptr(cs), _tptr(xc), _tptr(ws))
+    return xs, cs, xc
+
+
 def _filter_checks(states, cov, gate, name):
     """The host checks of the filter updates by measurements: states [n,16] and cov [n,225] float64 CUDA tensors on one device, and a
     gate that is None, a number other than NaN, or a float64 tensor [n] on that device.  Returns (device, n)."""

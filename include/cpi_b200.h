@@ -712,6 +712,37 @@ int cpi_rts_smooth_batch(int64_t n_runs, const int64_t* run_offsets, int64_t run
                          const double* cov, const double* pred_states, const double* pred_cov, const double* cross, double* states_out,
                          double* cov_out, double* cross_out /* or NULL */, void* stream);
 
+/*
+ * The same smoothing, parallel in time (DESIGN.md section 3p): a segmented associative scan over every keyframe of every run, so that
+ * one long run is spread over the whole device and its latency grows with the log of its length.  Inputs, outputs, layout and argument
+ * rules are cpi_rts_smooth_batch's, plus `workspace`: device, cpi_rts_smooth_scan_workspace(n_runs, n_states) bytes (0, and NULL
+ * allowed, when no run has a transition).  fp64, asynchronous on `stream`, a fixed number of launches for n_states (about
+ * 2 log16(n_states) + 3), no allocation, no host synchronisation; device offsets are never read on the host.
+ * tests/rts_scan_ref.py holds the numpy statement.  Per transition k of a run (keyframes k -> k+1):
+ *     G_k  = C_k Pb_{k+1}^-1                 (cpi_rts_smooth_batch's arithmetic: Cholesky of Pb_{k+1}, never an explicit inverse)
+ *     L_k  = P_k - G_k Pb_{k+1} G_k^T        (one triangle computed, mirrored)
+ *     d0_k = local(xb_{k+1}, x_{k+1})        (the filter's own correction at k+1; exactly 0 where no update was applied)
+ *     J_k  = d local(xb_{k+1}, retract(x_{k+1}, delta)) / d delta at 0 = diag(Jr^-1(phi), I_12), phi the rotation of d0_k and
+ *            Jr^-1(phi) = I + [phi]x / 2 + (1 - (t/2) cot(t/2)) / t^2 [phi]x^2, t = |phi|
+ * Covariances follow cpi_rts_smooth_batch's recursion Ps_k = L_k + G_k Ps_{k+1} G_k^T (Ps_{S-1} = P_{S-1}), reassociated: the
+ * elements (E, L) compose as (E_i, L_i) o (E_j, L_j) = (E_i E_j, L_i + E_i L_j E_i^T) (one triangle, mirrored: exactly symmetric),
+ * transition k's element starts as (G_k, L_k) and the run's terminal element is (0, P_{S-1}); Xs_k = G_k Ps_{k+1}.  Means follow the
+ * recursion linearised at the filtered states, xs_k = retract(x_k, delta_k) with
+ *     delta_k = G_k d0_k + G_k J_k delta_{k+1},   delta_{S-1} = 0
+ * (elements (B, a) = (G_k J_k, G_k d0_k) composing as (B_i B_j, a_i + B_i a_j)): the parallel extended RTS smoother of Sarkka and
+ * Garcia-Fernandez.  It agrees with cpi_rts_smooth_batch's means to second order in delta and is the same expression at a run's last
+ * transition; where every d0 = 0, delta = 0 exactly and xs_k = retract(x_k, 0) (the 12 linear entries bit for bit, the quaternion
+ * renormalised within an ulp).  The last keyframe of a run and one-keyframe runs are copied bit for bit; P_k = 0 gives G_k = 0.  Run
+ * boundaries are applied by selection, so a run whose Pb_{k+1} is not SPD is NaN alone, and every other run's bits do not depend on
+ * its neighbours.  No atomics: the same bits on every call.  CPI_EINVAL as cpi_rts_smooth_batch, and for a NULL workspace when a run
+ * has a transition or a workspace equal to an input or output; the workspace function returns CPI_EINVAL for a negative count or
+ * n_states < n_runs.
+ */
+int64_t cpi_rts_smooth_scan_workspace(int64_t n_runs, int64_t n_states);
+int cpi_rts_smooth_scan_batch(int64_t n_runs, const int64_t* run_offsets, int64_t run_uniform, int64_t n_states, const double* states,
+                              const double* cov, const double* pred_states, const double* pred_cov, const double* cross, double* states_out,
+                              double* cov_out, double* cross_out /* or NULL */, void* workspace, void* stream);
+
 /* ---- window builder (host) ------------------------------------------------------------------------------------------------------ */
 
 /*
