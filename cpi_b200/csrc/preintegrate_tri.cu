@@ -69,7 +69,10 @@ template <int MODEL, class T> struct TriSmem {
     // scalar sets: one slot per window + one dummy slot per warp for the two idle lanes
     static constexpr size_t off_buf = (off_sc + (size_t)(WPB + NT / 32) * TriSC<MODEL>::STRIDE * 8 + 127) / 128 * 128;
     static constexpr size_t off_bar = off_buf + (size_t)WPB * TRI_BUF_STRIDE;
-    static constexpr size_t bytes = off_bar + (size_t)WPB * 8 * TRI_NBUF;
+    // after the sample loop the whole allocation holds the CTA's records (rec_bytes, from offset 0), written out with 16-byte stores
+    static constexpr size_t rec_bytes = (size_t)WPB * (MODEL == 1 ? CPI_REC_V1_DOUBLES : CPI_REC_V2_DOUBLES) * sizeof(T);
+    static constexpr size_t loop_bytes = off_bar + (size_t)WPB * 8 * TRI_NBUF;
+    static constexpr size_t bytes = loop_bytes > rec_bytes ? loop_bytes : rec_bytes;
 };
 static_assert(TriSmem<1, double>::bytes <= 28160 - 1024 && TriSmem<1, float>::bytes <= 28160 - 1024 && TriSmem<2, double>::bytes <= 28160 - 1024 &&
               TriSmem<2, float>::bytes <= 28160 - 1024,
@@ -310,18 +313,21 @@ CPI_DEV void rot_col(double a, double b, const double* w, const double* v, doubl
 // Profiling-only builds (never shipped; tools/phase_builds.sh): the two phases the north_star wants measured separately.
 //   CPI_TRI_PHASE_LOAD  the TMA sample stream alone (stage, wait, read; no arithmetic)  -> achieved HBM GB/s of the sample-load phase
 //   CPI_TRI_PHASE_COV   the covariance RK4 alone on constant inputs (no fetch, no front)   -> fp64 FLOP/s of the covariance phase
+//   CPI_TRI_PHASE_NOPREPASS  constant scalar sets instead of the pre-pass (wrong output) -> the most that hiding the pre-pass can win
 #if defined(CPI_TRI_PHASE_LOAD)
-constexpr bool kLoadOnly = true, kCovOnly = false;
+constexpr bool kLoadOnly = true, kCovOnly = false, kNoPrepass = false;
 #elif defined(CPI_TRI_PHASE_COV)
-constexpr bool kLoadOnly = false, kCovOnly = true;
+constexpr bool kLoadOnly = false, kCovOnly = true, kNoPrepass = false;
+#elif defined(CPI_TRI_PHASE_NOPREPASS)
+constexpr bool kLoadOnly = false, kCovOnly = false, kNoPrepass = true;
 #else
-constexpr bool kLoadOnly = false, kCovOnly = false;
+constexpr bool kLoadOnly = false, kCovOnly = false, kNoPrepass = false;
 #endif
 
 enum : int { SC_A1 = 0, SC_B1, SC_A2, SC_B2, SC_F1, SC_F2, SC_F3, SC_F4, SC_DT6, SC_D1, SC_D2, SC_D3, SC_D4, SC_CA, SC_CB, SC_N };
 
 template <int MODEL, class T>
-__global__ void __launch_bounds__((TriNT<MODEL, T>::NT), 1) k_preintegrate_tri(const PreintParams p) {
+__global__ void __launch_bounds__((TriNT<MODEL, T>::NT), 1) k_preintegrate_tri(const PreintParams p, const bool tma) {
     using SM_ = TriSmem<MODEL, T>;
     constexpr int NT = SM_::NT;
     constexpr int CH = 8 / (int)sizeof(T) * 2;            // samples per TMA chunk: 2 (fp64) or 4 (fp32) = 112 B in one aligned 128-B fetch
@@ -342,7 +348,7 @@ __global__ void __launch_bounds__((TriNT<MODEL, T>::NT), 1) k_preintegrate_tri(c
     double* fs = reinterpret_cast<double*>(smem_raw + SM_::off_fs) + threadIdx.x;
     // per-window scalar sets of the current 3 samples (the two idle lanes of a warp get a dummy slot of their own)
     double* sc = reinterpret_cast<double*>(smem_raw + SM_::off_sc) + (size_t)(lane_ok ? wslot : SM_::WPB + wid) * TriSC<MODEL>::STRIDE;
-    const T* buf = reinterpret_cast<const T*>(smem_raw + SM_::off_buf + (size_t)wslot * TRI_BUF_STRIDE);
+    T* buf = reinterpret_cast<T*>(smem_raw + SM_::off_buf + (size_t)wslot * TRI_BUF_STRIDE);
     const uint32_t buf0 = smem_u32(buf);
     const uint32_t bar0 = smem_u32(smem_raw + SM_::off_bar + (size_t)wslot * (8 * TRI_NBUF));
 
@@ -377,9 +383,9 @@ __global__ void __launch_bounds__((TriNT<MODEL, T>::NT), 1) k_preintegrate_tri(c
     // ---- TMA pipeline: lane 0 of the trio stages the window's stream through a ring of TRI_NBUF 128-byte chunk buffers.  Chunk k
     // (samples CH k .. CH k + CH - 1, fetched as ONE aligned 128-byte transaction that also absorbs the misalignment of the
     // window start) lives in buffer k % NBUF, completes phase k / NBUF of barrier k % NBUF.  The last samples of a window are
-    // read with plain loads: an aligned 128-byte fetch there could run past the caller's buffer.
+    // not fetched by TMA (an aligned 128-byte fetch there could run past the caller's buffer) but copied by the pre-pass (ring).
     const int shift = (int)(((uintptr_t)sp & 15) / sizeof(T));      // misalignment of the window start w.r.t. 16 bytes, in elements
-    const int n_tma = nsteps > 0 ? (nsteps - 1) / CH : 0;           // chunks with at least one more sample after them
+    const int n_tma = (tma && nsteps > 0) ? (nsteps - 1) / CH : 0;  // chunks with at least one more sample after them (!tma: none)
     const int n_tma_samples = n_tma * CH;
     int next_issue = 0;
     if (active && c == 0) {
@@ -397,16 +403,11 @@ __global__ void __launch_bounds__((TriNT<MODEL, T>::NT), 1) k_preintegrate_tri(c
     }
     __syncwarp();                                                    // barrier init visible to the trio before anyone polls
 
-    // pointer to sample `is` of this window: staged copy (after waiting for its chunk) or global memory (tail); null steps return nullptr
-    auto sample_ptr = [&](int is, bool& from_smem) -> const T* {
-        from_smem = is < n_tma_samples;
-        if (from_smem) {
-            const int k = is / CH, b = k % TRI_NBUF;
-            mbar_wait(bar0 + 8 * b, (uint32_t)((k / TRI_NBUF) & 1));
-            return buf + b * EPC + shift + 7 * (is % CH);
-        }
-        return sp + (int64_t)is * CPI_SAMPLE_DOUBLES;
-    };
+    // ring position of sample `is`.  Samples before n_tma_samples arrive there by TMA (wait_chunk); the pre-pass copies the tail
+    // samples there from global memory, into the buffer of the never-fetched chunk n_tma (free: chunk n_tma - 3 was consumed groups
+    // earlier).  The sample bodies therefore read every sample with shared-memory loads, from one address and without a branch.
+    auto ring = [&](int is) -> T* { return buf + (is / CH % TRI_NBUF) * EPC + shift + 7 * (is % CH); };
+    auto wait_chunk = [&](int is) { const int k = is / CH; mbar_wait(bar0 + 8 * (k % TRI_NBUF), (uint32_t)((k / TRI_NBUF) & 1)); };
 
     // ---- state (CpiBase.h:99-124 initialisers), lane frame
     double R[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};                       // full old rotation, row-major
@@ -455,10 +456,14 @@ __global__ void __launch_bounds__((TriNT<MODEL, T>::NT), 1) k_preintegrate_tri(c
             const int is = it0 + c;
             double w0 = 0.0, w1 = 0.0, w2 = 0.0, dt = 0.0;
             if (is < nsteps && !kCovOnly) {
-                bool sm_;
-                const T* src = sample_ptr(is, sm_);
-                if (sm_) { w0 = (double)src[0]; w1 = (double)src[1]; w2 = (double)src[2]; dt = (double)src[6]; }
-                else { w0 = (double)__ldg(src); w1 = (double)__ldg(src + 1); w2 = (double)__ldg(src + 2); dt = (double)__ldg(src + 6); }
+                T* dst = ring(is);
+                if (is < n_tma_samples) wait_chunk(is);
+                else {                                               // tail sample: staged here for the sample bodies
+                    const T* src = sp + (int64_t)is * CPI_SAMPLE_DOUBLES;
+#pragma unroll
+                    for (int e = 0; e < CPI_SAMPLE_DOUBLES; e++) dst[e] = __ldg(src + e);
+                }
+                w0 = (double)dst[0]; w1 = (double)dst[1]; w2 = (double)dst[2]; dt = (double)dst[6];
             }
             w0 -= bwo[0]; w1 -= bwo[1]; w2 -= bwo[2];                // CpiV1.h:77-79
             const double mag = sqrt(w0 * w0 + w1 * w1 + w2 * w2);
@@ -473,7 +478,10 @@ __global__ void __launch_bounds__((TriNT<MODEL, T>::NT), 1) k_preintegrate_tri(c
 #pragma unroll
             for (int e = 0; e < SC_N; e++) v[e] = 0.0;
             if (kLoadOnly || kCovOnly) v[SC_A1] = w0 + w1 + w2 + dt;
-            else if (!null_step) {
+            else if (kNoPrepass) {
+#pragma unroll
+                for (int e = 0; e < SC_N; e++) v[e] = 1e-3;
+            } else if (!null_step) {
                 const double hd = 0.5 * dt, dt2 = dt * dt, dt3 = dt2 * dt;
                 v[SC_DT6] = dt / 6.0;                                // CpiV1.h:352
                 if (small_w) {                                       // Taylor forms: CpiV1.h:119-120, 132-136, 162-164, 196-216, 267-268
@@ -520,17 +528,11 @@ __global__ void __launch_bounds__((TriNT<MODEL, T>::NT), 1) k_preintegrate_tri(c
             double wm[3] = {0, 0, 0}, am[3] = {0, 0, 0}, dt = 0.0;
             if (kCovOnly) { wm[0] = 0.1; wm[1] = -0.2; wm[2] = 0.3; am[0] = 0.1; am[1] = 0.2; am[2] = 9.8; dt = 0.005; }
             else if (it < nsteps) {
-                bool sm_;
-                const T* src = sample_ptr(it, sm_);
-                if (sm_) {
-                    wm[0] = (double)src[i0]; wm[1] = (double)src[i1]; wm[2] = (double)src[i2];
-                    am[0] = (double)src[3 + i0]; am[1] = (double)src[3 + i1]; am[2] = (double)src[3 + i2];
-                    dt = (double)src[6];
-                } else {
-                    wm[0] = (double)__ldg(src + i0); wm[1] = (double)__ldg(src + i1); wm[2] = (double)__ldg(src + i2);
-                    am[0] = (double)__ldg(src + 3 + i0); am[1] = (double)__ldg(src + 3 + i1); am[2] = (double)__ldg(src + 3 + i2);
-                    dt = (double)__ldg(src + 6);
-                }
+                if (it < n_tma_samples) wait_chunk(it);
+                const T* src = ring(it);
+                wm[0] = (double)src[i0]; wm[1] = (double)src[i1]; wm[2] = (double)src[i2];
+                am[0] = (double)src[3 + i0]; am[1] = (double)src[3 + i1]; am[2] = (double)src[3 + i2];
+                dt = (double)src[6];
             }
             DT += dt;                                                // CpiV1.h:69 (before the dt == 0 return)
             if (kLoadOnly) { DT += wm[0] + wm[1] + wm[2] + am[0] + am[1] + am[2]; continue; }
@@ -728,42 +730,74 @@ __global__ void __launch_bounds__((TriNT<MODEL, T>::NT), 1) k_preintegrate_tri(c
     sTT[0] = P.TT[0]; sTT[1] = 0.5 * (P.TT[1] + shf(P.TT[2], nx)); sTT[2] = 0.5 * (P.TT[2] + shf(P.TT[1], pv));
     sVV[0] = P.VV[0]; sVV[1] = 0.5 * (P.VV[1] + shf(P.VV[2], nx)); sVV[2] = 0.5 * (P.VV[2] + shf(P.VV[1], pv));
     sPP[0] = P.PP[0] + P.PP[0]; sPP[1] = P.PP[1] + shf(P.PP[2], nx); sPP[2] = P.PP[2] + shf(P.PP[1], pv);     // PP = Q + Q^T (exactly symmetric: a + b == b + a)
-    if (!active) return;
+    // The record is assembled in shared memory (the sample loop's slots, scalar sets and TMA ring are dead now) and the warp then
+    // streams its windows' records, which are contiguous in `out`, with coalesced 16-byte stores.  The front state is read out of
+    // its slots first, and the barriers are invalidated before their memory is reused.
     constexpr int RD = (MODEL == 1) ? CPI_REC_V1_DOUBLES : CPI_REC_V2_DOUBLES;
-    T* rec = reinterpret_cast<T*>(p.out) + win * (int64_t)RD;
-    const int ri[3] = {i0, i1, i2};
-    if (c == 0) {                                                    // lane 0's frame is the original frame
-        double q[4];
-        rot_2_quat(R, q);                                            // CpiV1.h:358 (only the last one is ever consumed)
-        rec[CPI_REC_Q] = (T)q[0]; rec[CPI_REC_Q + 1] = (T)q[1]; rec[CPI_REC_Q + 2] = (T)q[2]; rec[CPI_REC_Q + 3] = (T)q[3];
-        rec[CPI_REC_DT] = (T)DT;
-    }
-    rec[CPI_REC_ALPHA + c] = (T)FST(FS_AL); rec[CPI_REC_BETA + c] = (T)FST(FS_BE);
+    constexpr int NJ = (MODEL == 1) ? 5 : 7;                         // 3x3 Jacobian blocks in the record
+    const double al = FST(FS_AL), be = FST(FS_BE);
+    double Jc[NJ][3];
 #pragma unroll
     for (int k = 0; k < 3; k++) {
-        const int r = ri[k];
-        rec[CPI_REC_R + r + 3 * c] = (T)R[3 * k];
-        if (MODEL == 1) {
-            rec[CPI_REC_JQ + r + 3 * c] = (T)FST(FS_JQ + k); rec[CPI_REC_JA + r + 3 * c] = (T)FST(FS_JA + k); rec[CPI_REC_JB + r + 3 * c] = (T)FST(FS_JB + k);
-            rec[CPI_REC_HA + r + 3 * c] = (T)FST(FS_HA + k); rec[CPI_REC_HB + r + 3 * c] = (T)FST(FS_HB + k);
+        if constexpr (MODEL == 1) {
+            Jc[0][k] = FST(FS_JQ + k); Jc[1][k] = FST(FS_JA + k); Jc[2][k] = FST(FS_JB + k); Jc[3][k] = FST(FS_HA + k); Jc[4][k] = FST(FS_HB + k);
         } else {   // read-out of Discrete_J_b (CpiV2.h:450-458): J_q = -D[theta,bg], J_a = D[p,bg], J_b = D[v,bg], H_a = D[p,ba], H_b = D[v,ba], O_a = D[p,l], O_b = D[v,l]
-            rec[CPI_REC_JQ + r + 3 * c] = (T)(-FST(FS_DTG + k)); rec[CPI_REC_JA + r + 3 * c] = (T)FST(FS_DPG + k); rec[CPI_REC_JB + r + 3 * c] = (T)FST(FS_DVG + k);
-            rec[CPI_REC_HA + r + 3 * c] = (T)FST(FS_DPA + k); rec[CPI_REC_HB + r + 3 * c] = (T)FST(FS_DVA + k);
-            rec[CPI_REC_OA + r + 3 * c] = (T)FST(FS_DPL + k); rec[CPI_REC_OB + r + 3 * c] = (T)FST(FS_DVL + k);
+            Jc[0][k] = -FST(FS_DTG + k); Jc[1][k] = FST(FS_DPG + k); Jc[2][k] = FST(FS_DVG + k); Jc[3][k] = FST(FS_DPA + k); Jc[4][k] = FST(FS_DVA + k);
+            Jc[5][k] = FST(FS_DPL + k); Jc[6][k] = FST(FS_DVL + k);
         }
     }
-    // P_meas, full 15x15: block (I,J), I,J in {theta=0, bg=1, v=2, ba=3, p=4}; every off-diagonal block is written twice
-    T* Pm = rec + CPI_REC_P;
-    auto put2 = [&](int I, int J, int r, T v) { Pm[(3 * I + r) + 15 * (3 * J + c)] = v; Pm[(3 * J + c) + 15 * (3 * I + r)] = v; };
+    if (active && c == 0) {
 #pragma unroll
-    for (int k = 0; k < 3; k++) {
-        const int r = ri[k];
-        put2(0, 0, r, (T)sTT[k]); put2(2, 2, r, (T)sVV[k]); put2(4, 4, r, (T)sPP[k]);
-        put2(0, 1, r, (T)P.TG[k]); put2(1, 2, r, (T)P.GV[k]); put2(0, 2, r, (T)P.TV[k]); put2(3, 2, r, (T)P.AV[k]);
-        put2(0, 4, r, (T)P.TP[k]); put2(1, 4, r, (T)P.GP[k]); put2(3, 4, r, (T)P.AP[k]); put2(2, 4, r, (T)P.VP[k]);
-        put2(1, 1, r, r == c ? (T)pgg : T(0)); put2(3, 3, r, r == c ? (T)paa : T(0));
-        put2(0, 3, r, T(0)); put2(1, 3, r, T(0));                    // P_theta,ba = P_bg,ba = 0 identically
+        for (int k = 0; k < TRI_NBUF; k++) mbar_inval(bar0 + 8 * k);
     }
+    __syncwarp();
+    if (active) {
+        T* rec = reinterpret_cast<T*>(smem_raw) + (size_t)wslot * RD;
+        const int ri[3] = {i0, i1, i2};
+        if (c == 0) {                                                // lane 0's frame is the original frame
+            double q[4];
+            rot_2_quat(R, q);                                        // CpiV1.h:358 (only the last one is ever consumed)
+            rec[CPI_REC_Q] = (T)q[0]; rec[CPI_REC_Q + 1] = (T)q[1]; rec[CPI_REC_Q + 2] = (T)q[2]; rec[CPI_REC_Q + 3] = (T)q[3];
+            rec[CPI_REC_DT] = (T)DT;
+        }
+        rec[CPI_REC_ALPHA + c] = (T)al; rec[CPI_REC_BETA + c] = (T)be;
+        constexpr int JOFF[7] = {CPI_REC_JQ, CPI_REC_JA, CPI_REC_JB, CPI_REC_HA, CPI_REC_HB, CPI_REC_OA, CPI_REC_OB};
+#pragma unroll
+        for (int k = 0; k < 3; k++) {
+            const int r = ri[k];
+            rec[CPI_REC_R + r + 3 * c] = (T)R[3 * k];
+#pragma unroll
+            for (int b = 0; b < NJ; b++) rec[JOFF[b] + r + 3 * c] = (T)Jc[b][k];
+        }
+        // P_meas, full 15x15: block (I,J), I,J in {theta=0, bg=1, v=2, ba=3, p=4}; every off-diagonal block is written twice
+        T* Pm = rec + CPI_REC_P;
+        auto put2 = [&](int I, int J, int r, T v) { Pm[(3 * I + r) + 15 * (3 * J + c)] = v; Pm[(3 * J + c) + 15 * (3 * I + r)] = v; };
+#pragma unroll
+        for (int k = 0; k < 3; k++) {
+            const int r = ri[k];
+            put2(0, 0, r, (T)sTT[k]); put2(2, 2, r, (T)sVV[k]); put2(4, 4, r, (T)sPP[k]);
+            put2(0, 1, r, (T)P.TG[k]); put2(1, 2, r, (T)P.GV[k]); put2(0, 2, r, (T)P.TV[k]); put2(3, 2, r, (T)P.AV[k]);
+            put2(0, 4, r, (T)P.TP[k]); put2(1, 4, r, (T)P.GP[k]); put2(3, 4, r, (T)P.AP[k]); put2(2, 4, r, (T)P.VP[k]);
+            put2(1, 1, r, r == c ? (T)pgg : T(0)); put2(3, 3, r, r == c ? (T)paa : T(0));
+            put2(0, 3, r, T(0)); put2(1, 3, r, T(0));                // P_theta,ba = P_bg,ba = 0 identically
+        }
+    }
+    __syncwarp();
+    // the warp's windows are slots 0 .. nw-1 (the one-warp CTA's first window is blockIdx.x * wpb), records win * RD in `out`;
+    // 16-byte stores when the first record is 16-byte aligned (`out` may be any slice of a caller's buffer), element stores otherwise
+    const int64_t win0 = (int64_t)blockIdx.x * p.wpb + wid * TRI_WPW;
+    const int nw = (int)min((int64_t)TRI_WPW, p.n_windows - win0);
+    const int ne = nw * RD;                                          // elements to write
+    T* dst = reinterpret_cast<T*>(p.out) + win0 * (int64_t)RD;
+    const T* tile = reinterpret_cast<const T*>(smem_raw) + (size_t)wid * TRI_WPW * RD;
+    int done = 0;
+    if (((uintptr_t)dst & 15) == 0) {
+        constexpr int EV = 16 / (int)sizeof(T);
+        const int n16 = ne / EV;
+        for (int i = lane; i < n16; i += 32) reinterpret_cast<int4*>(dst)[i] = reinterpret_cast<const int4*>(tile)[i];
+        done = n16 * EV;
+    }
+    for (int i = done + lane; i < ne; i += 32) dst[i] = tile[i];
 }
 
 #undef SLT
@@ -788,7 +822,10 @@ static cudaError_t launch_tri_one(const PreintParams& p0, int num_sms, cudaStrea
     constexpr int WPB = TriSmem<MODEL, T>::WPB;      // ten windows per one-warp CTA; the block scheduler spreads the CTAs over the SMs
     p.wpb = WPB;
     const int grid = (int)((p.n_windows + p.wpb - 1) / p.wpb);
-    kern<<<grid, TriSmem<MODEL, T>::NT, smem, st>>>(p);
+    // CPI_B200_TRI_NO_TMA (tests): stage no chunk by TMA, so that the pre-pass copies every sample from global memory -- the
+    // reference the staged stream is compared against bit for bit
+    const char* no_tma = getenv("CPI_B200_TRI_NO_TMA");
+    kern<<<grid, TriSmem<MODEL, T>::NT, smem, st>>>(p, !(no_tma && no_tma[0] == '1'));
     return cudaGetLastError();
 }
 

@@ -23,5 +23,7 @@ CPI_DEV void mbar_wait(uint32_t bar, uint32_t parity) {
 CPI_DEV void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 CPI_DEV void mbar_arrive(uint32_t bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory"); }
+// before an mbarrier's memory is reused for anything else
+CPI_DEV void mbar_inval(uint32_t bar) { asm volatile("mbarrier.inval.shared::cta.b64 [%0];" ::"r"(bar) : "memory"); }
 
 }  // namespace cpi
