@@ -5,6 +5,7 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
+#include <initializer_list>
 #include <mutex>
 #include <optional>
 #include <string>
@@ -17,16 +18,9 @@ namespace {
 
 thread_local std::string g_err;
 std::atomic<int64_t> g_launches{0};
-
-int fail(int code, const char* fmt, ...) {
-    char buf[512];
-    va_list ap; va_start(ap, fmt); vsnprintf(buf, sizeof buf, fmt, ap); va_end(ap);
-    g_err = buf;
-    return code;
-}
 }  // namespace
 namespace cpi {
-int capi_fail(int code, const char* fmt, ...) {      // same per-thread error slot, for the other translation units of the C ABI
+int capi_fail(int code, const char* fmt, ...) {      // the per-thread error slot, shared with the other translation units of the C ABI
     char buf[512];
     va_list ap; va_start(ap, fmt); vsnprintf(buf, sizeof buf, fmt, ap); va_end(ap);
     g_err = buf;
@@ -34,6 +28,7 @@ int capi_fail(int code, const char* fmt, ...) {      // same per-thread error sl
 }
 }  // namespace cpi
 namespace {
+constexpr auto fail = cpi::capi_fail;
 #define CU(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return fail(CPI_ECUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); } while (0)
 
 struct DevInfo { int sms = 0; int max_smem = 0; size_t mem = 0; bool ok = false; };
@@ -60,8 +55,8 @@ int device_info(DevInfo& d) {
 
 // grow-only scratch buffers for the *_host entry points (per process; guarded by one mutex: host calls serialise)
 struct Scratch {
-    static constexpr int NSTREAM = 8;
-    void* dev[8] = {nullptr}; size_t dev_sz[8] = {0};
+    static constexpr int NBUF = 8, NSTREAM = 8;
+    void* dev[NBUF] = {nullptr}; size_t dev_sz[NBUF] = {0};
     cudaStream_t stream = nullptr;            // copy-in / general stream
     cudaStream_t work[NSTREAM] = {nullptr};   // one per pipeline chunk (kernel + copy-out)
     cudaEvent_t ev[NSTREAM] = {nullptr};
@@ -76,7 +71,7 @@ int scratch_prepare() {
     CU(cudaGetDevice(&dev));
     if (g_scratch.device != dev) {
         // buffers belong to the device they were allocated on; drop them if the caller switched device
-        for (int i = 0; i < 8; i++) { if (g_scratch.dev[i]) cudaFree(g_scratch.dev[i]); g_scratch.dev[i] = nullptr; g_scratch.dev_sz[i] = 0; }
+        for (int i = 0; i < Scratch::NBUF; i++) { if (g_scratch.dev[i]) cudaFree(g_scratch.dev[i]); g_scratch.dev[i] = nullptr; g_scratch.dev_sz[i] = 0; }
         if (g_scratch.stream) { cudaStreamDestroy(g_scratch.stream); g_scratch.stream = nullptr; }
         for (int i = 0; i < Scratch::NSTREAM; i++) {
             if (g_scratch.work[i]) { cudaStreamDestroy(g_scratch.work[i]); g_scratch.work[i] = nullptr; }
@@ -91,17 +86,80 @@ int scratch_prepare() {
     }
     return CPI_OK;
 }
-int dev_buf(int slot, size_t bytes, void** out) {
-    if (bytes == 0) bytes = 8;
-    if (g_scratch.dev_sz[slot] < bytes) {
-        if (g_scratch.dev[slot]) CU(cudaFree(g_scratch.dev[slot]));
-        g_scratch.dev[slot] = nullptr; g_scratch.dev_sz[slot] = 0;
-        cudaError_t e = cudaMalloc(&g_scratch.dev[slot], bytes);
-        if (e != cudaSuccess) return fail(CPI_ENOMEM, "cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e));
-        g_scratch.dev_sz[slot] = bytes;
+
+// What every *_host entry point does around its kernels.  start() checks the device, takes the scratch lock and prepares the
+// scratch; buf() hands out the next free grow-only scratch buffer; copy_stream() and work_stream() hand out the streams and record
+// which ones the call used.  Those streams are drained on every exit, because async copies from / into the caller's buffers must
+// not outlive the call: finish(rc) drains them and returns rc, or the first synchronisation error when rc is CPI_OK; on an early
+// (error) return the destructor drains them.
+class HostCall {
+public:
+    DevInfo dev;
+    int start() {
+        if (int rc = device_info(dev)) return rc;
+        lk_ = std::unique_lock<std::mutex>(g_scratch_mu);
+        return scratch_prepare();
     }
-    *out = g_scratch.dev[slot];
+    int buf(size_t bytes, void** out) {
+        if (next_ == Scratch::NBUF) return fail(CPI_ENOMEM, "a host call has at most %d scratch buffers", Scratch::NBUF);
+        const int slot = next_++;
+        if (bytes == 0) bytes = 8;
+        if (g_scratch.dev_sz[slot] < bytes) {
+            if (g_scratch.dev[slot]) CU(cudaFree(g_scratch.dev[slot]));
+            g_scratch.dev[slot] = nullptr; g_scratch.dev_sz[slot] = 0;
+            cudaError_t e = cudaMalloc(&g_scratch.dev[slot], bytes);
+            if (e != cudaSuccess) return fail(CPI_ENOMEM, "cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e));
+            g_scratch.dev_sz[slot] = bytes;
+        }
+        *out = g_scratch.dev[slot];
+        return CPI_OK;
+    }
+    // a buf() filled from the caller's host buffer on the copy stream
+    int upload(const void* src, size_t bytes, void** out) {
+        if (int rc = buf(bytes, out)) return rc;
+        if (bytes > 0) CU(cudaMemcpyAsync(*out, src, bytes, cudaMemcpyHostToDevice, copy_stream()));
+        return CPI_OK;
+    }
+    cudaStream_t copy_stream() { used_ |= 1u << Scratch::NSTREAM; return g_scratch.stream; }
+    // pipeline work stream k (round robin), ordered after everything enqueued on the copy stream so far
+    int work_stream(int64_t k, cudaStream_t* out) {
+        const int si = (int)(k % Scratch::NSTREAM);
+        used_ |= 1u << si | 1u << Scratch::NSTREAM;
+        CU(cudaEventRecord(g_scratch.ev[si], g_scratch.stream));
+        CU(cudaStreamWaitEvent(g_scratch.work[si], g_scratch.ev[si], 0));
+        *out = g_scratch.work[si];
+        return CPI_OK;
+    }
+    int finish(int rc) {
+        for (int k = 0; k <= Scratch::NSTREAM; k++) {            // the work streams, then the copy stream
+            if (!(used_ >> k & 1)) continue;
+            cudaError_t e = cudaStreamSynchronize(k < Scratch::NSTREAM ? g_scratch.work[k] : g_scratch.stream);
+            if (e != cudaSuccess && rc == CPI_OK) rc = fail(CPI_ECUDA, "cudaStreamSynchronize failed: %s", cudaGetErrorString(e));
+        }
+        used_ = 0;
+        return rc;
+    }
+    ~HostCall() { finish(CPI_ECUDA); }      // an early return has already reported its error; a drain error does not replace it
+
+private:
+    std::unique_lock<std::mutex> lk_;
+    int next_ = 0;
+    unsigned used_ = 0;                     // bit k: work stream k; bit NSTREAM: the copy stream
+};
+
+// outputs (NULL ones skipped) must differ from every input and from each other
+int check_aliasing(std::initializer_list<const void*> ins, std::initializer_list<const void*> outs) {
+    for (const void* o : outs)
+        for (const void* q : ins)
+            if (o && o == q) return fail(CPI_EINVAL, "outputs must not overlap inputs");
+    for (auto a = outs.begin(); a != outs.end(); ++a)
+        for (auto b = a + 1; b != outs.end(); ++b)
+            if (*a && *a == *b) return fail(CPI_EINVAL, "outputs must not overlap each other");
     return CPI_OK;
+}
+
+bool bytes_overlap(const void* a, size_t a_bytes, const void* b, size_t b_bytes) {
+    return (const char*)a < (const char*)b + b_bytes && (const char*)b < (const char*)a + a_bytes;
 }
 
 // CPI_FLAG_DISCRETE produces model-1 records in fp64 only
@@ -245,16 +303,15 @@ int cpi_preintegrate_batch_host(int model, int dtype, int64_t n_windows, const i
     } else if (ns_uniform < 0) return fail(CPI_EINVAL, "negative count");
     const int rd = cpi_record_doubles(model);
     const size_t es = dtype == 32 ? 4 : 8;
-    DevInfo d;
-    int rc = device_info(d);
+    HostCall h;
+    int rc = h.start();
     if (rc) return rc;
-    std::lock_guard<std::mutex> lk(g_scratch_mu);
-    if ((rc = scratch_prepare())) return rc;
+    const DevInfo& d = h.dev;
     void *d_s, *d_l, *d_o, *d_off = nullptr;
-    if ((rc = dev_buf(0, (size_t)entries * CPI_SAMPLE_DOUBLES * es + 16, &d_s))) return rc;
-    if ((rc = dev_buf(1, (size_t)n_windows * CPI_LIN_DOUBLES * es, &d_l))) return rc;
-    if ((rc = dev_buf(2, (size_t)n_windows * rd * es, &d_o))) return rc;
-    if (sample_offsets && (rc = dev_buf(3, (size_t)(n_windows + 1) * 8, &d_off))) return rc;
+    if ((rc = h.buf((size_t)entries * CPI_SAMPLE_DOUBLES * es + 16, &d_s))) return rc;
+    if ((rc = h.buf((size_t)n_windows * CPI_LIN_DOUBLES * es, &d_l))) return rc;
+    if ((rc = h.buf((size_t)n_windows * rd * es, &d_o))) return rc;
+    if (sample_offsets && (rc = h.buf((size_t)(n_windows + 1) * 8, &d_off))) return rc;
 
     // Chunked pipeline: H2D of chunk k+1 runs under the kernel of chunk k, D2H of chunk k under the kernel of chunk k+1.  The
     // default kernels are one-warp CTAs, so chunk kernels of different streams co-reside on the SMs and a batch can be cut into
@@ -311,79 +368,63 @@ int cpi_preintegrate_batch_host(int model, int dtype, int64_t n_windows, const i
     const int64_t blocks_per_chunk = (head_blocks + nchunk - 1) / nchunk > 0 ? (head_blocks + nchunk - 1) / nchunk : 1;
     const auto t_start = std::chrono::steady_clock::now();
     int used = 0;                                                    // streams handed out so far (round robin)
-
-    cudaStream_t s_in = g_scratch.stream;
-    rc = CPI_OK;
-    // every error path drains the streams before returning: async copies into the caller's buffers must not outlive the call
-#define CUX(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { rc = fail(CPI_ECUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); goto drain; } } while (0)
-    if (sample_offsets) CUX(cudaMemcpyAsync(d_off, sample_offsets, (size_t)(n_windows + 1) * 8, cudaMemcpyHostToDevice, s_in));
-    for (int k = 0; k < nchunk; k++) {
-        const int64_t lo = (int64_t)k * blocks_per_chunk * wpb;
-        if (lo >= head_hi) break;
-        const int64_t hi = (lo + blocks_per_chunk * wpb < head_hi) ? lo + blocks_per_chunk * wpb : head_hi;
-        used = k + 1;
-        const int64_t e_lo = sample_offsets ? sample_offsets[lo] : lo * ent_w, e_hi = sample_offsets ? sample_offsets[hi] : hi * ent_w;
-        const int si = k % Scratch::NSTREAM;
-        cudaStream_t sk = g_scratch.work[si];
-        CUX(cudaMemcpyAsync((char*)d_l + (size_t)lo * CPI_LIN_DOUBLES * es, (const char*)lin + (size_t)lo * CPI_LIN_DOUBLES * es,
-                            (size_t)(hi - lo) * CPI_LIN_DOUBLES * es, cudaMemcpyHostToDevice, s_in));
-        if (e_hi > e_lo)
-            CUX(cudaMemcpyAsync((char*)d_s + (size_t)e_lo * CPI_SAMPLE_DOUBLES * es, (const char*)samples + (size_t)e_lo * CPI_SAMPLE_DOUBLES * es,
-                                (size_t)(e_hi - e_lo) * CPI_SAMPLE_DOUBLES * es, cudaMemcpyHostToDevice, s_in));
-        CUX(cudaEventRecord(g_scratch.ev[si], s_in));
-        CUX(cudaStreamWaitEvent(sk, g_scratch.ev[si], 0));
-        {
+    cudaStream_t s_in = h.copy_stream();
+    rc = [&]() -> int {
+        if (sample_offsets) CU(cudaMemcpyAsync(d_off, sample_offsets, (size_t)(n_windows + 1) * 8, cudaMemcpyHostToDevice, s_in));
+        for (int k = 0; k < nchunk; k++) {
+            const int64_t lo = (int64_t)k * blocks_per_chunk * wpb;
+            if (lo >= head_hi) break;
+            const int64_t hi = (lo + blocks_per_chunk * wpb < head_hi) ? lo + blocks_per_chunk * wpb : head_hi;
+            used = k + 1;
+            const int64_t e_lo = sample_offsets ? sample_offsets[lo] : lo * ent_w, e_hi = sample_offsets ? sample_offsets[hi] : hi * ent_w;
+            CU(cudaMemcpyAsync((char*)d_l + (size_t)lo * CPI_LIN_DOUBLES * es, (const char*)lin + (size_t)lo * CPI_LIN_DOUBLES * es,
+                               (size_t)(hi - lo) * CPI_LIN_DOUBLES * es, cudaMemcpyHostToDevice, s_in));
+            if (e_hi > e_lo)
+                CU(cudaMemcpyAsync((char*)d_s + (size_t)e_lo * CPI_SAMPLE_DOUBLES * es, (const char*)samples + (size_t)e_lo * CPI_SAMPLE_DOUBLES * es,
+                                   (size_t)(e_hi - e_lo) * CPI_SAMPLE_DOUBLES * es, cudaMemcpyHostToDevice, s_in));
+            cudaStream_t sk = nullptr;
+            if (int r = h.work_stream(k, &sk)) return r;
             // offsets are absolute entry indices, so CSR chunks keep the global sample base; uniform chunks shift it
             const void* s_base = sample_offsets ? d_s : (const void*)((const char*)d_s + (size_t)e_lo * CPI_SAMPLE_DOUBLES * es);
-            rc = preintegrate_dev(model, dtype, hi - lo, sample_offsets ? (const int64_t*)d_off + lo : nullptr, ns_uniform, s_base,
-                                  (const char*)d_l + (size_t)lo * CPI_LIN_DOUBLES * es, sigmas, flags, (char*)d_o + (size_t)lo * rd * es, sk, wpb);
-            if (rc) goto drain;
+            if (int r = preintegrate_dev(model, dtype, hi - lo, sample_offsets ? (const int64_t*)d_off + lo : nullptr, ns_uniform, s_base,
+                                         (const char*)d_l + (size_t)lo * CPI_LIN_DOUBLES * es, sigmas, flags, (char*)d_o + (size_t)lo * rd * es, sk, wpb))
+                return r;
+            CU(cudaMemcpyAsync((char*)out_records + (size_t)lo * rd * es, (const char*)d_o + (size_t)lo * rd * es, (size_t)(hi - lo) * rd * es,
+                               cudaMemcpyDeviceToHost, sk));
         }
-        CUX(cudaMemcpyAsync((char*)out_records + (size_t)lo * rd * es, (const char*)d_o + (size_t)lo * rd * es, (size_t)(hi - lo) * rd * es,
-                            cudaMemcpyDeviceToHost, sk));
-    }
-    if (wave && head_hi < n_windows) {
-        const size_t sb = (size_t)CPI_SAMPLE_DOUBLES * es;            // bytes per sample
-        const int64_t wblocks = blocks - head_blocks;
-        const int64_t bpg = (wblocks + wave_G - 1) / wave_G;          // blocks per group
-        const int64_t G = (wblocks + bpg - 1) / bpg;
-        const int64_t seg_len = (ns_uniform + wave_S - 1) / wave_S;
-        const int64_t S = (ns_uniform + seg_len - 1) / seg_len;
-        for (int64_t t = 0; t < G + S - 1; t++) {
-            for (int64_t g = t - S + 1 > 0 ? t - S + 1 : 0; g <= t && g < G; g++) {      // oldest group (latest segment) first
-                const int64_t sidx = t - g, s0 = sidx * seg_len;
-                const int64_t len = s0 + seg_len <= ns_uniform ? seg_len : ns_uniform - s0;
-                const int64_t lo = head_hi + g * bpg * wpb, hi = (lo + bpg * wpb < n_windows) ? lo + bpg * wpb : n_windows, ng = hi - lo;
-                const int si = (int)((used + g) % Scratch::NSTREAM);
-                cudaStream_t sk = g_scratch.work[si];
-                char* d_lg = (char*)d_l + (size_t)lo * CPI_LIN_DOUBLES * es;
-                char* d_og = (char*)d_o + (size_t)lo * rd * es;
-                if (sidx == 0)
-                    CUX(cudaMemcpyAsync(d_lg, (const char*)lin + (size_t)lo * CPI_LIN_DOUBLES * es, (size_t)ng * CPI_LIN_DOUBLES * es, cudaMemcpyHostToDevice, s_in));
-                // the tiles of a group are compact ([window][len]) and together fill the group's share of the device sample buffer
-                char* d_seg = (char*)d_s + ((size_t)lo * ns_uniform + (size_t)ng * s0) * sb;
-                CUX(cudaMemcpy2DAsync(d_seg, (size_t)len * sb, (const char*)samples + ((size_t)lo * ns_uniform + (size_t)s0) * sb, (size_t)ns_uniform * sb,
-                                      (size_t)len * sb, (size_t)ng, cudaMemcpyHostToDevice, s_in));
-                CUX(cudaEventRecord(g_scratch.ev[si], s_in));
-                CUX(cudaStreamWaitEvent(sk, g_scratch.ev[si], 0));
-                rc = preintegrate_dev(model, dtype, ng, nullptr, len, d_seg, d_lg, sigmas, flags, d_og, sk, wpb, sidx > 0 ? d_og : nullptr);
-                if (rc) goto drain;
-                if (sidx == S - 1)
-                    CUX(cudaMemcpyAsync((char*)out_records + (size_t)lo * rd * es, d_og, (size_t)ng * rd * es, cudaMemcpyDeviceToHost, sk));
+        if (wave && head_hi < n_windows) {
+            const size_t sb = (size_t)CPI_SAMPLE_DOUBLES * es;            // bytes per sample
+            const int64_t wblocks = blocks - head_blocks;
+            const int64_t bpg = (wblocks + wave_G - 1) / wave_G;          // blocks per group
+            const int64_t G = (wblocks + bpg - 1) / bpg;
+            const int64_t seg_len = (ns_uniform + wave_S - 1) / wave_S;
+            const int64_t S = (ns_uniform + seg_len - 1) / seg_len;
+            for (int64_t t = 0; t < G + S - 1; t++) {
+                for (int64_t g = t - S + 1 > 0 ? t - S + 1 : 0; g <= t && g < G; g++) {      // oldest group (latest segment) first
+                    const int64_t sidx = t - g, s0 = sidx * seg_len;
+                    const int64_t len = s0 + seg_len <= ns_uniform ? seg_len : ns_uniform - s0;
+                    const int64_t lo = head_hi + g * bpg * wpb, hi = (lo + bpg * wpb < n_windows) ? lo + bpg * wpb : n_windows, ng = hi - lo;
+                    char* d_lg = (char*)d_l + (size_t)lo * CPI_LIN_DOUBLES * es;
+                    char* d_og = (char*)d_o + (size_t)lo * rd * es;
+                    if (sidx == 0)
+                        CU(cudaMemcpyAsync(d_lg, (const char*)lin + (size_t)lo * CPI_LIN_DOUBLES * es, (size_t)ng * CPI_LIN_DOUBLES * es, cudaMemcpyHostToDevice, s_in));
+                    // the tiles of a group are compact ([window][len]) and together fill the group's share of the device sample buffer
+                    char* d_seg = (char*)d_s + ((size_t)lo * ns_uniform + (size_t)ng * s0) * sb;
+                    CU(cudaMemcpy2DAsync(d_seg, (size_t)len * sb, (const char*)samples + ((size_t)lo * ns_uniform + (size_t)s0) * sb, (size_t)ns_uniform * sb,
+                                         (size_t)len * sb, (size_t)ng, cudaMemcpyHostToDevice, s_in));
+                    cudaStream_t sk = nullptr;
+                    if (int r = h.work_stream(used + g, &sk)) return r;
+                    if (int r = preintegrate_dev(model, dtype, ng, nullptr, len, d_seg, d_lg, sigmas, flags, d_og, sk, wpb, sidx > 0 ? d_og : nullptr))
+                        return r;
+                    if (sidx == S - 1)
+                        CU(cudaMemcpyAsync((char*)out_records + (size_t)lo * rd * es, d_og, (size_t)ng * rd * es, cudaMemcpyDeviceToHost, sk));
+                }
             }
         }
-    }
-drain:
-#undef CUX
+        return CPI_OK;
+    }();
     g_host_submit_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_start).count();
-    for (int k = 0; k < Scratch::NSTREAM; k++) {
-        cudaError_t e_ = cudaStreamSynchronize(g_scratch.work[k]);
-        if (e_ != cudaSuccess && rc == CPI_OK) rc = fail(CPI_ECUDA, "cudaStreamSynchronize failed: %s", cudaGetErrorString(e_));
-    }
-    {
-        cudaError_t e_ = cudaStreamSynchronize(s_in);
-        if (e_ != cudaSuccess && rc == CPI_OK) rc = fail(CPI_ECUDA, "cudaStreamSynchronize failed: %s", cudaGetErrorString(e_));
-    }
+    rc = h.finish(rc);
     g_host_total_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_start).count();
     return rc;
 }
@@ -434,34 +475,26 @@ int cpi_imu_factor_eval_batch_host(int model, int64_t n_factors, int64_t n_state
             if (idx_i[f] < 0 || idx_i[f] >= n_states || idx_j[f] < 0 || idx_j[f] >= n_states)
                 return fail(CPI_EINVAL, "factor %lld: state index out of range [0, %lld)", (long long)f, (long long)n_states);
     const int rd = cpi_record_doubles(model);
-    std::lock_guard<std::mutex> lk(g_scratch_mu);
-    int rc = scratch_prepare();
+    HostCall h;
+    int rc = h.start();
     if (rc) return rc;
-    cudaStream_t st = g_scratch.stream;
     void *d_x, *d_r, *d_l, *d_e, *d_h1 = nullptr, *d_h2 = nullptr, *d_i = nullptr, *d_j = nullptr;
-    if ((rc = dev_buf(0, (size_t)n_states * CPI_STATE_DOUBLES * 8, &d_x))) return rc;
-    if ((rc = dev_buf(1, (size_t)n_factors * CPI_LIN_DOUBLES * 8, &d_l))) return rc;
-    if ((rc = dev_buf(2, (size_t)n_factors * rd * 8, &d_r))) return rc;
-    if ((rc = dev_buf(4, (size_t)n_factors * 15 * 8, &d_e))) return rc;
-    if (H1 && (rc = dev_buf(5, (size_t)n_factors * 225 * 8, &d_h1))) return rc;
-    if (H2 && (rc = dev_buf(6, (size_t)n_factors * 225 * 8, &d_h2))) return rc;
-    if (idx_i) {
-        if ((rc = dev_buf(3, (size_t)n_factors * 8, &d_i))) return rc;
-        if ((rc = dev_buf(7, (size_t)n_factors * 8, &d_j))) return rc;
-        CU(cudaMemcpyAsync(d_i, idx_i, (size_t)n_factors * 8, cudaMemcpyHostToDevice, st));
-        CU(cudaMemcpyAsync(d_j, idx_j, (size_t)n_factors * 8, cudaMemcpyHostToDevice, st));
-    }
-    CU(cudaMemcpyAsync(d_x, states, (size_t)n_states * CPI_STATE_DOUBLES * 8, cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(d_l, lin, (size_t)n_factors * CPI_LIN_DOUBLES * 8, cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(d_r, records, (size_t)n_factors * rd * 8, cudaMemcpyHostToDevice, st));
+    if (idx_i && (rc = h.upload(idx_i, (size_t)n_factors * 8, &d_i))) return rc;
+    if (idx_i && (rc = h.upload(idx_j, (size_t)n_factors * 8, &d_j))) return rc;
+    if ((rc = h.upload(states, (size_t)n_states * CPI_STATE_DOUBLES * 8, &d_x))) return rc;
+    if ((rc = h.upload(lin, (size_t)n_factors * CPI_LIN_DOUBLES * 8, &d_l))) return rc;
+    if ((rc = h.upload(records, (size_t)n_factors * rd * 8, &d_r))) return rc;
+    if ((rc = h.buf((size_t)n_factors * 15 * 8, &d_e))) return rc;
+    if (H1 && (rc = h.buf((size_t)n_factors * 225 * 8, &d_h1))) return rc;
+    if (H2 && (rc = h.buf((size_t)n_factors * 225 * 8, &d_h2))) return rc;
+    cudaStream_t st = h.copy_stream();
     rc = cpi_imu_factor_eval_batch(model, n_factors, (const double*)d_x, (const int64_t*)d_i, (const int64_t*)d_j, (const double*)d_r,
                                    (const double*)d_l, (double*)d_e, (double*)d_h1, (double*)d_h2, st);
     if (rc) return rc;
     CU(cudaMemcpyAsync(e, d_e, (size_t)n_factors * 15 * 8, cudaMemcpyDeviceToHost, st));
     if (H1) CU(cudaMemcpyAsync(H1, d_h1, (size_t)n_factors * 225 * 8, cudaMemcpyDeviceToHost, st));
     if (H2) CU(cudaMemcpyAsync(H2, d_h2, (size_t)n_factors * 225 * 8, cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    return CPI_OK;
+    return h.finish(CPI_OK);
 }
 
 int cpi_imu_factor_hessian_batch(int model, int64_t n_factors, const double* records, const double* e, const double* H1, const double* H2,
@@ -808,13 +841,11 @@ int cpi_merge_records(int model, int dtype, int64_t n_groups, const int64_t* gro
     if (rc || n_groups == 0) return rc;
     if (!out_records) return fail(CPI_EINVAL, "null pointer argument (out_records)");
     if ((!records || !lin) && (group_offsets || group_uniform > 0)) return fail(CPI_EINVAL, "null pointer argument (records / lin)");
-    if (out_records == records) return fail(CPI_EINVAL, "out_records must not overlap records");
-    if (!group_offsets && records) {           // the uniform layout's extent is known: check the whole range
-        const size_t es = dtype == 32 ? 4 : 8, rb = (size_t)CPI_REC_V1_DOUBLES * es;
-        const char *r0 = (const char*)records, *r1 = r0 + (size_t)n_groups * group_uniform * rb;
-        const char *o0 = (const char*)out_records, *o1 = o0 + (size_t)n_groups * rb;
-        if (o0 < r1 && r0 < o1) return fail(CPI_EINVAL, "out_records must not overlap records");
-    }
+    const size_t rb = (size_t)CPI_REC_V1_DOUBLES * (dtype == 32 ? 4 : 8);
+    // equal pointers always overlap; the uniform layout's extent is known, so check its whole range
+    if (out_records == records ||
+        (!group_offsets && records && bytes_overlap(records, (size_t)n_groups * group_uniform * rb, out_records, (size_t)n_groups * rb)))
+        return fail(CPI_EINVAL, "out_records must not overlap records");
     DevInfo d;
     if ((rc = device_info(d))) return rc;
     CU(cpi::merge_launch(dtype, n_groups, group_offsets, group_uniform, records, lin, out_records, (cudaStream_t)stream));
@@ -832,34 +863,18 @@ int cpi_merge_records_host(int model, int dtype, int64_t n_groups, const int64_t
     if ((rc = host_layout_check(dtype, n_groups, group_offsets, group_uniform, &n_rec))) return rc;
     if (n_rec > 0 && (!records || !lin)) return fail(CPI_EINVAL, "null pointer argument (records / lin)");
     if (n_rec > 0 && out_records == records) return fail(CPI_EINVAL, "out_records must not overlap records");
-    DevInfo d;
-    if ((rc = device_info(d))) return rc;
-    std::lock_guard<std::mutex> lk(g_scratch_mu);
-    if ((rc = scratch_prepare())) return rc;
+    HostCall h;
+    if ((rc = h.start())) return rc;
     const size_t rb = (size_t)CPI_REC_V1_DOUBLES * es;
     void *d_r, *d_l, *d_o, *d_off = nullptr;
-    if ((rc = dev_buf(0, (size_t)n_rec * rb, &d_r))) return rc;
-    if ((rc = dev_buf(1, (size_t)n_rec * CPI_LIN_DOUBLES * es, &d_l))) return rc;
-    if ((rc = dev_buf(2, (size_t)n_groups * rb, &d_o))) return rc;
-    if (group_offsets && (rc = dev_buf(3, (size_t)(n_groups + 1) * 8, &d_off))) return rc;
-    cudaStream_t st = g_scratch.stream;
-    // every error path drains the stream before returning: async copies from / into the caller's buffers must not outlive the call
-#define CUX(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { rc = fail(CPI_ECUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); goto drain; } } while (0)
-    if (group_offsets) CUX(cudaMemcpyAsync(d_off, group_offsets, (size_t)(n_groups + 1) * 8, cudaMemcpyHostToDevice, st));
-    if (n_rec > 0) {
-        CUX(cudaMemcpyAsync(d_r, records, (size_t)n_rec * rb, cudaMemcpyHostToDevice, st));
-        CUX(cudaMemcpyAsync(d_l, lin, (size_t)n_rec * CPI_LIN_DOUBLES * es, cudaMemcpyHostToDevice, st));
-    }
-    rc = cpi_merge_records(model, dtype, n_groups, (const int64_t*)d_off, group_uniform, d_r, d_l, d_o, st);
-    if (rc) goto drain;
-    CUX(cudaMemcpyAsync(out_records, d_o, (size_t)n_groups * rb, cudaMemcpyDeviceToHost, st));
-drain:
-#undef CUX
-    {
-        cudaError_t e_ = cudaStreamSynchronize(st);
-        if (e_ != cudaSuccess && rc == CPI_OK) rc = fail(CPI_ECUDA, "cudaStreamSynchronize failed: %s", cudaGetErrorString(e_));
-    }
-    return rc;
+    if (group_offsets && (rc = h.upload(group_offsets, (size_t)(n_groups + 1) * 8, &d_off))) return rc;
+    if ((rc = h.upload(records, (size_t)n_rec * rb, &d_r))) return rc;
+    if ((rc = h.upload(lin, (size_t)n_rec * CPI_LIN_DOUBLES * es, &d_l))) return rc;
+    if ((rc = h.buf((size_t)n_groups * rb, &d_o))) return rc;
+    cudaStream_t st = h.copy_stream();
+    if ((rc = cpi_merge_records(model, dtype, n_groups, (const int64_t*)d_off, group_uniform, d_r, d_l, d_o, st))) return rc;
+    CU(cudaMemcpyAsync(out_records, d_o, (size_t)n_groups * rb, cudaMemcpyDeviceToHost, st));
+    return h.finish(CPI_OK);
 }
 
 int64_t cpi_scan_records_workspace(int64_t n_groups, int64_t n_records) {
@@ -874,13 +889,10 @@ int cpi_scan_records(int model, int dtype, int64_t n_groups, const int64_t* grou
     if (!out_records) return fail(CPI_EINVAL, "null pointer argument (out_records)");
     if (!workspace) return fail(CPI_EINVAL, "null pointer argument (workspace: cpi_scan_records_workspace bytes)");
     if ((!records || !lin) && (group_offsets || group_uniform > 0)) return fail(CPI_EINVAL, "null pointer argument (records / lin)");
-    if (out_records == records) return fail(CPI_EINVAL, "out_records must not overlap records");
-    const size_t es = dtype == 32 ? 4 : 8, rb = (size_t)CPI_REC_V1_DOUBLES * es;
-    if (!group_offsets && records) {           // the uniform layout's extent is known: check the whole range
-        const size_t bytes = (size_t)n_groups * group_uniform * rb;
-        const char *r0 = (const char*)records, *r1 = r0 + bytes, *o0 = (const char*)out_records, *o1 = o0 + bytes;
-        if (o0 < r1 && r0 < o1) return fail(CPI_EINVAL, "out_records must not overlap records");
-    }
+    const size_t rb = (size_t)CPI_REC_V1_DOUBLES * (dtype == 32 ? 4 : 8), bytes = (size_t)n_groups * group_uniform * rb;
+    // equal pointers always overlap; the uniform layout's extent is known, so check its whole range
+    if (out_records == records || (!group_offsets && records && bytes_overlap(records, bytes, out_records, bytes)))
+        return fail(CPI_EINVAL, "out_records must not overlap records");
     DevInfo d;
     if ((rc = device_info(d))) return rc;
     // device offsets are not read here: the records of one call fit in device memory, which bounds their count
@@ -905,40 +917,27 @@ int cpi_scan_records_host(int model, int dtype, int64_t n_groups, const int64_t*
     if (n_rec > 0 && (!records || !lin)) return fail(CPI_EINVAL, "null pointer argument (records / lin)");
     if (n_rec > 0 && out_records == records) return fail(CPI_EINVAL, "out_records must not overlap records");
     if (n_rec == 0) return CPI_OK;             // only empty groups: nothing to write
-    DevInfo d;
-    if ((rc = device_info(d))) return rc;
-    std::lock_guard<std::mutex> lk(g_scratch_mu);
-    if ((rc = scratch_prepare())) return rc;
     const size_t rb = (size_t)CPI_REC_V1_DOUBLES * es, lb = (size_t)CPI_LIN_DOUBLES * es;
-    // the device copies start at record b0; the offsets are shifted to match
-    void *d_r, *d_l, *d_o, *d_ws, *d_off = nullptr;
-    if ((rc = dev_buf(0, (size_t)n_rec * rb, &d_r))) return rc;
-    if ((rc = dev_buf(1, (size_t)n_rec * lb, &d_l))) return rc;
-    if ((rc = dev_buf(2, (size_t)n_rec * rb, &d_o))) return rc;
-    if ((rc = dev_buf(3, (size_t)cpi::scan_workspace_bytes(n_rec), &d_ws))) return rc;
+    // the device copies start at record b0; the offsets are shifted to match (declared before the host call, which drains the copy
+    // out of it before it is freed)
     std::string shifted;
     if (group_offsets) {
-        if ((rc = dev_buf(4, (size_t)(n_groups + 1) * 8, &d_off))) return rc;
         shifted.resize((size_t)(n_groups + 1) * 8);
         int64_t* so = (int64_t*)&shifted[0];
         for (int64_t g = 0; g <= n_groups; g++) so[g] = group_offsets[g] - b0;
     }
-    cudaStream_t st = g_scratch.stream;
-    // every error path drains the stream before returning: async copies from / into the caller's buffers must not outlive the call
-#define CUX(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { rc = fail(CPI_ECUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); goto drain; } } while (0)
-    if (group_offsets) CUX(cudaMemcpyAsync(d_off, shifted.data(), (size_t)(n_groups + 1) * 8, cudaMemcpyHostToDevice, st));
-    CUX(cudaMemcpyAsync(d_r, (const char*)records + (size_t)b0 * rb, (size_t)n_rec * rb, cudaMemcpyHostToDevice, st));
-    CUX(cudaMemcpyAsync(d_l, (const char*)lin + (size_t)b0 * lb, (size_t)n_rec * lb, cudaMemcpyHostToDevice, st));
-    rc = cpi_scan_records(model, dtype, n_groups, (const int64_t*)d_off, group_uniform, d_r, d_l, d_o, d_ws, st);
-    if (rc) goto drain;
-    CUX(cudaMemcpyAsync((char*)out_records + (size_t)b0 * rb, d_o, (size_t)n_rec * rb, cudaMemcpyDeviceToHost, st));
-drain:
-#undef CUX
-    {
-        cudaError_t e_ = cudaStreamSynchronize(st);
-        if (e_ != cudaSuccess && rc == CPI_OK) rc = fail(CPI_ECUDA, "cudaStreamSynchronize failed: %s", cudaGetErrorString(e_));
-    }
-    return rc;
+    HostCall h;
+    if ((rc = h.start())) return rc;
+    void *d_r, *d_l, *d_o, *d_ws, *d_off = nullptr;
+    if (group_offsets && (rc = h.upload(shifted.data(), (size_t)(n_groups + 1) * 8, &d_off))) return rc;
+    if ((rc = h.upload((const char*)records + (size_t)b0 * rb, (size_t)n_rec * rb, &d_r))) return rc;
+    if ((rc = h.upload((const char*)lin + (size_t)b0 * lb, (size_t)n_rec * lb, &d_l))) return rc;
+    if ((rc = h.buf((size_t)n_rec * rb, &d_o))) return rc;
+    if ((rc = h.buf((size_t)cpi::scan_workspace_bytes(n_rec), &d_ws))) return rc;
+    cudaStream_t st = h.copy_stream();
+    if ((rc = cpi_scan_records(model, dtype, n_groups, (const int64_t*)d_off, group_uniform, d_r, d_l, d_o, d_ws, st))) return rc;
+    CU(cudaMemcpyAsync((char*)out_records + (size_t)b0 * rb, d_o, (size_t)n_rec * rb, cudaMemcpyDeviceToHost, st));
+    return h.finish(CPI_OK);
 }
 
 }  // extern "C"
@@ -951,13 +950,7 @@ int propagate_check(int model, int64_t n, const double* states_k, const double* 
     if (n < 0) return fail(CPI_EINVAL, "negative count");
     if (n == 0) return CPI_OK;
     if (!states_k || !cov_k || !records || !lin || !states_k1 || !cov_k1) return fail(CPI_EINVAL, "null pointer argument");
-    const void* ins[4] = {states_k, cov_k, records, lin};
-    const void* outs[3] = {states_k1, cov_k1, cross};
-    for (const void* o : outs)
-        for (const void* q : ins)
-            if (o && o == q) return fail(CPI_EINVAL, "outputs must not overlap inputs");
-    if (states_k1 == cov_k1 || (cross && (cross == states_k1 || cross == cov_k1))) return fail(CPI_EINVAL, "outputs must not overlap each other");
-    return CPI_OK;
+    return check_aliasing({states_k, cov_k, records, lin}, {states_k1, cov_k1, cross});
 }
 }  // namespace
 
@@ -987,40 +980,25 @@ int cpi_propagate_batch_host(int model, int64_t n, int64_t n_anchors, const doub
                 return fail(CPI_EINVAL, "window %lld: anchor index %lld out of range [0, %lld)", (long long)i, (long long)anchor[i], (long long)n_anchors);
     const int64_t na = anchor ? n_anchors : n;           // anchor entries the windows read
     const size_t rb = (size_t)cpi_record_doubles(model) * 8;
-    DevInfo d;
-    if ((rc = device_info(d))) return rc;
-    std::lock_guard<std::mutex> lk(g_scratch_mu);
-    if ((rc = scratch_prepare())) return rc;
+    HostCall h;
+    if ((rc = h.start())) return rc;
     void *d_x, *d_c, *d_r, *d_l, *d_a = nullptr, *d_x1, *d_c1, *d_cr = nullptr;
-    if ((rc = dev_buf(0, (size_t)na * CPI_STATE_DOUBLES * 8, &d_x))) return rc;
-    if ((rc = dev_buf(1, (size_t)na * 225 * 8, &d_c))) return rc;
-    if ((rc = dev_buf(2, (size_t)n * rb, &d_r))) return rc;
-    if ((rc = dev_buf(3, (size_t)n * CPI_LIN_DOUBLES * 8, &d_l))) return rc;
-    if (anchor && (rc = dev_buf(4, (size_t)n * 8, &d_a))) return rc;
-    if ((rc = dev_buf(5, (size_t)n * CPI_STATE_DOUBLES * 8, &d_x1))) return rc;
-    if ((rc = dev_buf(6, (size_t)n * 225 * 8, &d_c1))) return rc;
-    if (cross && (rc = dev_buf(7, (size_t)n * 225 * 8, &d_cr))) return rc;
-    cudaStream_t st = g_scratch.stream;
-    // every error path drains the stream before returning: async copies from / into the caller's buffers must not outlive the call
-#define CUX(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { rc = fail(CPI_ECUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); goto drain; } } while (0)
-    CUX(cudaMemcpyAsync(d_x, states_k, (size_t)na * CPI_STATE_DOUBLES * 8, cudaMemcpyHostToDevice, st));
-    CUX(cudaMemcpyAsync(d_c, cov_k, (size_t)na * 225 * 8, cudaMemcpyHostToDevice, st));
-    CUX(cudaMemcpyAsync(d_r, records, (size_t)n * rb, cudaMemcpyHostToDevice, st));
-    CUX(cudaMemcpyAsync(d_l, lin, (size_t)n * CPI_LIN_DOUBLES * 8, cudaMemcpyHostToDevice, st));
-    if (anchor) CUX(cudaMemcpyAsync(d_a, anchor, (size_t)n * 8, cudaMemcpyHostToDevice, st));
+    if ((rc = h.upload(states_k, (size_t)na * CPI_STATE_DOUBLES * 8, &d_x))) return rc;
+    if ((rc = h.upload(cov_k, (size_t)na * 225 * 8, &d_c))) return rc;
+    if ((rc = h.upload(records, (size_t)n * rb, &d_r))) return rc;
+    if ((rc = h.upload(lin, (size_t)n * CPI_LIN_DOUBLES * 8, &d_l))) return rc;
+    if (anchor && (rc = h.upload(anchor, (size_t)n * 8, &d_a))) return rc;
+    if ((rc = h.buf((size_t)n * CPI_STATE_DOUBLES * 8, &d_x1))) return rc;
+    if ((rc = h.buf((size_t)n * 225 * 8, &d_c1))) return rc;
+    if (cross && (rc = h.buf((size_t)n * 225 * 8, &d_cr))) return rc;
+    cudaStream_t st = h.copy_stream();
     rc = cpi_propagate_batch(model, n, (const double*)d_x, (const double*)d_c, (const int64_t*)d_a, (const double*)d_r, (const double*)d_l,
                              (double*)d_x1, (double*)d_c1, (double*)d_cr, st);
-    if (rc) goto drain;
-    CUX(cudaMemcpyAsync(states_k1, d_x1, (size_t)n * CPI_STATE_DOUBLES * 8, cudaMemcpyDeviceToHost, st));
-    CUX(cudaMemcpyAsync(cov_k1, d_c1, (size_t)n * 225 * 8, cudaMemcpyDeviceToHost, st));
-    if (cross) CUX(cudaMemcpyAsync(cross, d_cr, (size_t)n * 225 * 8, cudaMemcpyDeviceToHost, st));
-drain:
-#undef CUX
-    {
-        cudaError_t e_ = cudaStreamSynchronize(st);
-        if (e_ != cudaSuccess && rc == CPI_OK) rc = fail(CPI_ECUDA, "cudaStreamSynchronize failed: %s", cudaGetErrorString(e_));
-    }
-    return rc;
+    if (rc) return rc;
+    CU(cudaMemcpyAsync(states_k1, d_x1, (size_t)n * CPI_STATE_DOUBLES * 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(cov_k1, d_c1, (size_t)n * 225 * 8, cudaMemcpyDeviceToHost, st));
+    if (cross) CU(cudaMemcpyAsync(cross, d_cr, (size_t)n * 225 * 8, cudaMemcpyDeviceToHost, st));
+    return h.finish(CPI_OK);
 }
 
 int cpi_retract_batch(int64_t n, const double* states, const double* xi, double* states_out, void* stream) {
@@ -1040,17 +1018,10 @@ int cpi_state_update_batch(int64_t n, const double* states, const double* cov, c
     if (n < 0) return fail(CPI_EINVAL, "negative count");
     if (n == 0) return CPI_OK;
     if (!states || !cov || !meas_info || !meas_states || !states_out || !cov_out) return fail(CPI_EINVAL, "null pointer argument");
-    const void* ins[5] = {states, cov, meas_info, meas_states, gate};
-    const void* outs[4] = {states_out, cov_out, nis, applied};
-    for (const void* o : outs)
-        for (const void* q : ins)
-            if (o && o == q) return fail(CPI_EINVAL, "outputs must not overlap inputs");
-    for (int a = 0; a < 4; a++)
-        for (int b = a + 1; b < 4; b++)
-            if (outs[a] && outs[a] == outs[b]) return fail(CPI_EINVAL, "outputs must not overlap each other");
-    DevInfo d;
-    int rc = device_info(d);
+    int rc = check_aliasing({states, cov, meas_info, meas_states, gate}, {states_out, cov_out, nis, applied});
     if (rc) return rc;
+    DevInfo d;
+    if ((rc = device_info(d))) return rc;
     CU(cpi::state_update_launch(n, states, cov, meas_info, meas_states, gate, states_out, cov_out, nis, applied, (cudaStream_t)stream));
     g_launches += 1;
     return CPI_OK;
@@ -1063,17 +1034,10 @@ int cpi_state_update_measurements_batch(int64_t n, const double* states, const d
     if (n == 0) return CPI_OK;
     if (!states || !cov || !meas_offsets || !kind || !z || !sqrt_info || !aux || !states_out || !cov_out)
         return fail(CPI_EINVAL, "null pointer argument");
-    const void* ins[8] = {states, cov, meas_offsets, kind, z, sqrt_info, aux, gate};
-    const void* outs[4] = {states_out, cov_out, nis, applied};
-    for (const void* o : outs)
-        for (const void* q : ins)
-            if (o && o == q) return fail(CPI_EINVAL, "outputs must not overlap inputs");
-    for (int a = 0; a < 4; a++)
-        for (int b = a + 1; b < 4; b++)
-            if (outs[a] && outs[a] == outs[b]) return fail(CPI_EINVAL, "outputs must not overlap each other");
-    DevInfo d;
-    int rc = device_info(d);
+    int rc = check_aliasing({states, cov, meas_offsets, kind, z, sqrt_info, aux, gate}, {states_out, cov_out, nis, applied});
     if (rc) return rc;
+    DevInfo d;
+    if ((rc = device_info(d))) return rc;
     CU(cpi::state_update_meas_launch(n, states, cov, meas_offsets, kind, z, sqrt_info, aux, gate, states_out, cov_out, nis, applied,
                                      (cudaStream_t)stream));
     g_launches += 1;
@@ -1092,17 +1056,11 @@ int cpi_state_update_measurements_iterated_batch(int64_t n, const double* states
     if (n == 0) return CPI_OK;
     if (!states || !cov || !meas_offsets || !kind || !z || !sqrt_info || !aux || !states_out || !cov_out)
         return fail(CPI_EINVAL, "null pointer argument");
-    const void* ins[10] = {states, cov, meas_offsets, kind, z, sqrt_info, aux, loss, loss_k, gate};
-    const void* outs[5] = {states_out, cov_out, nis, status, iterations};
-    for (const void* o : outs)
-        for (const void* q : ins)
-            if (o && o == q) return fail(CPI_EINVAL, "outputs must not overlap inputs");
-    for (int a = 0; a < 5; a++)
-        for (int b = a + 1; b < 5; b++)
-            if (outs[a] && outs[a] == outs[b]) return fail(CPI_EINVAL, "outputs must not overlap each other");
-    DevInfo d;
-    int rc = device_info(d);
+    int rc = check_aliasing({states, cov, meas_offsets, kind, z, sqrt_info, aux, loss, loss_k, gate},
+                            {states_out, cov_out, nis, status, iterations});
     if (rc) return rc;
+    DevInfo d;
+    if ((rc = device_info(d))) return rc;
     CU(cpi::state_update_meas_iter_launch(n, states, cov, meas_offsets, kind, z, sqrt_info, aux, loss, loss_k, gate, max_iterations, tol,
                                           states_out, cov_out, nis, status, iterations, (cudaStream_t)stream));
     g_launches += 1;
@@ -1117,13 +1075,7 @@ int cpi_rts_smooth_batch(int64_t n_runs, const int64_t* run_offsets, int64_t run
     const bool any_step = n_states > n_runs;                       // a transition exists
     if (!states || !cov || !states_out || !cov_out || (any_step && (!pred_states || !pred_cov || !cross)))
         return fail(CPI_EINVAL, "null pointer argument");
-    const void* ins[6] = {run_offsets, states, cov, pred_states, pred_cov, cross};
-    const void* outs[3] = {states_out, cov_out, cross_out};
-    for (const void* o : outs)
-        for (const void* q : ins)
-            if (o && o == q) return fail(CPI_EINVAL, "outputs must not overlap inputs");
-    if (states_out == cov_out || (cross_out && (cross_out == states_out || cross_out == cov_out)))
-        return fail(CPI_EINVAL, "outputs must not overlap each other");
+    if ((rc = check_aliasing({run_offsets, states, cov, pred_states, pred_cov, cross}, {states_out, cov_out, cross_out}))) return rc;
     DevInfo d;
     if ((rc = device_info(d))) return rc;
     CU(cpi::rts_smooth_launch(n_runs, run_offsets, run_offsets ? 0 : run_uniform, states, cov, pred_states, pred_cov, cross, states_out, cov_out,
@@ -1148,14 +1100,7 @@ int cpi_rts_smooth_scan_batch(int64_t n_runs, const int64_t* run_offsets, int64_
     if (!states || !cov || !states_out || !cov_out || (any_step && (!pred_states || !pred_cov || !cross)))
         return fail(CPI_EINVAL, "null pointer argument");
     if (any_step && !workspace) return fail(CPI_EINVAL, "null pointer argument (workspace: cpi_rts_smooth_scan_workspace bytes)");
-    const void* ins[6] = {run_offsets, states, cov, pred_states, pred_cov, cross};
-    const void* outs[4] = {states_out, cov_out, cross_out, workspace};
-    for (const void* o : outs)
-        for (const void* q : ins)
-            if (o && o == q) return fail(CPI_EINVAL, "outputs must not overlap inputs");
-    for (int i = 0; i < 4; i++)
-        for (int j = i + 1; j < 4; j++)
-            if (outs[i] && outs[i] == outs[j]) return fail(CPI_EINVAL, "outputs must not overlap each other");
+    if ((rc = check_aliasing({run_offsets, states, cov, pred_states, pred_cov, cross}, {states_out, cov_out, cross_out, workspace}))) return rc;
     DevInfo d;
     if ((rc = device_info(d))) return rc;
     int launches = 0;
@@ -1173,15 +1118,10 @@ int cpi_imu_measurements_linearize(int64_t n, const int32_t* kind, const int64_t
     if (n > ((int64_t)1 << 31)) return fail(CPI_EINVAL, "too many measurements (%lld; at most 2^31 per call)", (long long)n);
     if (!kind || !state_idx || !states || !z || !sqrt_info || !aux || !f) return fail(CPI_EINVAL, "null pointer argument");
     if ((info == nullptr) != (rhs == nullptr)) return fail(CPI_EINVAL, "info and rhs must both be given or both be null");
-    const void* ins[6] = {kind, state_idx, states, z, sqrt_info, aux};
-    const void* outs[3] = {info, rhs, f};
-    for (const void* o : outs)
-        for (const void* q : ins)
-            if (o && o == q) return fail(CPI_EINVAL, "outputs must not overlap inputs");
-    if (info == f || rhs == f || (info && info == rhs)) return fail(CPI_EINVAL, "outputs must not overlap each other");
-    DevInfo d;
-    int rc = device_info(d);
+    int rc = check_aliasing({kind, state_idx, states, z, sqrt_info, aux}, {info, rhs, f});
     if (rc) return rc;
+    DevInfo d;
+    if ((rc = device_info(d))) return rc;
     CU(cpi::measurements_linearize_launch(n, kind, state_idx, states, z, sqrt_info, aux, info, rhs, f, (cudaStream_t)stream));
     g_launches += 1;
     return CPI_OK;
