@@ -25,6 +25,7 @@
 #include <cstdlib>
 #include "cpi_common.cuh"
 #include "cpi_kernels.h"
+#include "exact_math.cuh"
 #include "tma.cuh"
 
 namespace cpi {
@@ -326,8 +327,85 @@ constexpr bool kLoadOnly = false, kCovOnly = false, kNoPrepass = false;
 
 enum : int { SC_A1 = 0, SC_B1, SC_A2, SC_B2, SC_F1, SC_F2, SC_F3, SC_F4, SC_DT6, SC_D1, SC_D2, SC_D3, SC_D4, SC_CA, SC_CB, SC_N };
 
+// Closed-form coefficients (|w| >= 0.008726646) from the sines and cosines of the full and the half step and the reciprocals of
+// |w| and th = |w| dt.  Shared by both pre-passes below, so that both round every expression alike.
+template <int MODEL>
+CPI_DEV void tri_closed_set(double th, double dt, double sn, double cs_, double sh, double ch, double im, double ith, double* v) {
+    const double im2 = im * im, im3 = im2 * im, im4 = im2 * im2, th2 = th * th;
+    v[SC_A1] = sn * im; v[SC_B1] = (1.0 - cs_) * im2;                                   // CpiV1.h:119-120
+    v[SC_A2] = sh * im; v[SC_B2] = (1.0 - ch) * im2;                                    // CpiV1.h:267-268
+    v[SC_F1] = (th * cs_ - sn) * im3;                                                   // CpiV1.h:138-141
+    v[SC_F2] = (th2 - 2.0 * cs_ - 2.0 * th * sn + 2.0) * (0.5 * im4);
+    v[SC_F3] = -(1.0 - cs_) * im2;
+    v[SC_F4] = (th - sn) * im3;
+    if (MODEL == 1) {
+        v[SC_D1] = (th2 * sn - 3.0 * sn + 3.0 * th * cs_) * (im4 * im);                 // CpiV1.h:218-234
+        v[SC_D2] = (th2 - 4.0 * cs_ - 4.0 * th * sn + th2 * cs_ + 4.0) * (im4 * im2);
+        v[SC_D3] = (2.0 * (cs_ - 1.0) + th * sn) * im4;
+        v[SC_D4] = (2.0 * th + th * cs_ - 3.0 * sn) * (im4 * im);
+        // right Jacobian of w dt (CpiV1.h:162-164): w_tx = dt W, w_tx^2 = dt^2 W2
+        v[SC_CA] = ((1.0 - cs_) * (ith * ith)) * dt; v[SC_CB] = ((th - sn) * (ith * ith * ith)) * dt * dt;
+    }
+}
+
+// The scalar set of one sample with the IEEE operations, branching on the step kind: the reference for tri_scalars_fast, and its
+// fallback for inputs outside the fast primitives' domains (huge or subnormal dt, |w dt| >= 2^31, NaN).
+template <int MODEL> __device__ __noinline__ void tri_scalars_ieee(double w0, double w1, double w2, double dt, double* v) {
+#pragma unroll
+    for (int e = 0; e < SC_N; e++) v[e] = 0.0;
+    const double mag = sqrt(w0 * w0 + w1 * w1 + w2 * w2);
+    const double th = mag * dt;
+    if (dt == 0.0) return;
+    const double hd = 0.5 * dt, dt2 = dt * dt, dt3 = dt2 * dt;
+    v[SC_DT6] = dt / 6.0;                                // CpiV1.h:352
+    if (mag < 0.008726646) {                             // Taylor forms: CpiV1.h:101, 119-120, 132-136, 162-164, 196-216, 267-268
+        v[SC_A1] = dt; v[SC_B1] = dt2 * 0.5; v[SC_A2] = hd; v[SC_B2] = (hd * hd) * 0.5;
+        v[SC_F1] = -(dt3 / 3.0); v[SC_F2] = (dt2 * dt2) / 8.0; v[SC_F3] = -(dt2 / 2.0); v[SC_F4] = dt3 / 6.0;
+        if (MODEL == 1) {
+            v[SC_D1] = -(dt3 * dt2 / 15.0); v[SC_D2] = (dt3 * dt3) / 72.0; v[SC_D3] = -(dt2 * dt2 / 12.0); v[SC_D4] = (dt3 * dt2) / 60.0;
+            v[SC_CA] = 0.5 * dt; v[SC_CB] = (1.0 / 6.0) * dt * dt;
+        }
+    } else {
+        double sn, cs_, sh, ch;
+        sincos(th, &sn, &cs_);
+        sincos(mag * 0.5 * dt, &sh, &ch);
+        tri_closed_set<MODEL>(th, dt, sn, cs_, sh, ch, 1.0 / mag, MODEL == 1 ? 1.0 / th : 0.0, v);
+    }
+}
+
+// The same scalar set in one basic block: both coefficient sets are evaluated with the branch-free primitives of exact_math.cuh
+// and one is selected per lane, so that the warp runs one instruction stream whatever mix of Taylor, closed-form and null steps
+// its lanes hold, and nothing calls out of line.  Bit for bit tri_scalars_ieee's result when it returns true.
+template <int MODEL> CPI_DEV bool tri_scalars_fast(double w0, double w1, double w2, double dt, double* v) {
+    const double ss = w0 * w0 + w1 * w1 + w2 * w2;
+    bool ok_m = true, ok_d = true, ok_t = true, ok_c = true;
+    const double mag = ss == 0.0 ? 0.0 : sqrt_rn(ss, ok_m);      // w_hat = 0 exactly: sqrt(+0) = +0, a Taylor step
+    const double th = mag * dt;
+    const bool null_step = dt == 0.0, small_w = mag < 0.008726646;
+    const double hd = 0.5 * dt, dt2 = dt * dt, dt3 = dt2 * dt;
+    const double dt6 = div_const<6>(dt, ok_d);
+    double tv[SC_N], cv[SC_N];
+    tv[SC_A1] = dt; tv[SC_B1] = dt2 * 0.5; tv[SC_A2] = hd; tv[SC_B2] = (hd * hd) * 0.5;
+    tv[SC_F1] = -div_const<3>(dt3, ok_t); tv[SC_F2] = (dt2 * dt2) / 8.0; tv[SC_F3] = -(dt2 / 2.0); tv[SC_F4] = div_const<6>(dt3, ok_t);
+    if (MODEL == 1) {
+        tv[SC_D1] = -div_const<15>(dt3 * dt2, ok_t); tv[SC_D2] = div_const<72>(dt3 * dt3, ok_t); tv[SC_D3] = -div_const<12>(dt2 * dt2, ok_t);
+        tv[SC_D4] = div_const<60>(dt3 * dt2, ok_t);
+        tv[SC_CA] = 0.5 * dt; tv[SC_CB] = (1.0 / 6.0) * dt * dt;
+    }
+    double sn, cs_, sh, ch;
+    sincos_rn(th, &sn, &cs_, ok_c);
+    sincos_rn(mag * 0.5 * dt, &sh, &ch, ok_c);
+    const double im = rcp_rn(mag, ok_c);
+    const double ith = MODEL == 1 ? rcp_rn(th, ok_c) : 0.0;
+    tri_closed_set<MODEL>(th, dt, sn, cs_, sh, ch, im, ith, cv);
+    constexpr int NSC = (MODEL == 1) ? (int)SC_N : (int)SC_D1;
+#pragma unroll
+    for (int e = 0; e < SC_N; e++) v[e] = (null_step || e >= NSC) ? 0.0 : (e == SC_DT6 ? dt6 : (small_w ? tv[e] : cv[e]));
+    return null_step || (ok_m && ok_d && (small_w ? ok_t : ok_c));
+}
+
 template <int MODEL, class T>
-__global__ void __launch_bounds__((TriNT<MODEL, T>::NT), 1) k_preintegrate_tri(const PreintParams p, const bool tma) {
+__global__ void __launch_bounds__((TriNT<MODEL, T>::NT), 1) k_preintegrate_tri(const PreintParams p, const bool tma, const bool ieee_prepass) {
     using SM_ = TriSmem<MODEL, T>;
     constexpr int NT = SM_::NT;
     constexpr int CH = 8 / (int)sizeof(T) * 2;            // samples per TMA chunk: 2 (fp64) or 4 (fp32) = 112 B in one aligned 128-B fetch
@@ -466,51 +544,25 @@ __global__ void __launch_bounds__((TriNT<MODEL, T>::NT), 1) k_preintegrate_tri(c
                 w0 = (double)dst[0]; w1 = (double)dst[1]; w2 = (double)dst[2]; dt = (double)dst[6];
             }
             w0 -= bwo[0]; w1 -= bwo[1]; w2 -= bwo[2];                // CpiV1.h:77-79
-            const double mag = sqrt(w0 * w0 + w1 * w1 + w2 * w2);
-            const double th = mag * dt;
-            // dt == 0 is the reference's silent no-op (CpiV1.h:72-74).  With every scalar below equal to zero the step body is exactly
-            // that (D = I, all increments 0), so null steps -- finished windows, idle lanes, dt = 0 samples -- need no branch around
-            // the shuffles of the body, and they skip the divisions here (a zero operand would send the whole warp through the
-            // slow path of the fp64 division routine).
-            const bool null_step = dt == 0.0;
-            const bool small_w = mag < 0.008726646;                  // CpiV1.h:101
+            // dt == 0 is the reference's silent no-op (CpiV1.h:72-74).  With every scalar equal to zero the step body is exactly that
+            // (D = I, all increments 0), so null steps -- finished windows, idle lanes, dt = 0 samples -- need no branch around the
+            // shuffles of the body.  The set is evaluated straight-line; a warp that holds a lane outside the fast primitives'
+            // domains (or every warp, with ieee_prepass) recomputes the group's sets with the IEEE operations.
             double v[SC_N];
+            if (kLoadOnly || kCovOnly) {
 #pragma unroll
-            for (int e = 0; e < SC_N; e++) v[e] = 0.0;
-            if (kLoadOnly || kCovOnly) v[SC_A1] = w0 + w1 + w2 + dt;
-            else if (kNoPrepass) {
+                for (int e = 0; e < SC_N; e++) v[e] = 0.0;
+                v[SC_A1] = w0 + w1 + w2 + dt;
+            } else if (kNoPrepass) {
 #pragma unroll
                 for (int e = 0; e < SC_N; e++) v[e] = 1e-3;
-            } else if (!null_step) {
-                const double hd = 0.5 * dt, dt2 = dt * dt, dt3 = dt2 * dt;
-                v[SC_DT6] = dt / 6.0;                                // CpiV1.h:352
-                if (small_w) {                                       // Taylor forms: CpiV1.h:119-120, 132-136, 162-164, 196-216, 267-268
-                    v[SC_A1] = dt; v[SC_B1] = dt2 * 0.5; v[SC_A2] = hd; v[SC_B2] = (hd * hd) * 0.5;
-                    v[SC_F1] = -(dt3 / 3.0); v[SC_F2] = (dt2 * dt2) / 8.0; v[SC_F3] = -(dt2 / 2.0); v[SC_F4] = dt3 / 6.0;
-                    if (MODEL == 1) {
-                        v[SC_D1] = -(dt3 * dt2 / 15.0); v[SC_D2] = (dt3 * dt3) / 72.0; v[SC_D3] = -(dt2 * dt2 / 12.0); v[SC_D4] = (dt3 * dt2) / 60.0;
-                        v[SC_CA] = 0.5 * dt; v[SC_CB] = (1.0 / 6.0) * dt * dt;
-                    }
-                } else {
-                    double sn, cs_, sh, ch;
-                    sincos(th, &sn, &cs_);
-                    sincos(mag * 0.5 * dt, &sh, &ch);
-                    const double im = 1.0 / mag;                     // one reciprocal instead of ~16 divisions
-                    const double im2 = im * im, im3 = im2 * im, im4 = im2 * im2, th2 = th * th;
-                    v[SC_A1] = sn * im; v[SC_B1] = (1.0 - cs_) * im2;                                   // CpiV1.h:119-120
-                    v[SC_A2] = sh * im; v[SC_B2] = (1.0 - ch) * im2;                                    // CpiV1.h:267-268
-                    v[SC_F1] = (th * cs_ - sn) * im3;                                                   // CpiV1.h:138-141
-                    v[SC_F2] = (th2 - 2.0 * cs_ - 2.0 * th * sn + 2.0) * (0.5 * im4);
-                    v[SC_F3] = -(1.0 - cs_) * im2;
-                    v[SC_F4] = (th - sn) * im3;
-                    if (MODEL == 1) {
-                        v[SC_D1] = (th2 * sn - 3.0 * sn + 3.0 * th * cs_) * (im4 * im);                 // CpiV1.h:218-234
-                        v[SC_D2] = (th2 - 4.0 * cs_ - 4.0 * th * sn + th2 * cs_ + 4.0) * (im4 * im2);
-                        v[SC_D3] = (2.0 * (cs_ - 1.0) + th * sn) * im4;
-                        v[SC_D4] = (2.0 * th + th * cs_ - 3.0 * sn) * (im4 * im);
-                        const double ith = 1.0 / th;                 // right Jacobian of w dt (CpiV1.h:162-164): w_tx = dt W, w_tx^2 = dt^2 W2
-                        v[SC_CA] = ((1.0 - cs_) * (ith * ith)) * dt; v[SC_CB] = ((th - sn) * (ith * ith * ith)) * dt * dt;
-                    }
+            } else {
+                const bool ok = tri_scalars_fast<MODEL>(w0, w1, w2, dt, v);
+                if (__any_sync(0xffffffffu, !ok || ieee_prepass)) {
+                    double u[SC_N];                                  // not v: the fast set stays in registers on the common path
+                    tri_scalars_ieee<MODEL>(w0, w1, w2, dt, u);
+#pragma unroll
+                    for (int e = 0; e < SC_N; e++) v[e] = u[e];
                 }
             }
             constexpr int NSC = (MODEL == 1) ? (int)SC_N : (int)SC_D1;
@@ -825,7 +877,10 @@ static cudaError_t launch_tri_one(const PreintParams& p0, int num_sms, cudaStrea
     // CPI_B200_TRI_NO_TMA (tests): stage no chunk by TMA, so that the pre-pass copies every sample from global memory -- the
     // reference the staged stream is compared against bit for bit
     const char* no_tma = getenv("CPI_B200_TRI_NO_TMA");
-    kern<<<grid, TriSmem<MODEL, T>::NT, smem, st>>>(p, !(no_tma && no_tma[0] == '1'));
+    // CPI_B200_TRI_IEEE_PREPASS (tests): every group's scalar sets from the IEEE-operation pre-pass, the reference the branch-free
+    // one is compared against bit for bit
+    const char* ieee = getenv("CPI_B200_TRI_IEEE_PREPASS");
+    kern<<<grid, TriSmem<MODEL, T>::NT, smem, st>>>(p, !(no_tma && no_tma[0] == '1'), ieee && ieee[0] == '1');
     return cudaGetLastError();
 }
 
