@@ -952,6 +952,19 @@ int propagate_check(int model, int64_t n, const double* states_k, const double* 
     if (!states_k || !cov_k || !records || !lin || !states_k1 || !cov_k1) return fail(CPI_EINVAL, "null pointer argument");
     return check_aliasing({states_k, cov_k, records, lin}, {states_k1, cov_k1, cross});
 }
+
+// argument checks shared by the two smoother entry points (no CUDA call); scan: the parallel smoother, which needs the workspace
+int rts_check(bool scan, int64_t n_runs, const int64_t* run_offsets, int64_t run_uniform, int64_t n_states, const double* states,
+              const double* cov, const double* pred_states, const double* pred_cov, const double* cross, const double* states_out,
+              const double* cov_out, const double* cross_out, const void* workspace) {
+    int rc = chain_layout_check(n_runs, run_offsets, run_uniform, n_states);
+    if (rc || n_runs == 0) return rc;
+    const bool any_step = n_states > n_runs;                       // a transition exists
+    if (!states || !cov || !states_out || !cov_out || (any_step && (!pred_states || !pred_cov || !cross)))
+        return fail(CPI_EINVAL, "null pointer argument");
+    if (scan && any_step && !workspace) return fail(CPI_EINVAL, "null pointer argument (workspace: cpi_rts_smooth_scan_workspace bytes)");
+    return check_aliasing({run_offsets, states, cov, pred_states, pred_cov, cross}, {states_out, cov_out, cross_out, workspace});
+}
 }  // namespace
 
 extern "C" {
@@ -1070,12 +1083,9 @@ int cpi_state_update_measurements_iterated_batch(int64_t n, const double* states
 int cpi_rts_smooth_batch(int64_t n_runs, const int64_t* run_offsets, int64_t run_uniform, int64_t n_states, const double* states,
                          const double* cov, const double* pred_states, const double* pred_cov, const double* cross, double* states_out,
                          double* cov_out, double* cross_out, void* stream) {
-    int rc = chain_layout_check(n_runs, run_offsets, run_uniform, n_states);
+    int rc = rts_check(false, n_runs, run_offsets, run_uniform, n_states, states, cov, pred_states, pred_cov, cross, states_out, cov_out,
+                       cross_out, nullptr);
     if (rc || n_runs == 0) return rc;
-    const bool any_step = n_states > n_runs;                       // a transition exists
-    if (!states || !cov || !states_out || !cov_out || (any_step && (!pred_states || !pred_cov || !cross)))
-        return fail(CPI_EINVAL, "null pointer argument");
-    if ((rc = check_aliasing({run_offsets, states, cov, pred_states, pred_cov, cross}, {states_out, cov_out, cross_out}))) return rc;
     DevInfo d;
     if ((rc = device_info(d))) return rc;
     CU(cpi::rts_smooth_launch(n_runs, run_offsets, run_offsets ? 0 : run_uniform, states, cov, pred_states, pred_cov, cross, states_out, cov_out,
@@ -1094,13 +1104,9 @@ int64_t cpi_rts_smooth_scan_workspace(int64_t n_runs, int64_t n_states) {
 int cpi_rts_smooth_scan_batch(int64_t n_runs, const int64_t* run_offsets, int64_t run_uniform, int64_t n_states, const double* states,
                               const double* cov, const double* pred_states, const double* pred_cov, const double* cross, double* states_out,
                               double* cov_out, double* cross_out, void* workspace, void* stream) {
-    int rc = chain_layout_check(n_runs, run_offsets, run_uniform, n_states);
+    int rc = rts_check(true, n_runs, run_offsets, run_uniform, n_states, states, cov, pred_states, pred_cov, cross, states_out, cov_out,
+                       cross_out, workspace);
     if (rc || n_runs == 0) return rc;
-    const bool any_step = n_states > n_runs;                       // a transition exists
-    if (!states || !cov || !states_out || !cov_out || (any_step && (!pred_states || !pred_cov || !cross)))
-        return fail(CPI_EINVAL, "null pointer argument");
-    if (any_step && !workspace) return fail(CPI_EINVAL, "null pointer argument (workspace: cpi_rts_smooth_scan_workspace bytes)");
-    if ((rc = check_aliasing({run_offsets, states, cov, pred_states, pred_cov, cross}, {states_out, cov_out, cross_out, workspace}))) return rc;
     DevInfo d;
     if ((rc = device_info(d))) return rc;
     int launches = 0;

@@ -93,6 +93,27 @@ CPI_DEV void quat_multiply(const double* q, const double* p, double* o) {   // q
     o[0] = t[0] / n; o[1] = t[1] / n; o[2] = t[2] / n; o[3] = t[3] / n;
 }
 
+// JPLNavState::retract (gtsam/JPLNavState.cpp:37-71): o = x retracted by the tangent step d (15 doubles)
+CPI_DEV void retract_state(const double* x, const double* d, double* o) {
+    const double nrm = sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
+    double s, c;
+    sincos(nrm / 2.0, &s, &c);
+    double dq[4] = {(s / nrm) * d[0], (s / nrm) * d[1], (s / nrm) * d[2], c};
+    double nn = sqrt(dq[0] * dq[0] + dq[1] * dq[1] + dq[2] * dq[2] + dq[3] * dq[3]);
+#pragma unroll
+    for (int k = 0; k < 4; k++) dq[k] /= nn;
+    if (dq[3] < 0) { dq[0] = -dq[0]; dq[1] = -dq[1]; dq[2] = -dq[2]; dq[3] = -dq[3]; }
+    nn = sqrt(dq[0] * dq[0] + dq[1] * dq[1] + dq[2] * dq[2] + dq[3] * dq[3]);
+    if (isnan(nn)) { dq[0] = dq[1] = dq[2] = 0.0; dq[3] = 1.0; }                       // :53-55 (dtheta == 0 -> 0/0)
+    const double q[4] = {x[0], x[1], x[2], x[3]};
+    double qn[4];
+    quat_multiply(dq, q, qn);
+#pragma unroll
+    for (int k = 0; k < 4; k++) o[k] = qn[k];
+#pragma unroll
+    for (int k = 0; k < 12; k++) o[4 + k] = x[4 + k] + d[3 + k];
+}
+
 CPI_DEV void Exp_so3(const double* w, double* R) {            // quat_ops.h:145-162
     const double th2 = w[0] * w[0] + w[1] * w[1] + w[2] * w[2];
     const double th = sqrt(th2);

@@ -119,11 +119,11 @@ cudaError_t state_update_meas_iter_launch(int64_t n, const double* states, const
                                           const double* z, const double* sqrt_info, const double* aux, const int32_t* loss, const double* loss_k,
                                           const double* gate, int max_iter, double tol, double* states_out, double* cov_out, double* nis,
                                           int32_t* status, int32_t* iterations, cudaStream_t st);
-// update.cu: Rauch-Tung-Striebel smoothing of filter runs from their posteriors and K7's predictions and cross (K15; cross_out may be NULL)
+// rts.cu: Rauch-Tung-Striebel smoothing of filter runs from their posteriors and K7's predictions and cross (K15; cross_out may be NULL)
 cudaError_t rts_smooth_launch(int64_t n_runs, const int64_t* offs, int64_t uniform, const double* states, const double* cov,
                               const double* pred_states, const double* pred_cov, const double* cross, double* states_out, double* cov_out,
                               double* cross_out, cudaStream_t st);
-// rts_scan.cu: the same smoothing by a segmented parallel scan over every keyframe (K16; cross_out may be NULL; workspace
+// rts.cu: the same smoothing by a segmented parallel scan over every keyframe (K16; cross_out may be NULL; workspace
 // rts_scan_workspace_bytes(n), unused when no run has a transition)
 int64_t rts_scan_workspace_bytes(int64_t n_states);
 cudaError_t rts_scan_launch(int64_t n_runs, const int64_t* offs, int64_t uniform, int64_t n, const double* states, const double* cov,

@@ -218,26 +218,7 @@ __global__ void k_predict(int64_t n, const double* states, const double* records
 __global__ void k_retract(int64_t n, const double* states, const double* xi, double* out) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const double* x = states + i * CPI_STATE_DOUBLES;
-    const double* d = xi + i * 15;
-    double* o = out + i * CPI_STATE_DOUBLES;
-    const double nrm = sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
-    double s, c;
-    sincos(nrm / 2.0, &s, &c);
-    double dq[4] = {(s / nrm) * d[0], (s / nrm) * d[1], (s / nrm) * d[2], c};
-    double nn = sqrt(dq[0] * dq[0] + dq[1] * dq[1] + dq[2] * dq[2] + dq[3] * dq[3]);
-#pragma unroll
-    for (int k = 0; k < 4; k++) dq[k] /= nn;
-    if (dq[3] < 0) { dq[0] = -dq[0]; dq[1] = -dq[1]; dq[2] = -dq[2]; dq[3] = -dq[3]; }
-    nn = sqrt(dq[0] * dq[0] + dq[1] * dq[1] + dq[2] * dq[2] + dq[3] * dq[3]);
-    if (isnan(nn)) { dq[0] = dq[1] = dq[2] = 0.0; dq[3] = 1.0; }                       // :53-55 (dtheta == 0 -> 0/0)
-    const double q[4] = {x[0], x[1], x[2], x[3]};
-    double qn[4];
-    quat_multiply(dq, q, qn);
-#pragma unroll
-    for (int k = 0; k < 4; k++) o[k] = qn[k];
-#pragma unroll
-    for (int k = 0; k < 12; k++) o[4 + k] = x[4 + k] + d[3 + k];
+    retract_state(states + i * CPI_STATE_DOUBLES, xi + i * 15, out + i * CPI_STATE_DOUBLES);
 }
 
 // ---- information-form linearisation of the IMU factors ("next" row 1 of SURVEY.md 8f) -------------------------------------

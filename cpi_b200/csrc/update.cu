@@ -15,12 +15,164 @@
 #include "local15.cuh"
 #include "measurement.cuh"
 #include "robust_loss.cuh"
-#include "rts.cuh"
 
 namespace cpi {
 
 constexpr int UWARPS = 4;                        // filters (warps) per CTA
 constexpr int UP = 240;                          // one 15x15 matrix, row-major with pitch 16
+
+// The steps of the square-root update that K10, K11 and K13 share, each the work of one lane role.  Matrices live in shared memory,
+// row-major with pitch 16; C holds chol(I + ...) with v (u on entry) in its spare column 15.
+
+// lane < 15: row lane of M = L C^-T, i.e. (C^-1 L^T)(:, lane) = C^-1 L(lane, :)^T
+CPI_DEV void m_row(const double* L, const double* C, double* M, int lane) {
+    double y[15];
+#pragma unroll
+    for (int k = 0; k < 15; k++) y[k] = k <= lane ? L[lane * 16 + k] : 0.0;
+    fwd15(C, y);
+#pragma unroll
+    for (int k = 0; k < 15; k++) M[lane * 16 + k] = y[k];
+}
+
+// lane 15: v = C^-1 u, in place of u
+CPI_DEV void solve_v(double* C) {
+    double v[15];
+#pragma unroll
+    for (int k = 0; k < 15; k++) v[k] = C[k * 16 + 15];
+    fwd15(C, v);
+#pragma unroll
+    for (int k = 0; k < 15; k++) C[k * 16 + 15] = v[k];
+}
+
+// the warp: w = C^-T v, lane k < 15 storing w_k to w[k * pitch]
+CPI_DEV void solve_w(const double* C, double* w, int pitch, int lane) {
+    const double wk = warp_bwd15(C, lane < 15 ? C[lane * 16 + 15] : 0.0, lane);
+    if (lane < 15) w[lane * pitch] = wk;
+}
+
+// lane < 15: row lane of Sigma+ = M M^T left of the diagonal, mirrored into S, so Sigma+ is exactly symmetric
+CPI_DEV void sigma_row(const double* M, double* S, int lane) {
+    double y[15];
+#pragma unroll
+    for (int k = 0; k < 15; k++) y[k] = M[lane * 16 + k];
+    for (int j = 0; j <= lane; j++) {
+        double t = 0.0;
+#pragma unroll
+        for (int k = 0; k < 15; k++) t = fma(y[k], M[j * 16 + k], t);
+        S[lane * 16 + j] = t;
+        S[j * 16 + lane] = t;
+    }
+}
+
+// lane 15: xi = -L w from w (w_k at w[k * pitch]); returns |w|^2
+CPI_DEV double neg_Lw(const double* L, const double* w, int pitch, double* xi) {
+    double g2 = 0.0;
+#pragma unroll
+    for (int k = 0; k < 15; k++) { xi[k] = w[k * pitch]; g2 = fma(xi[k], xi[k], g2); }
+#pragma unroll
+    for (int r = 14; r >= 0; r--) {               // in place: row r reads xi[0..r]
+        double t = 0.0;
+#pragma unroll
+        for (int k = 0; k <= r; k++) t = fma(L[r * 16 + k], xi[k], t);
+        xi[r] = -t;
+    }
+    return g2;
+}
+
+// lane 15 of K10 and K11: gamma = g1 + g2 against the gate; x retracted by xi if the update applies, else copied bit for bit; nis
+// and applied.  Returns gamma.
+CPI_DEV double finish_state(int64_t i, const double* x, const double* xi, double g1, double g2, const double* gate, double* states_out,
+                            double* nis, int32_t* applied) {
+    const double g = g1 + g2;
+    const bool on = !(gate && g > __ldg(gate + i));
+    double xo[16];
+    if (on) retract_state(x, xi, xo);
+    else
+#pragma unroll
+        for (int k = 0; k < 16; k++) xo[k] = x[k];
+    double* o = states_out + i * CPI_STATE_DOUBLES;
+#pragma unroll
+    for (int k = 0; k < 16; k++) o[k] = xo[k];
+    if (nis) nis[i] = g;
+    if (applied) applied[i] = on ? 1 : 0;
+    return g;
+}
+
+// the warp of K10 and K11, after finish_state: the covariance out (column-major), Sigma+ from S if lane 15's gamma g passes the
+// gate, else the input sg bit for bit
+CPI_DEV void write_cov(int64_t i, double g, const double* gate, const double* S, const double* sg, double* co, int lane) {
+    g = __shfl_sync(0xffffffffu, g, 15);
+    const bool on = !(gate && g > __ldg(gate + i));
+    __syncwarp();
+    if (on)
+        for (int e = lane; e < 225; e += 32) co[e] = S[(e % 15) * 16 + e / 15];
+    else
+        for (int e = lane; e < 225; e += 32) co[e] = __ldg(sg + e);
+}
+
+// the warp: filter i copied bit for bit, its covariance sg and state x (no measurements, or K13's gate)
+CPI_DEV void copy_filter(int64_t i, const double* x, const double* sg, double* states_out, double* co, int lane) {
+    for (int e = lane; e < 225; e += 32) co[e] = __ldg(sg + e);
+    if (lane < CPI_STATE_DOUBLES) states_out[i * CPI_STATE_DOUBLES + lane] = x[lane];
+}
+
+// the warp (K11, K13): C = I + sum_j B_j^T B_j with u = sum_j B_j^T b_j in column 15, over measurements j0 .. j1-1 linearised at x.
+// M is scratch: A_j, b_j (row-major 3x15, then 3) and from M + 48 B_j | b_j (3 rows, pitch 16).  kIter (K13): lane 0 shifts b_j by
+// -A_j d_t (D; t > 0) and weights A_j and b_j by sqrt(om_j) of the loss.
+template <bool kIter>
+CPI_DEV void gram(const double* L, double* C, double* M, const double* x, int64_t j0, int64_t j1, const int32_t* kind, const double* z,
+                  const double* sqrt_info, const double* aux, const int32_t* loss, const double* loss_k, int t, const double* D, int lane) {
+    double* B = M + 48;
+    double y[15];                                 // lane c < 15: column c of sum B^T B; lane 15: u
+#pragma unroll
+    for (int r = 0; r < 15; r++) y[r] = 0.0;
+    for (int64_t j = j0; j < j1; j++) {
+        if (lane == 0) {
+            meas_linearize(__ldg(kind + j), x, z + j * 3, sqrt_info + j * 9, aux + j * 3, M + 45, M);
+            if constexpr (kIter) {
+                double om, c;
+                robust_loss(loss ? __ldg(loss + j) : CPI_LOSS_GAUSSIAN, loss ? __ldg(loss_k + j) : 0.0,
+                            fma(M[47], M[47], fma(M[46], M[46], M[45] * M[45])), om, c);
+                if (t > 0)                        // b_j - A_j d_t (d_0 = 0)
+#pragma unroll
+                    for (int k = 0; k < 3; k++) {
+                        double e = M[45 + k];
+#pragma unroll
+                        for (int m = 0; m < 15; m++) e = fma(-M[k * 15 + m], D[m], e);
+                        M[45 + k] = e;
+                    }
+                if (om != 1.0) {
+                    const double sw = sqrt(om);
+#pragma unroll
+                    for (int k = 0; k < 48; k++) M[k] *= sw;
+                }
+            }
+        }
+        __syncwarp();
+        if (lane < 15) {                          // B_j(k, lane) = sum_{m >= lane} A_j(k, m) L(m, lane)
+#pragma unroll
+            for (int k = 0; k < 3; k++) {
+                double s = 0.0;
+#pragma unroll
+                for (int m = 0; m < 15; m++) s = m >= lane ? fma(M[k * 15 + m], L[m * 16 + lane], s) : s;
+                B[k * 16 + lane] = s;
+            }
+        } else if (lane == 15) {
+#pragma unroll
+            for (int k = 0; k < 3; k++) B[k * 16 + 15] = M[45 + k];
+        }
+        __syncwarp();
+        if (lane < 16) {
+#pragma unroll
+            for (int r = 0; r < 15; r++) y[r] = fma(B[32 + r], B[32 + lane], fma(B[16 + r], B[16 + lane], fma(B[r], B[lane], y[r])));
+        }
+        __syncwarp();
+    }
+    if (lane < 16) {
+#pragma unroll
+        for (int r = 0; r < 15; r++) C[r * 16 + lane] = r == lane ? y[r] + 1.0 : y[r];
+    }
+}
 
 __global__ void __launch_bounds__(UWARPS * 32) k_state_update(int64_t n, const double* states, const double* cov, const double* meas_info,
                                                              const double* meas_states, const double* gate, double* states_out,
@@ -71,50 +223,17 @@ __global__ void __launch_bounds__(UWARPS * 32) k_state_update(int64_t n, const d
     __syncwarp();
     warp_chol15(C, lane);                         // eigenvalues >= 1 for a PSD W; column 15 is not touched
 
-    if (lane < 15) {                              // row lane of M: (C^-1 L^T)(:, lane) = C^-1 L(lane, :)^T
-        double y[15];
-#pragma unroll
-        for (int k = 0; k < 15; k++) y[k] = k <= lane ? L[lane * 16 + k] : 0.0;
-        fwd15(C, y);
-#pragma unroll
-        for (int k = 0; k < 15; k++) M[lane * 16 + k] = y[k];
-    } else if (lane == 15) {                      // v = C^-1 u, in place of u
-        double v[15];
-#pragma unroll
-        for (int k = 0; k < 15; k++) v[k] = C[k * 16 + 15];
-        fwd15(C, v);
-#pragma unroll
-        for (int k = 0; k < 15; k++) C[k * 16 + 15] = v[k];
-    }
+    if (lane < 15) m_row(L, C, M, lane);
+    else if (lane == 15) solve_v(C);
     __syncwarp();
-    {                                             // w = C^-T v = -L^-1 xi, lane k holds w_k; into the spare column 15 of M
-        const double wk = warp_bwd15(C, lane < 15 ? C[lane * 16 + 15] : 0.0, lane);
-        if (lane < 15) M[lane * 16 + 15] = wk;
-    }
+    solve_w(C, M + 15, 16, lane);                 // w = -L^-1 xi, into the spare column 15 of M
     __syncwarp();
     double g = 0.0;
-    if (lane < 15) {                              // Sigma+(lane, j) = M(lane, :) M(j, :)^T, j <= lane, mirrored
-        double y[15];
-#pragma unroll
-        for (int k = 0; k < 15; k++) y[k] = M[lane * 16 + k];
-        for (int j = 0; j <= lane; j++) {
-            double t = 0.0;
-#pragma unroll
-            for (int k = 0; k < 15; k++) t = fma(y[k], M[j * 16 + k], t);
-            C[lane * 16 + j] = t;
-            C[j * 16 + lane] = t;
-        }
+    if (lane < 15) {
+        sigma_row(M, C, lane);
     } else if (lane == 15) {
-        double w[15], g2 = 0.0;
-#pragma unroll
-        for (int k = 0; k < 15; k++) { w[k] = M[k * 16 + 15]; g2 = fma(w[k], w[k], g2); }
-#pragma unroll
-        for (int r = 14; r >= 0; r--) {           // xi = -L w in place (row r reads w[0..r])
-            double t = 0.0;
-#pragma unroll
-            for (int k = 0; k <= r; k++) t = fma(L[r * 16 + k], w[k], t);
-            w[r] = -t;
-        }
+        double w[15];                             // xi
+        const double g2 = neg_Lw(L, M + 15, 16, w);
         double g1 = 0.0;
 #pragma unroll
         for (int r = 0; r < 15; r++) {            // (d + xi)^T W (d + xi)
@@ -123,27 +242,9 @@ __global__ void __launch_bounds__(UWARPS * 32) k_state_update(int64_t n, const d
             for (int k = 0; k < 15; k++) t = fma(W[r * 16 + k], W[k * 16 + 15] + w[k], t);
             g1 = fma(W[r * 16 + 15] + w[r], t, g1);
         }
-        g = g1 + g2;
-        const bool on = !(gate && g > __ldg(gate + i));
-        double xo[16];
-        if (on) retract_state(x, w, xo);
-        else
-#pragma unroll
-            for (int k = 0; k < 16; k++) xo[k] = x[k];
-        double* o = states_out + i * CPI_STATE_DOUBLES;
-#pragma unroll
-        for (int k = 0; k < 16; k++) o[k] = xo[k];
-        if (nis) nis[i] = g;
-        if (applied) applied[i] = on ? 1 : 0;
+        g = finish_state(i, x, w, g1, g2, gate, states_out, nis, applied);
     }
-    g = __shfl_sync(0xffffffffu, g, 15);
-    const bool on = !(gate && g > __ldg(gate + i));
-    __syncwarp();
-    double* co = cov_out + i * 225;
-    if (on)
-        for (int e = lane; e < 225; e += 32) co[e] = C[(e % 15) * 16 + e / 15];
-    else
-        for (int e = lane; e < 225; e += 32) co[e] = __ldg(sg + e);
+    write_cov(i, g, gate, C, sg, cov_out + i * 225, lane);
 }
 
 cudaError_t state_update_launch(int64_t n, const double* states, const double* cov, const double* meas_info, const double* meas_states,
@@ -175,8 +276,7 @@ __global__ void __launch_bounds__(UWARPS * 32) k_state_update_meas(int64_t n, co
     double* co = cov_out + i * 225;
     const int64_t j0 = __ldg(meas_offsets + i), j1 = __ldg(meas_offsets + i + 1);
     if (j0 >= j1) {                               // nothing to apply
-        for (int e = lane; e < 225; e += 32) co[e] = __ldg(sg + e);
-        if (lane < CPI_STATE_DOUBLES) states_out[i * CPI_STATE_DOUBLES + lane] = x[lane];
+        copy_filter(i, x, sg, states_out, co, lane);
         if (lane == 0) {
             if (nis) nis[i] = 0.0;
             if (applied) applied[i] = 1;
@@ -186,87 +286,24 @@ __global__ void __launch_bounds__(UWARPS * 32) k_state_update_meas(int64_t n, co
     double* L = smem[warp];                       // Sigma, then its Cholesky factor (lower triangle)
     double* C = L + UP;                           // I + sum B^T B (column 15: u), its Cholesky factor, then Sigma+
     double* M = C + UP;                           // A_j, b_j (row-major 3x15, then 3) and B_j | b_j (3 rows, pitch 16); then L C^-T
-    double* B = M + 48;
     for (int e = lane; e < 225; e += 32) L[(e % 15) * 16 + e / 15] = __ldg(sg + e);
     __syncwarp();
     warp_chol15(L, lane);
-
-    double y[15];                                 // lane c < 15: column c of sum B^T B; lane 15: u
-#pragma unroll
-    for (int r = 0; r < 15; r++) y[r] = 0.0;
-    for (int64_t j = j0; j < j1; j++) {
-        if (lane == 0) meas_linearize(__ldg(kind + j), x, z + j * 3, sqrt_info + j * 9, aux + j * 3, M + 45, M);
-        __syncwarp();
-        if (lane < 15) {                          // B_j(k, lane) = sum_{m >= lane} A_j(k, m) L(m, lane)
-#pragma unroll
-            for (int k = 0; k < 3; k++) {
-                double t = 0.0;
-#pragma unroll
-                for (int m = 0; m < 15; m++) t = m >= lane ? fma(M[k * 15 + m], L[m * 16 + lane], t) : t;
-                B[k * 16 + lane] = t;
-            }
-        } else if (lane == 15) {
-#pragma unroll
-            for (int k = 0; k < 3; k++) B[k * 16 + 15] = M[45 + k];
-        }
-        __syncwarp();
-        if (lane < 16) {
-#pragma unroll
-            for (int r = 0; r < 15; r++) y[r] = fma(B[32 + r], B[32 + lane], fma(B[16 + r], B[16 + lane], fma(B[r], B[lane], y[r])));
-        }
-        __syncwarp();
-    }
-    if (lane < 16) {
-#pragma unroll
-        for (int r = 0; r < 15; r++) C[r * 16 + lane] = r == lane ? y[r] + 1.0 : y[r];
-    }
+    gram<false>(L, C, M, x, j0, j1, kind, z, sqrt_info, aux, nullptr, nullptr, 0, nullptr, lane);
     __syncwarp();
     warp_chol15(C, lane);                         // eigenvalues >= 1; column 15 is not touched
 
-    if (lane < 15) {                              // row lane of M = L C^-T
-        double t[15];
-#pragma unroll
-        for (int k = 0; k < 15; k++) t[k] = k <= lane ? L[lane * 16 + k] : 0.0;
-        fwd15(C, t);
-#pragma unroll
-        for (int k = 0; k < 15; k++) M[lane * 16 + k] = t[k];
-    } else if (lane == 15) {                      // v = C^-1 u, in place of u
-        double v[15];
-#pragma unroll
-        for (int k = 0; k < 15; k++) v[k] = C[k * 16 + 15];
-        fwd15(C, v);
-#pragma unroll
-        for (int k = 0; k < 15; k++) C[k * 16 + 15] = v[k];
-    }
+    if (lane < 15) m_row(L, C, M, lane);
+    else if (lane == 15) solve_v(C);
     __syncwarp();
-    {                                             // w = C^-T v, lane k holds w_k; into the spare column 15 of M
-        const double wk = warp_bwd15(C, lane < 15 ? C[lane * 16 + 15] : 0.0, lane);
-        if (lane < 15) M[lane * 16 + 15] = wk;
-    }
+    solve_w(C, M + 15, 16, lane);                 // into the spare column 15 of M
     __syncwarp();
     double g = 0.0;
-    if (lane < 15) {                              // Sigma+(lane, j) = M(lane, :) M(j, :)^T, j <= lane, mirrored
-        double t[15];
-#pragma unroll
-        for (int k = 0; k < 15; k++) t[k] = M[lane * 16 + k];
-        for (int j = 0; j <= lane; j++) {
-            double s = 0.0;
-#pragma unroll
-            for (int k = 0; k < 15; k++) s = fma(t[k], M[j * 16 + k], s);
-            C[lane * 16 + j] = s;
-            C[j * 16 + lane] = s;
-        }
+    if (lane < 15) {
+        sigma_row(M, C, lane);
     } else if (lane == 15) {
-        double w[15], g2 = 0.0;
-#pragma unroll
-        for (int k = 0; k < 15; k++) { w[k] = M[k * 16 + 15]; g2 = fma(w[k], w[k], g2); }
-#pragma unroll
-        for (int r = 14; r >= 0; r--) {           // xi = -L w in place (row r reads w[0..r])
-            double t = 0.0;
-#pragma unroll
-            for (int k = 0; k <= r; k++) t = fma(L[r * 16 + k], w[k], t);
-            w[r] = -t;
-        }
+        double w[15];                             // xi
+        const double g2 = neg_Lw(L, M + 15, 16, w);
         double g1 = 0.0;
         for (int64_t j = j0; j < j1; j++) {       // |b_j + A_j xi|^2
             double A[45], b[3];
@@ -279,26 +316,9 @@ __global__ void __launch_bounds__(UWARPS * 32) k_state_update_meas(int64_t n, co
                 g1 = fma(e, e, g1);
             }
         }
-        g = g1 + g2;
-        const bool on = !(gate && g > __ldg(gate + i));
-        double xo[16];
-        if (on) retract_state(x, w, xo);
-        else
-#pragma unroll
-            for (int k = 0; k < 16; k++) xo[k] = x[k];
-        double* o = states_out + i * CPI_STATE_DOUBLES;
-#pragma unroll
-        for (int k = 0; k < 16; k++) o[k] = xo[k];
-        if (nis) nis[i] = g;
-        if (applied) applied[i] = on ? 1 : 0;
+        g = finish_state(i, x, w, g1, g2, gate, states_out, nis, applied);
     }
-    g = __shfl_sync(0xffffffffu, g, 15);
-    const bool on = !(gate && g > __ldg(gate + i));
-    __syncwarp();
-    if (on)
-        for (int e = lane; e < 225; e += 32) co[e] = C[(e % 15) * 16 + e / 15];
-    else
-        for (int e = lane; e < 225; e += 32) co[e] = __ldg(sg + e);
+    write_cov(i, g, gate, C, sg, co, lane);
 }
 
 cudaError_t state_update_meas_launch(int64_t n, const double* states, const double* cov, const int64_t* meas_offsets, const int32_t* kind,
@@ -339,8 +359,7 @@ __global__ void __launch_bounds__(UWARPS * 32) k_state_update_meas_iter(int64_t 
     double* co = cov_out + i * 225;
     const int64_t j0 = __ldg(meas_offsets + i), j1 = __ldg(meas_offsets + i + 1);
     if (j0 >= j1) {                               // nothing to apply
-        for (int e = lane; e < 225; e += 32) co[e] = __ldg(sg + e);
-        if (lane < CPI_STATE_DOUBLES) states_out[i * CPI_STATE_DOUBLES + lane] = x[lane];
+        copy_filter(i, x, sg, states_out, co, lane);
         if (lane == 0) {
             if (nis) nis[i] = 0.0;
             if (status) status[i] = 1;
@@ -351,7 +370,6 @@ __global__ void __launch_bounds__(UWARPS * 32) k_state_update_meas_iter(int64_t 
     double* L = smem[warp];                       // Sigma, then its Cholesky factor (lower triangle)
     double* C = L + UP;                           // I + sum B^T B (column 15: u), its Cholesky factor; after the loop Sigma+
     double* M = C + UP;                           // weighted A_j, b'_j (row-major 3x15, then 3) and B_j | b'_j (3 rows, pitch 16); then L C^-T
-    double* B = M + 48;
     double* X = M + UP;                           // x_t
     double* D = X + 16;                           // d_t
     double* W = D + 16;                           // w
@@ -370,81 +388,17 @@ __global__ void __launch_bounds__(UWARPS * 32) k_state_update_meas_iter(int64_t 
             for (int r = 0; r < 15; r++) D[r] = d[r];
         }
         __syncwarp();
-        double y[15];                             // lane c < 15: column c of sum B^T B; lane 15: u
-#pragma unroll
-        for (int r = 0; r < 15; r++) y[r] = 0.0;
-        for (int64_t j = j0; j < j1; j++) {
-            if (lane == 0) {
-                meas_linearize(__ldg(kind + j), X, z + j * 3, sqrt_info + j * 9, aux + j * 3, M + 45, M);
-                double om, c;
-                robust_loss(loss ? __ldg(loss + j) : CPI_LOSS_GAUSSIAN, loss ? __ldg(loss_k + j) : 0.0,
-                            fma(M[47], M[47], fma(M[46], M[46], M[45] * M[45])), om, c);
-                if (t > 0)                        // b_j - A_j d_t (d_0 = 0)
-#pragma unroll
-                    for (int k = 0; k < 3; k++) {
-                        double e = M[45 + k];
-#pragma unroll
-                        for (int m = 0; m < 15; m++) e = fma(-M[k * 15 + m], D[m], e);
-                        M[45 + k] = e;
-                    }
-                if (om != 1.0) {
-                    const double sw = sqrt(om);
-#pragma unroll
-                    for (int k = 0; k < 48; k++) M[k] *= sw;
-                }
-            }
-            __syncwarp();
-            if (lane < 15) {                      // B_j(k, lane) = sum_{m >= lane} A_j(k, m) L(m, lane)
-#pragma unroll
-                for (int k = 0; k < 3; k++) {
-                    double s = 0.0;
-#pragma unroll
-                    for (int m = 0; m < 15; m++) s = m >= lane ? fma(M[k * 15 + m], L[m * 16 + lane], s) : s;
-                    B[k * 16 + lane] = s;
-                }
-            } else if (lane == 15) {
-#pragma unroll
-                for (int k = 0; k < 3; k++) B[k * 16 + 15] = M[45 + k];
-            }
-            __syncwarp();
-            if (lane < 16) {
-#pragma unroll
-                for (int r = 0; r < 15; r++) y[r] = fma(B[32 + r], B[32 + lane], fma(B[16 + r], B[16 + lane], fma(B[r], B[lane], y[r])));
-            }
-            __syncwarp();
-        }
-        if (lane < 16) {
-#pragma unroll
-            for (int r = 0; r < 15; r++) C[r * 16 + lane] = r == lane ? y[r] + 1.0 : y[r];
-        }
+        gram<true>(L, C, M, X, j0, j1, kind, z, sqrt_info, aux, loss, loss_k, t, D, lane);
         __syncwarp();
         warp_chol15(C, lane);                     // eigenvalues >= 1; column 15 is not touched
-        if (lane == 15) {                         // v = C^-1 u, in place of u
-            double v[15];
-#pragma unroll
-            for (int k = 0; k < 15; k++) v[k] = C[k * 16 + 15];
-            fwd15(C, v);
-#pragma unroll
-            for (int k = 0; k < 15; k++) C[k * 16 + 15] = v[k];
-        }
+        if (lane == 15) solve_v(C);
         __syncwarp();
-        {                                         // w = C^-T v, lane k holds w_k
-            const double wk = warp_bwd15(C, lane < 15 ? C[lane * 16 + 15] : 0.0, lane);
-            if (lane < 15) W[lane] = wk;
-        }
+        solve_w(C, W, 1, lane);
         __syncwarp();
         st = -1;
         if (lane == 15) {
-            double w[15], g2 = 0.0;
-#pragma unroll
-            for (int k = 0; k < 15; k++) { w[k] = W[k]; g2 = fma(w[k], w[k], g2); }
-#pragma unroll
-            for (int r = 14; r >= 0; r--) {       // eps = -L w in place (row r reads w[0..r])
-                double s = 0.0;
-#pragma unroll
-                for (int k = 0; k <= r; k++) s = fma(L[r * 16 + k], w[k], s);
-                w[r] = -s;
-            }
+            double w[15];                         // eps
+            const double g2 = neg_Lw(L, W, 1, w);
             if (t == 0) {                         // gamma: sum om_j |b_j + A_j eps_0|^2 + |w_0|^2 at x_hat
                 double g1 = 0.0;
                 for (int64_t j = j0; j < j1; j++) {
@@ -483,30 +437,11 @@ __global__ void __launch_bounds__(UWARPS * 32) k_state_update_meas_iter(int64_t 
     } while (st < 0);
 
     if (st == 0) {                                // gated: the inputs
-        for (int e = lane; e < 225; e += 32) co[e] = __ldg(sg + e);
-        if (lane < CPI_STATE_DOUBLES) states_out[i * CPI_STATE_DOUBLES + lane] = x[lane];
+        copy_filter(i, x, sg, states_out, co, lane);
     } else {
-        if (lane < 15) {                          // row lane of M = L C^-T, from the last C
-            double r[15];
-#pragma unroll
-            for (int k = 0; k < 15; k++) r[k] = k <= lane ? L[lane * 16 + k] : 0.0;
-            fwd15(C, r);
-#pragma unroll
-            for (int k = 0; k < 15; k++) M[lane * 16 + k] = r[k];
-        }
+        if (lane < 15) m_row(L, C, M, lane);      // from the last C
         __syncwarp();
-        if (lane < 15) {                          // Sigma+(lane, j) = M(lane, :) M(j, :)^T, j <= lane, mirrored
-            double r[15];
-#pragma unroll
-            for (int k = 0; k < 15; k++) r[k] = M[lane * 16 + k];
-            for (int j = 0; j <= lane; j++) {
-                double s = 0.0;
-#pragma unroll
-                for (int k = 0; k < 15; k++) s = fma(r[k], M[j * 16 + k], s);
-                C[lane * 16 + j] = s;
-                C[j * 16 + lane] = s;
-            }
-        }
+        if (lane < 15) sigma_row(M, C, lane);
         __syncwarp();
         for (int e = lane; e < 225; e += 32) co[e] = C[(e % 15) * 16 + e / 15];
         if (lane < CPI_STATE_DOUBLES) states_out[i * CPI_STATE_DOUBLES + lane] = X[lane];
@@ -526,140 +461,6 @@ cudaError_t state_update_meas_iter_launch(int64_t n, const double* states, const
     const int64_t grid = (n + UWARPS - 1) / UWARPS;
     k_state_update_meas_iter<<<(unsigned)grid, UWARPS * 32, 0, st>>>(n, states, cov, meas_offsets, kind, z, sqrt_info, aux, loss, loss_k, gate,
                                                                      max_iter, tol, states_out, cov_out, nis, status, iterations);
-    return cudaGetLastError();
-}
-
-// K15: Rauch-Tung-Striebel smoothing of filter runs (DESIGN.md section 3o).  Run c holds keyframes o[c] .. o[c+1]-1 with the
-// filter's posteriors (x_k, P_k); its transitions are stored from o[c] - c, transition k carrying K7's prediction (xb_{k+1},
-// Pb_{k+1}) and cross C_k = P_k A_k^T from (x_k, P_k).  From the last keyframe (copied bit for bit) backwards:
-//   G = C_k Pb^-1 (Pb = L L^T),  d = local(xb_{k+1}, xs_{k+1}),  xs_k = retract(x_k, G d),
-//   Ps_k = P_k + G (Ps_{k+1} - Pb) G^T,  Xs_k = G Ps_{k+1}  (the smoothed (x_k, x_{k+1}) block)
-// One warp per run, sequential over its keyframes; xs_{k+1} and Ps_{k+1} are carried in shared memory.  Lane i < 15 solves row i
-// of G from row i of C_k with L (two per-lane triangular solves) while lane 15 forms d, then row i of T = G (Ps_{k+1} - Pb), row i
-// of Xs_k and (G d)_i; after a sync it forms row i of Ps_k left of the diagonal and mirrors it, so Ps_k is exactly symmetric, while
-// lane 15 retracts.  A Pb that is not SPD gives NaN from that keyframe back, in that run only.  No atomics: the same bits on every run.
-constexpr int RP = 240;                          // one 15x15 matrix, row-major with pitch 16
-
-__global__ void __launch_bounds__(UWARPS * 32) k_rts_smooth(int64_t n_runs, const int64_t* offs, int64_t uniform, const double* states,
-                                                           const double* cov, const double* pred_states, const double* pred_cov,
-                                                           const double* cross, double* states_out, double* cov_out, double* cross_out) {
-    __shared__ double smem[UWARPS][5 * RP + 64];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int64_t c = (int64_t)blockIdx.x * UWARPS + warp;
-    if (c >= n_runs) return;
-    double* Pb = smem[warp];                      // Pb_{k+1}
-    double* L = Pb + RP;                          // its Cholesky factor (lower triangle)
-    double* G = L + RP;                           // C_k, then G row by row
-    double* Ps = G + RP;                          // Ps_{k+1}, then Ps_k
-    double* Pk = Ps + RP;                         // P_k
-    double* XS = Pk + RP;                         // xs_{k+1}, then xs_k
-    double* XK = XS + 16;                         // x_k
-    double* XB = XK + 16;                         // xb_{k+1}
-    double* GD = XB + 16;                         // G d
-    const int64_t o0 = offs ? __ldg(offs + c) : c * uniform;
-    const int64_t o1 = offs ? __ldg(offs + c + 1) : o0 + uniform;
-    const int64_t last = o1 - 1, t0 = o0 - c;     // the run's last keyframe and its first transition
-    {                                             // the last keyframe: copied, and carried
-        const double* sg = cov + last * 225;
-        double* co = cov_out + last * 225;
-        for (int e = lane; e < 225; e += 32) {
-            const double v = __ldg(sg + e);
-            co[e] = v;
-            Ps[(e % 15) * 16 + e / 15] = v;
-        }
-        if (lane < CPI_STATE_DOUBLES) {
-            const double v = __ldg(states + last * CPI_STATE_DOUBLES + lane);
-            states_out[last * CPI_STATE_DOUBLES + lane] = v;
-            XS[lane] = v;
-        }
-    }
-    for (int64_t s = last - 1; s >= o0; s--) {
-        const int64_t t = t0 + (s - o0);
-        const double* pg = pred_cov + t * 225;
-        const double* cg = cross + t * 225;
-        const double* sg = cov + s * 225;
-        for (int e = lane; e < 225; e += 32) {    // column-major (r, c) -> row-major pitch 16
-            const int r = e % 15, q = e / 15;
-            const double p = __ldg(pg + e);
-            Pb[r * 16 + q] = p;
-            L[r * 16 + q] = p;
-            G[r * 16 + q] = __ldg(cg + e);
-            Pk[r * 16 + q] = __ldg(sg + e);
-        }
-        if (lane < CPI_STATE_DOUBLES) {
-            XK[lane] = __ldg(states + s * CPI_STATE_DOUBLES + lane);
-            XB[lane] = __ldg(pred_states + t * CPI_STATE_DOUBLES + lane);
-        }
-        __syncwarp();
-        rts_gain(L, G, lane, [&] {                // d = local(xb_{k+1}, xs_{k+1}) in the spare column 15 of G
-            double d[15];
-            local15(XB, XS, d);
-#pragma unroll
-            for (int r = 0; r < 15; r++) G[r * 16 + 15] = d[r];
-        });
-        __syncwarp();
-        if (lane < 15) {                          // row lane of T = G (Ps_{k+1} - Pb) into L (free after the solves), of Xs_k, and (G d)_lane
-            const double* g = G + lane * 16;
-            double gd = 0.0;
-#pragma unroll
-            for (int m = 0; m < 15; m++) gd = fma(g[m], G[m * 16 + 15], gd);
-            GD[lane] = gd;
-            double tr[15];
-#pragma unroll
-            for (int j = 0; j < 15; j++) tr[j] = 0.0;
-#pragma unroll 1
-            for (int m = 0; m < 15; m++) {
-                const double gm = g[m];
-#pragma unroll
-                for (int j = 0; j < 15; j++) tr[j] = fma(gm, Ps[m * 16 + j] - Pb[m * 16 + j], tr[j]);
-            }
-#pragma unroll
-            for (int j = 0; j < 15; j++) L[lane * 16 + j] = tr[j];
-            if (cross_out) {                      // Xs_k(lane, j) = G(lane, :) Ps_{k+1}(:, j), column-major: coalesced over lanes
-                double* xo = cross_out + t * 225;
-#pragma unroll 1
-                for (int j = 0; j < 15; j++) {
-                    double x = 0.0;
-#pragma unroll
-                    for (int m = 0; m < 15; m++) x = fma(g[m], Ps[m * 16 + j], x);
-                    xo[lane + 15 * j] = x;
-                }
-            }
-        }
-        __syncwarp();
-        if (lane < 15) {                          // Ps_k(lane, j) = P_k(lane, j) + T(lane, :) G(j, :)^T, j <= lane, mirrored
-            double tr[15];
-#pragma unroll
-            for (int m = 0; m < 15; m++) tr[m] = L[lane * 16 + m];
-            for (int j = 0; j <= lane; j++) {
-                double v = 0.0;
-#pragma unroll
-                for (int m = 0; m < 15; m++) v = fma(tr[m], G[j * 16 + m], v);
-                v += Pk[lane * 16 + j];
-                Ps[lane * 16 + j] = v;
-                Ps[j * 16 + lane] = v;
-            }
-        } else if (lane == 15) {                  // xs_k = retract(x_k, G d)
-            double xo[16];
-            retract_state(XK, GD, xo);
-            double* o = states_out + s * CPI_STATE_DOUBLES;
-#pragma unroll
-            for (int k = 0; k < 16; k++) { XS[k] = xo[k]; o[k] = xo[k]; }
-        }
-        __syncwarp();
-        double* co = cov_out + s * 225;
-        for (int e = lane; e < 225; e += 32) co[e] = Ps[(e % 15) * 16 + e / 15];
-        __syncwarp();
-    }
-}
-
-cudaError_t rts_smooth_launch(int64_t n_runs, const int64_t* offs, int64_t uniform, const double* states, const double* cov,
-                              const double* pred_states, const double* pred_cov, const double* cross, double* states_out, double* cov_out,
-                              double* cross_out, cudaStream_t st) {
-    if (n_runs == 0) return cudaSuccess;
-    const int64_t grid = (n_runs + UWARPS - 1) / UWARPS;
-    k_rts_smooth<<<(unsigned)grid, UWARPS * 32, 0, st>>>(n_runs, offs, uniform, states, cov, pred_states, pred_cov, cross, states_out,
-                                                        cov_out, cross_out);
     return cudaGetLastError();
 }
 

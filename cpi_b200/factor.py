@@ -1204,30 +1204,16 @@ def update(states, cov, meas_info, meas_states, gate=None, stream=None):
     Returns (states [n,16], cov [n,225] exactly symmetric, nis [n], applied [n] int32 0/1)."""
     import torch
 
-    dev = states.device
-    for name, t in (("states", states), ("cov", cov), ("meas_info", meas_info), ("meas_states", meas_states)):
+    dev, n = _filter_checks(states, cov, gate, "update")
+    for name, t in (("meas_info", meas_info), ("meas_states", meas_states)):
         if not isinstance(t, torch.Tensor):
             raise ValueError(f"{name} must be a tensor")
-    if not states.is_cuda:
-        raise ValueError("states must be a CUDA tensor")
-    _check_f64(dev, states=states, cov=cov, meas_info=meas_info, meas_states=meas_states)
-    n = states.numel() // 16
-    if states.numel() != 16 * n or cov.numel() != 225 * n or meas_info.numel() != 225 * n or meas_states.numel() != 16 * n:
-        raise ValueError("update needs states [n,16], cov [n,225], meas_info [n,225] and meas_states [n,16]")
-    if isinstance(gate, torch.Tensor):
-        _check_f64(dev, gate=gate)
-        if gate.numel() != n:
-            raise ValueError(f"gate needs one entry per filter ({n}), got {gate.numel()}")
-    elif gate is not None and math.isnan(float(gate)):
-        raise ValueError("gate must not be NaN (+inf applies every fix)")
+    _check_f64(dev, meas_info=meas_info, meas_states=meas_states)
+    if meas_info.numel() != 225 * n or meas_states.numel() != 16 * n:
+        raise ValueError("update needs meas_info [n,225] and meas_states [n,16]")
     f64 = dict(dtype=torch.float64, device=dev)
     with _on(dev, stream):                                           # the gate's check and fill are ordered with the launch
-        if isinstance(gate, torch.Tensor):
-            gate = gate.contiguous()
-            if bool(torch.isnan(gate).any()):
-                raise ValueError("gate must not be NaN (+inf applies every fix)")
-        elif gate is not None:
-            gate = torch.full((n,), float(gate), **f64)
+        gate = _filter_gate(gate, n, f64)
         x1, c1, nis = torch.empty((n, 16), **f64), torch.empty((n, 225), **f64), torch.empty(n, **f64)
         applied = torch.empty(n, dtype=torch.int32, device=dev)
         if n:
@@ -1318,44 +1304,7 @@ def rts_smooth(model, states, cov, records, lin, run_offsets, cross=False, n_run
     A Pb_{k+1} that is not SPD gives NaN for that run only.  Enqueues on ``stream`` (default: torch's current stream) without
     synchronising.  Returns (states_s [N,16], cov_s [N,225] exactly symmetric, cross_s [N - n_runs,225] with Xs_k in transition k's
     slot, the slots and orientation of chains_covariance's cross, or None)."""
-    import torch
-
-    if model not in (1, 2):
-        raise ValueError(f"model must be 1 or 2 (got {model!r})")
-    for name, t in (("states", states), ("cov", cov), ("records", records), ("lin", lin)):
-        if not isinstance(t, torch.Tensor):
-            raise ValueError(f"{name} must be a tensor")
-    if not states.is_cuda:
-        raise ValueError("states must be a CUDA tensor")
-    dev = states.device
-    _check_f64(dev, states=states, cov=cov, records=records, lin=lin)
-    N = states.numel() // 16
-    if N < 1 or states.numel() != 16 * N or cov.numel() != 225 * N:
-        raise ValueError("rts_smooth needs states [N,16] and cov [N,225] with at least one keyframe")
-    if isinstance(run_offsets, torch.Tensor):
-        if run_offsets.numel() - 1 > N:
-            raise ValueError(f"run_offsets has {run_offsets.numel()} entries: more runs than the {N} keyframes")
-        if n_runs is not None and n_runs != run_offsets.numel() - 1:
-            raise ValueError(f"run_offsets has {run_offsets.numel()} entries, not n_runs + 1 = {n_runs + 1}")
-    with _on(dev, stream):
-        C, offs, S = _chain_layout(run_offsets, dev, n_states=N, n_chains=n_runs)
-        nt = N - C
-        if C < 1 or nt < 0:
-            raise ValueError(f"{C} runs over {N} keyframes: every run holds a keyframe")
-        if records.numel() != nt * REC_DOUBLES[model] or lin.numel() != 13 * nt:
-            raise ValueError(f"{N - C} transitions need records [{nt},{REC_DOUBLES[model]}] and lin [{nt},13]")
-        states, cov = states.contiguous(), cov.contiguous()
-        if nt:
-            idx_i, _ = _chain_factor_states(C, offs, S, nt, dev)
-            xp, cp, cr = propagate(model, states, cov, records, lin, anchor=idx_i, want_cross=True, stream=stream)
-        else:
-            xp = cp = cr = None
-        f64 = dict(dtype=torch.float64, device=dev)
-        xs, cs = torch.empty((N, 16), **f64), torch.empty((N, 225), **f64)
-        xc = torch.empty((nt, 225), **f64) if cross else None
-        _launch(capi.load().cpi_rts_smooth_batch, dev, stream, C, _tptr(offs), S, N, _tptr(states), _tptr(cov), _tptr(xp), _tptr(cp),
-                _tptr(cr), _tptr(xs), _tptr(cs), _tptr(xc))
-    return xs, cs, xc
+    return _rts_smooth(False, model, states, cov, records, lin, run_offsets, cross, n_runs, stream)
 
 
 def rts_smooth_scan(model, states, cov, records, lin, run_offsets, cross=False, n_runs=None, stream=None):
@@ -1369,20 +1318,27 @@ def rts_smooth_scan(model, states, cov, records, lin, run_offsets, cross=False, 
     workspace (cpi_rts_smooth_scan_workspace bytes: about 5.5 KB per keyframe) on the stream's device.  Enqueues on ``stream``
     (default: torch's current stream) without synchronising.  Returns (states_s [N,16], cov_s [N,225] exactly symmetric, cross_s
     [N - n_runs,225] or None)."""
+    return _rts_smooth(True, model, states, cov, records, lin, run_offsets, cross, n_runs, stream)
+
+
+def _rts_smooth(scan, model, states, cov, records, lin, run_offsets, cross, n_runs, stream):
+    """rts_smooth (K15) or, scan True, rts_smooth_scan (K16): the checks, the run layout, the K7 pass, the outputs, the scan's
+    workspace and the launch."""
     import torch
 
+    name = "rts_smooth_scan" if scan else "rts_smooth"
     if model not in (1, 2):
         raise ValueError(f"model must be 1 or 2 (got {model!r})")
-    for name, t in (("states", states), ("cov", cov), ("records", records), ("lin", lin)):
+    for what, t in (("states", states), ("cov", cov), ("records", records), ("lin", lin)):
         if not isinstance(t, torch.Tensor):
-            raise ValueError(f"{name} must be a tensor")
+            raise ValueError(f"{what} must be a tensor")
     if not states.is_cuda:
         raise ValueError("states must be a CUDA tensor")
     dev = states.device
     _check_f64(dev, states=states, cov=cov, records=records, lin=lin)
     N = states.numel() // 16
     if N < 1 or states.numel() != 16 * N or cov.numel() != 225 * N:
-        raise ValueError("rts_smooth_scan needs states [N,16] and cov [N,225] with at least one keyframe")
+        raise ValueError(f"{name} needs states [N,16] and cov [N,225] with at least one keyframe")
     if isinstance(run_offsets, torch.Tensor):
         if run_offsets.numel() - 1 > N:
             raise ValueError(f"run_offsets has {run_offsets.numel()} entries: more runs than the {N} keyframes")
@@ -1400,14 +1356,17 @@ def rts_smooth_scan(model, states, cov, records, lin, run_offsets, cross=False, 
         if nt:
             idx_i, _ = _chain_factor_states(C, offs, S, nt, dev)
             xp, cp, cr = propagate(model, states, cov, records, lin, anchor=idx_i, want_cross=True, stream=stream)
-            ws = torch.empty(int(lib.cpi_rts_smooth_scan_workspace(C, N)), dtype=torch.uint8, device=dev)
+            ws = torch.empty(int(lib.cpi_rts_smooth_scan_workspace(C, N)), dtype=torch.uint8, device=dev) if scan else None
         else:
             xp = cp = cr = ws = None
         f64 = dict(dtype=torch.float64, device=dev)
         xs, cs = torch.empty((N, 16), **f64), torch.empty((N, 225), **f64)
         xc = torch.empty((nt, 225), **f64) if cross else None
-        _launch(lib.cpi_rts_smooth_scan_batch, dev, stream, C, _tptr(offs), S, N, _tptr(states), _tptr(cov), _tptr(xp), _tptr(cp),
-                _tptr(cr), _tptr(xs), _tptr(cs), _tptr(xc), _tptr(ws))
+        args = (C, _tptr(offs), S, N, _tptr(states), _tptr(cov), _tptr(xp), _tptr(cp), _tptr(cr), _tptr(xs), _tptr(cs), _tptr(xc))
+        if scan:
+            _launch(lib.cpi_rts_smooth_scan_batch, dev, stream, *args, _tptr(ws))
+        else:
+            _launch(lib.cpi_rts_smooth_batch, dev, stream, *args)
     return xs, cs, xc
 
 
@@ -1431,7 +1390,7 @@ def _filter_checks(states, cov, gate, name):
         if gate.numel() != n:
             raise ValueError(f"gate needs one entry per filter ({n}), got {gate.numel()}")
     elif gate is not None and math.isnan(float(gate)):
-        raise ValueError("gate must not be NaN (+inf applies every measurement)")
+        raise ValueError("gate must not be NaN (+inf applies every update)")
     return dev, n
 
 
@@ -1442,7 +1401,7 @@ def _filter_gate(gate, n, f64):
     if isinstance(gate, torch.Tensor):
         gate = gate.contiguous()
         if bool(torch.isnan(gate).any()):
-            raise ValueError("gate must not be NaN (+inf applies every measurement)")
+            raise ValueError("gate must not be NaN (+inf applies every update)")
     elif gate is not None:
         gate = torch.full((n,), float(gate), **f64)
     return gate
