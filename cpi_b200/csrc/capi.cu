@@ -665,6 +665,30 @@ int cpi_imu_chains_marginals(int64_t n_chains, const int64_t* chain_offsets, int
     return CPI_OK;
 }
 
+int64_t cpi_imu_chains_pair_covariance_workspace(int64_t n_chains, int64_t n_states) {
+    if (n_chains < 0 || n_states < 0 || n_states < n_chains) return (int64_t)CPI_EINVAL;
+    return cpi::chains_pair_cov_workspace_bytes(n_states);
+}
+
+int cpi_imu_chains_pair_covariance(int64_t n_chains, const int64_t* chain_offsets, int64_t chain_uniform, int64_t n_states, const double* D,
+                                   const double* E, int64_t n_pairs, const int64_t* pair_i, const int64_t* pair_j, double* out, void* workspace,
+                                   void* stream) {
+    int rc = chain_layout_check(n_chains, chain_offsets, chain_uniform, n_states);
+    if (rc) return rc;
+    if (n_pairs < 0) return fail(CPI_EINVAL, "negative count (n_pairs)");
+    if (n_pairs == 0) return CPI_OK;
+    if (n_chains == 0) return fail(CPI_EINVAL, "n_pairs > 0 needs at least one state");
+    if (!D || !workspace || (n_states > 1 && !E) || !pair_i || !pair_j || !out) return fail(CPI_EINVAL, "null pointer argument");
+    if ((rc = check_aliasing({D, E, pair_i, pair_j, workspace}, {out}))) return rc;
+    DevInfo d;
+    if ((rc = device_info(d))) return rc;
+    int launches = 0;
+    CU(cpi::chains_pair_cov_launch(n_chains, chain_offsets, chain_uniform, n_states, D, E, n_pairs, pair_i, pair_j, out, (double*)workspace, d.sms,
+                                   (cudaStream_t)stream, &launches));
+    g_launches += launches;
+    return CPI_OK;
+}
+
 int64_t cpi_imu_chains_lm_workspace(int64_t n_states) { return n_states < 0 ? (int64_t)CPI_EINVAL : cpi::lm_workspace_bytes(n_states); }
 
 int cpi_imu_chains_lm_update(int64_t n_chains, const int64_t* chain_offsets, int64_t chain_uniform, int64_t n_states, const cpi_lm_params* params,

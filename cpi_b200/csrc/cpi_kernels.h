@@ -74,6 +74,11 @@ cudaError_t chains_solve_launch(int64_t n_chains, const int64_t* offs, int64_t u
 int64_t chains_marginals_workspace_bytes(int64_t n_states);
 cudaError_t chains_marginals_launch(int64_t n_chains, const int64_t* offs, int64_t uniform, int64_t n_states, const double* D, const double* E,
                                     double* cov, double* cross, double* ws, int sms, cudaStream_t st, int* launches);
+// any blocks Sigma_ij of the inverse by a walk up the same levels (cpi_imu_chains_pair_covariance)
+int64_t chains_pair_cov_workspace_bytes(int64_t n_states);
+cudaError_t chains_pair_cov_launch(int64_t n_chains, const int64_t* offs, int64_t uniform, int64_t n_states, const double* D, const double* E,
+                                   int64_t n_pairs, const int64_t* pi, const int64_t* pj, double* out, double* ws, int sms, cudaStream_t st,
+                                   int* launches);
 // merge.cu: one merged model-1 record per group (dtype 64 or 32)
 cudaError_t merge_launch(int dtype, int64_t n_groups, const int64_t* offsets, int64_t uniform, const void* records, const void* lin,
                          void* out, cudaStream_t st);

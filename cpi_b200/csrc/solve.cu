@@ -410,6 +410,154 @@ __global__ void __launch_bounds__(128) k_bcr_selinv_iso(int64_t m, int64_t strid
     }
 }
 
+// ---- pair covariances: any block Sigma_ij of the inverse (cpi_imu_chains_pair_covariance) --------------------------------------------
+// Odd node x of level l is, given the level's other nodes, x = K- x_{x-1} + K+ x_{x+1} + w with K- = -Lc^-T Za, K+ = -Lc^-T Zb and
+// Cov(w) = Lc^-T Lc^-1 (a neighbour of another chain has no term).  Sigma_ij = R + sum_{a in A, b in B} C_a Sigma_ab D_b^T starts at
+// A = {i}, B = {j}, C = D = I, R = 0; each level replaces every node of A and B it eliminates by its neighbours (C_nbr += C_x K-/+),
+// adding C_x Lc^-T Lc^-1 D_x^T to R first where x is in both; at the root R += C_0 Sigma_root D_0^T.  A holds the level's nodes that
+// bracket i, so at most two, level-local a0 and a0 + 1 with a0 = i >> l (likewise B); exactly one of them is odd.  A chain other than
+// chain 0 never reaches the root: its brackets empty out at some level, and the walk stops there.
+struct PairWalk { int nl; int64_t m[64]; const double *Lc[64], *Za[64], *Zb[64]; };
+
+// One warp per pair, grid-stride over the pairs.  Lanes 0..14 hold rows of side A's matrices (i), lanes 15..29 those of side B (j).
+__global__ void __launch_bounds__(64) k_bcr_pair_cov(PairWalk w, int64_t n_states, const int64_t* cid, const double* root, int64_t n_pairs,
+                                                     const int64_t* pi, const int64_t* pj, double* out) {
+    __shared__ double sL[2][2][15 * 16];       // [warp][side] Lc of the side's eliminated node
+    __shared__ double sZ[2][2][2][225];        // [warp][side][Za | Zb] (column-major), Sigma_root in [warp][0][0] at the end
+    __shared__ double sC[2][2][2][225];        // [warp][side][slot] C (side A) or D (side B) of bracket node a0 + slot, row-major
+    __shared__ double sR[2][225];              // [warp] R, row-major
+    const int wib = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int s = lane >= 15, r = lane - 15 * s; // lane < 30: side s, row r
+    double* R = sR[wib];
+    for (int64_t p = (int64_t)blockIdx.x * 2 + wib; p < n_pairs; p += (int64_t)gridDim.x * 2) {
+        const int64_t i = pi[p], j = pj[p];
+        double* o = out + p * 225;
+        if (i < 0 || i >= n_states || j < 0 || j >= n_states || cid[i] != cid[j]) {
+            const double v = (i < 0 || i >= n_states || j < 0 || j >= n_states) ? __longlong_as_double(0x7ff8000000000000ll) : 0.0;
+            for (int k = lane; k < 225; k += 32) o[k] = v;
+            continue;
+        }
+        int64_t a0[2] = {i, j};
+        bool live[2][2] = {{true, false}, {true, false}};
+        for (int k = lane; k < 225; k += 32) {
+            const double e = (k % 16 == 0) ? 1.0 : 0.0;            // k = r * 15 + c is diagonal when k % 16 == 0
+            sC[wib][0][0][k] = e; sC[wib][1][0][k] = e; R[k] = 0.0;
+        }
+        int l = 0;
+        for (; l < w.nl; l++) {
+            if (!(live[0][0] || live[0][1]) || !(live[1][0] || live[1][1])) break;
+            const int64_t m = w.m[l], stride = (int64_t)1 << l;
+            int os[2];
+            int64_t x[2];
+            bool ex[2], hl[2], hr[2];
+#pragma unroll
+            for (int q = 0; q < 2; q++) {
+                os[q] = (a0[q] & 1) ? 0 : 1;                          // the slot holding the level's odd bracket node
+                x[q] = a0[q] + os[q];
+                ex[q] = live[q][os[q]];
+                const int64_t cx = ex[q] ? cid[x[q] * stride] : 0;
+                hl[q] = ex[q] && cid[(x[q] - 1) * stride] == cx;
+                hr[q] = ex[q] && x[q] + 1 < m && cid[(x[q] + 1) * stride] == cx;
+            }
+            __syncwarp();
+#pragma unroll
+            for (int q = 0; q < 2; q++) {
+                if (!ex[q]) continue;
+                const int64_t t = x[q] >> 1;
+                for (int k = lane; k < 225; k += 32) {
+                    const int rr = k % 15, cc = k / 15;
+                    if (rr >= cc) sL[wib][q][rr * 16 + cc] = w.Lc[l][t * 225 + k];
+                    if (hl[q]) sZ[wib][q][0][k] = w.Za[l][t * 225 + k];
+                    if (hr[q]) sZ[wib][q][1][k] = w.Zb[l][t * 225 + k];
+                }
+            }
+            __syncwarp();
+            // row r of Y = C_x Lc^-T (Lc Y^T = C_x^T), kept in place of C_x for the shared-node term
+            const int os_s = s ? os[1] : os[0];                        // this lane's side, selected without a local-memory index
+            const bool act = lane < 30 && (s ? ex[1] : ex[0]);
+            const bool hl_s = s ? hl[1] : hl[0], hr_s = s ? hr[1] : hr[0];
+            const bool live_s[2] = {s ? live[1][0] : live[0][0], s ? live[1][1] : live[0][1]};
+            double* Cx = sC[wib][s][os_s];
+            double y[15];
+            if (act) {
+#pragma unroll
+                for (int q = 0; q < 15; q++) y[q] = Cx[r * 15 + q];
+                fwd15(sL[wib][s], y);
+#pragma unroll
+                for (int q = 0; q < 15; q++) Cx[r * 15 + q] = y[q];
+            }
+            __syncwarp();
+            if (ex[0] && ex[1] && x[0] == x[1]) {                  // x in A and B: R += Y_A Y_B^T
+                const double *YA = sC[wib][0][os[0]], *YB = sC[wib][1][os[1]];
+                for (int k = lane; k < 225; k += 32) {
+                    const int rr = k / 15, cc = k % 15;
+                    double v = R[k];
+#pragma unroll
+                    for (int q = 0; q < 15; q++) v = fma(YA[rr * 15 + q], YB[cc * 15 + q], v);
+                    R[k] = v;
+                }
+            }
+            __syncwarp();
+            // the neighbours: slot 0 (node a0 or a0 - 1) takes -Y Za, slot 1 (node a0 + 1 or a0 + 2) takes -Y Zb; the slot that held x is
+            // replaced, the other accumulated into
+            if (act) {
+#pragma unroll
+                for (int q = 0; q < 2; q++) {
+                    if (!(q ? hr_s : hl_s)) continue;
+                    const double* Z = sZ[wib][s][q];
+                    double* dst = sC[wib][s][q] + r * 15;
+                    const bool acc = q != os_s && live_s[q];
+#pragma unroll
+                    for (int c = 0; c < 15; c++) {
+                        double v = acc ? dst[c] : 0.0;
+#pragma unroll
+                        for (int k = 0; k < 15; k++) v = fma(-y[k], Z[k + 15 * c], v);
+                        dst[c] = v;
+                    }
+                }
+            }
+#pragma unroll
+            for (int q = 0; q < 2; q++) {
+                if (ex[q]) {
+                    live[q][0] = os[q] == 0 ? hl[q] : (live[q][0] || hl[q]);
+                    live[q][1] = os[q] == 1 ? hr[q] : (live[q][1] || hr[q]);
+                }
+                a0[q] >>= 1;
+            }
+            __syncwarp();
+        }
+        if (l == w.nl && live[0][0] && live[1][0]) {               // both brackets reached the root (node 0): R += C_0 Sigma_root D_0^T
+            double* S = sZ[wib][0][0];
+            for (int k = lane; k < 225; k += 32) S[k] = root[k];
+            __syncwarp();
+            if (lane < 15) {
+                const double *CA = sC[wib][0][0], *CB = sC[wib][1][0];
+                double t[15];
+#pragma unroll
+                for (int c = 0; c < 15; c++) {
+                    double v = 0.0;
+#pragma unroll
+                    for (int q = 0; q < 15; q++) v = fma(CA[lane * 15 + q], S[q + 15 * c], v);
+                    t[c] = v;
+                }
+#pragma unroll
+                for (int c = 0; c < 15; c++) {
+                    double v = R[lane * 15 + c];
+#pragma unroll
+                    for (int q = 0; q < 15; q++) v = fma(t[q], CB[c * 15 + q], v);
+                    R[lane * 15 + c] = v;
+                }
+            }
+        }
+        __syncwarp();
+        for (int k = lane; k < 225; k += 32) {                      // column-major; Sigma_ii as its lower triangle mirrored
+            const int rr = k % 15, cc = k / 15;
+            o[k] = (i == j && rr < cc) ? R[rr + 15 * cc] : R[rr * 15 + cc];
+        }
+        __syncwarp();
+    }
+}
+
 // ---- launchers ----------------------------------------------------------------------------------------------------------------------
 cudaError_t whiten_launch(int rd, int64_t n, const double* records, const double* e, const double* H1, const double* H2, double* A1, double* A2, double* b, cudaStream_t st) {
     if (n == 0) return cudaSuccess;
@@ -475,8 +623,9 @@ static void bcr_forward(const BcrLevel* lv, int nl, const double* D, const doubl
 }
 // What follows the levels (offsets in doubles): the solve's chain id of every state (int64), then the selected inversion's
 // zero right-hand side [n_states, 15] for the forward phase and the neighbour blocks Sigma_{k,k+1} of every level l >= 1 with two nodes
-// or more (m_l - 1 blocks each, level order).  solve_end / selinv_end: the doubles the solve / the selected inversion take.
-struct BcrTail { int64_t cid, solve_end, b0, nbr[64], selinv_end; };
+// or more (m_l - 1 blocks each, level order), then the pair covariances' Sigma_root (225).  solve_end / selinv_end / pair_end: the doubles
+// the solve / the selected inversion / the pair covariances take.
+struct BcrTail { int64_t cid, solve_end, b0, nbr[64], selinv_end, root, pair_end; };
 static BcrTail bcr_tail(int64_t n_states, const BcrLevel* lv, int nl) {
     BcrTail t;
     t.cid = bcr_doubles(n_states);
@@ -484,7 +633,8 @@ static BcrTail bcr_tail(int64_t n_states, const BcrLevel* lv, int nl) {
     int64_t p = t.b0 + n_states * 15;
     for (int l = 0; l < 64; l++) t.nbr[l] = -1;
     for (int l = 1; l < nl; l++) { t.nbr[l] = p; p += (lv[l].m - 1) * 225; }
-    t.selinv_end = p;
+    t.selinv_end = t.root = p;
+    t.pair_end = t.root + 225;
     return t;
 }
 static BcrTail bcr_tail(int64_t n_states) {
@@ -545,6 +695,40 @@ cudaError_t chains_marginals_launch(int64_t n_chains, const int64_t* offs, int64
                                                                nbr[l + 1], cov, nbr[l], l ? nullptr : cross);
     }
     if (launches) *launches = 3 * nl + 2;
+    return cudaGetLastError();
+}
+
+// the pair covariances' workspace: the selected inversion's, then Sigma_root
+int64_t chains_pair_cov_workspace_bytes(int64_t n_states) { return bcr_tail(n_states).pair_end * 8; }
+
+// The chain ids, the forward phase on a zero right-hand side (as chains_marginals_launch), Sigma_root, then one walk per pair.
+cudaError_t chains_pair_cov_launch(int64_t n_chains, const int64_t* offs, int64_t uniform, int64_t n_states, const double* D, const double* E,
+                                   int64_t n_pairs, const int64_t* pi, const int64_t* pj, double* out, double* ws, int sms, cudaStream_t st,
+                                   int* launches) {
+    if (launches) *launches = 0;
+    if (n_pairs == 0) return cudaSuccess;
+    BcrLevel lv[64];
+    int64_t end;
+    const int nl = bcr_levels(n_states, lv, &end);
+    const BcrTail tail = bcr_tail(n_states, lv, nl);
+    int64_t* cid = reinterpret_cast<int64_t*>(ws + tail.cid);
+    double* b0 = ws + tail.b0;
+    cudaError_t e = cudaMemsetAsync(b0, 0, (size_t)n_states * 15 * 8, st);
+    if (e != cudaSuccess) return e;
+    const int64_t blocks = (n_states + 255) / 256, cap = (int64_t)sms * 8;
+    k_chain_ids<<<(int)(blocks < cap ? blocks : cap), 256, 0, st>>>(n_chains, offs, uniform, n_states, cid);
+    bcr_forward(lv, nl, D, E, b0, ws, cid, st);
+    k_bcr_selinv_root<<<1, 32, 0, st>>>(nl ? ws + lv[nl - 1].D : D, ws + tail.root);
+    PairWalk w;
+    w.nl = nl;
+    for (int l = 0; l < nl; l++) { w.m[l] = lv[l].m; w.Lc[l] = ws + lv[l].Lc; w.Za[l] = ws + lv[l].Za; w.Zb[l] = ws + lv[l].Zb; }
+    // one pass of resident CTAs (five per SM on sm_90: 40 080 B of static shared memory each), striding over the pairs
+    int per_sm = 0;
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_bcr_pair_cov, 64, 0);
+    if (e != cudaSuccess) return e;
+    const int64_t ctas = (n_pairs + 1) / 2, pcap = (int64_t)sms * (per_sm > 0 ? per_sm : 1);
+    k_bcr_pair_cov<<<(int)(ctas < pcap ? ctas : pcap), 64, 0, st>>>(w, n_states, cid, ws + tail.root, n_pairs, pi, pj, out);
+    if (launches) *launches = 2 * nl + 3;
     return cudaGetLastError();
 }
 

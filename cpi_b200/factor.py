@@ -897,6 +897,23 @@ def chains_covariance(D, E, chain_offsets, cross=False, n_chains=None, workspace
     with cross, [N - n_chains, 225] with chain c's slot o[c] - c + j = (A^-1)_{o[c]+j, o[c]+j+1}, the factors' order; else None)."""
     import torch
 
+    N = _inverse_checks(D, E, chain_offsets, n_chains, workspace)
+    lib = capi.load()
+    dev = D.device
+    with _on(dev, stream):
+        C, offs, S = _chain_layout(chain_offsets, dev, n_states=N, n_chains=n_chains)
+        workspace = _inverse_workspace(lib, "cpi_imu_chains_marginals_workspace", C, N, dev, D, E, workspace)
+        cov = torch.empty((N, 225), dtype=torch.float64, device=dev)
+        cr = torch.empty((N - C, 225), dtype=torch.float64, device=dev) if cross else None
+        _launch(lib.cpi_imu_chains_marginals, dev, stream, C, _tptr(offs), S, N, _tptr(D.contiguous()), _tptr(None if E is None else E.contiguous()),
+                _tptr(cov), _tptr(cr), _tptr(workspace))
+    return cov, cr
+
+
+def _inverse_checks(D, E, chain_offsets, n_chains, workspace):
+    """The host-side checks of chains_covariance and chains_pair_covariance on the system and its layout; returns N."""
+    import torch
+
     for name, t in (("D", D), ("E", E), ("workspace", workspace)):
         if t is not None and (not isinstance(t, torch.Tensor) or t.dtype != torch.float64):
             raise ValueError(f"{name} must be a float64 tensor")
@@ -907,23 +924,68 @@ def chains_covariance(D, E, chain_offsets, cross=False, n_chains=None, workspace
         raise ValueError(f"chain_offsets has {chain_offsets.numel()} entries: more chains than the {N} states")
     if isinstance(chain_offsets, torch.Tensor) and n_chains is not None and n_chains != chain_offsets.numel() - 1:
         raise ValueError(f"chain_offsets has {chain_offsets.numel()} entries, not n_chains + 1 = {n_chains + 1}")
-    lib = capi.load()
+    return N
+
+
+def _inverse_workspace(lib, ws_name, C, N, dev, D, E, workspace):
+    """The workspace of C chains over N states that the C ABI's ws_name sizes: the caller's, checked, or a new one; D, E and the
+    workspace checked to be float64 tensors on dev."""
+    import torch
+
+    nbytes = int(getattr(lib, ws_name)(C, N))
+    if nbytes < 0:
+        raise ValueError(f"{C} chains over {N} states: every chain holds a state")
+    if workspace is not None and (workspace.numel() * 8 < nbytes or not workspace.is_contiguous()):
+        raise ValueError(f"workspace needs {nbytes} contiguous bytes ({ws_name}), got {workspace.numel() * 8}")
+    _check_f64(dev, D=D, E=E, workspace=workspace)
+    if workspace is None:
+        workspace = torch.empty((nbytes + 7) // 8, dtype=torch.float64, device=dev)
+    return workspace
+
+
+def chains_pair_covariance(D, E, chain_offsets, pairs, n_chains=None, workspace=None, stream=None):
+    """Any blocks of A^-1, A = tridiag(E^T, D, E) the system chains_covariance inverts (cpi_imu_chains_pair_covariance; DESIGN.md
+    section 3q): GTSAM's Marginals::jointMarginalCovariance for pairs of keyframes.  D, E, chain_offsets, n_chains and the workspace
+    (cpi_imu_chains_pair_covariance_workspace bytes) as chains_covariance.  pairs: int64 [q,2] of global state indices (i, j), a CUDA
+    tensor on D's device (an index outside [0, N) gives a NaN block) or numpy (range-checked here, then copied to the device from
+    pageable memory: the call then waits for `stream`, as the numpy paths of retract and predict_state do).  Returns [q,225]: row p is
+    (A^-1)_{i,j}, column-major; (A^-1)_{j,i} is its transpose, a pair (i, i) is exactly symmetric, a pair of states in different chains
+    is exactly 0.  GTSAM's 30x30 joint of keyframes {i, j} is the pairs (i, i), (j, j), (i, j)."""
+    import torch
+
+    N = _inverse_checks(D, E, chain_offsets, n_chains, workspace)
     dev = D.device
+    if isinstance(pairs, torch.Tensor):
+        if not pairs.is_cuda or pairs.device != dev or pairs.dtype != torch.int64 or pairs.dim() != 2 or pairs.shape[1] != 2:
+            raise ValueError(f"pairs must be an int64 CUDA tensor [q,2] on {dev}, or numpy")
+    else:
+        pairs = np.asarray(pairs)
+        if pairs.dtype.kind not in "iu" or pairs.ndim != 2 or pairs.shape[1] != 2:
+            raise ValueError("pairs must be integer [q,2]")
+        if pairs.size and (pairs.min() < 0 or pairs.max() >= N):
+            raise ValueError(f"pairs index the states 0 .. {N - 1}")
+    lib = capi.load()
     with _on(dev, stream):
         C, offs, S = _chain_layout(chain_offsets, dev, n_states=N, n_chains=n_chains)
-        nbytes = int(lib.cpi_imu_chains_marginals_workspace(C, N))
-        if nbytes < 0:
-            raise ValueError(f"{C} chains over {N} states: every chain holds a state")
-        if workspace is not None and (workspace.numel() * 8 < nbytes or not workspace.is_contiguous()):
-            raise ValueError(f"workspace needs {nbytes} contiguous bytes (cpi_imu_chains_marginals_workspace), got {workspace.numel() * 8}")
-        _check_f64(dev, D=D, E=E, workspace=workspace)
-        if workspace is None:
-            workspace = torch.empty((nbytes + 7) // 8, dtype=torch.float64, device=dev)
-        cov = torch.empty((N, 225), dtype=torch.float64, device=dev)
-        cr = torch.empty((N - C, 225), dtype=torch.float64, device=dev) if cross else None
-        _launch(lib.cpi_imu_chains_marginals, dev, stream, C, _tptr(offs), S, N, _tptr(D.contiguous()), _tptr(None if E is None else E.contiguous()),
-                _tptr(cov), _tptr(cr), _tptr(workspace))
-    return cov, cr
+        workspace = _inverse_workspace(lib, "cpi_imu_chains_pair_covariance_workspace", C, N, dev, D, E, workspace)
+        if not isinstance(pairs, torch.Tensor):
+            pairs = torch.from_numpy(np.ascontiguousarray(pairs, dtype=np.int64)).to(dev)
+        q = pairs.shape[0]
+        out = torch.empty((q, 225), dtype=torch.float64, device=dev)
+        _launch(lib.cpi_imu_chains_pair_covariance, dev, stream, C, _tptr(offs), S, N, _tptr(D.contiguous()),
+                _tptr(None if E is None else E.contiguous()), q, _tptr(pairs[:, 0].contiguous()), _tptr(pairs[:, 1].contiguous()), _tptr(out),
+                _tptr(workspace))
+    return out
+
+
+def _marginal_system(model, states, records, lin, chain_offsets, prior, stream, state_priors, state_prior_loss, measurements,
+                     measurement_loss):
+    """What chains_marginals and chains_pair_marginals invert: the linearisation of chains_lm_step at `states`, assembled with
+    lambda = 0.  Returns (n_chains, D, E).  Its callers run it under _on(dev, stream)."""
+    (C, _, _), _, (G11, G12, G22, g1, g2, _), (pi_a, pr_c, _) = _linearized(model, states, records, lin, chain_offsets, prior, stream,
+                                                                            state_priors, state_prior_loss, measurements, measurement_loss)
+    D, E, _ = chains_assemble(G11, G12, G22, g1, g2, chain_offsets, 0.0, pi_a, pr_c, n_chains=C, stream=stream)
+    return C, D, E
 
 
 def chains_marginals(model, states, records, lin, chain_offsets, prior=None, state_priors=None, state_prior_loss=None, cross=False, stream=None,
@@ -935,10 +997,21 @@ def chains_marginals(model, states, records, lin, chain_offsets, prior=None, sta
     without priors on later states are numerically singular in fp64: their covariances are meaningless.  Returns (cov [N,225],
     cross [N - n_chains,225] or None) as chains_covariance, in the tangent space of retract at the states."""
     with _on(states.device, stream):
-        (C, _, _), _, (G11, G12, G22, g1, g2, _), (pi_a, pr_c, _) = _linearized(model, states, records, lin, chain_offsets, prior, stream,
-                                                                                state_priors, state_prior_loss, measurements, measurement_loss)
-        D, E, _ = chains_assemble(G11, G12, G22, g1, g2, chain_offsets, 0.0, pi_a, pr_c, n_chains=C, stream=stream)
+        C, D, E = _marginal_system(model, states, records, lin, chain_offsets, prior, stream, state_priors, state_prior_loss, measurements,
+                                   measurement_loss)
         return chains_covariance(D, E, chain_offsets, cross=cross, n_chains=C, stream=stream)
+
+
+def chains_pair_marginals(model, states, records, lin, chain_offsets, pairs, prior=None, state_priors=None, state_prior_loss=None,
+                          measurements=None, measurement_loss=None, stream=None):
+    """Joint marginal covariances of pairs of keyframes of many IMU chains at the states (GTSAM's Marginals::jointMarginalCovariance;
+    DESIGN.md section 3q): the system chains_marginals inverts, then chains_pair_covariance on `pairs` (int64 [q,2] of global state
+    indices, a CUDA tensor or numpy; numpy pairs make the call wait for `stream`, as in chains_pair_covariance).  Arguments otherwise
+    as chains_marginals.  Returns [q,225] as chains_pair_covariance, in the tangent spaces of retract at the states."""
+    with _on(states.device, stream):
+        C, D, E = _marginal_system(model, states, records, lin, chain_offsets, prior, stream, state_priors, state_prior_loss, measurements,
+                                   measurement_loss)
+        return chains_pair_covariance(D, E, chain_offsets, pairs, n_chains=C, stream=stream)
 
 
 def chains_lm(model, states, records, lin, chain_offsets, prior=None, lam=1e-5, diagonal_damping=True, params=None, max_rounds=200, check_every=8,

@@ -505,6 +505,29 @@ int cpi_imu_chains_marginals(int64_t n_chains, const int64_t* chain_offsets, int
                              const double* D, const double* E, double* cov, double* cross, void* workspace, void* stream);
 
 /*
+ * Any blocks of the inverse of many chains (DESIGN.md section 3q): GTSAM's Marginals::jointMarginalCovariance for any two keyframes of
+ * a chain, for many pairs at once.  fp64, DEVICE pointers, asynchronous on `stream`, no allocation.  PARITY UNPINNED;
+ * tests/pair_cov_ref.py holds the numpy statement of the walk.
+ *
+ *   cpi_imu_chains_pair_covariance   out[p] = (A^-1)_{pair_i[p], pair_j[p]} (device double[n_pairs*225], column-major) for the system
+ *       A of cpi_imu_chains_marginals (same layout, same validation, same error codes); pair_i, pair_j: device int64[n_pairs] of global
+ *       state indices, in either order ((A^-1)_{j,i} = (A^-1)_{i,j}^T).  A pair (i, i) gives Sigma_ii exactly symmetric (its lower
+ *       triangle mirrored).  A pair of states in different chains gives exact 0; an index outside [0, n_states) gives a NaN block and
+ *       reads nothing.  The forward phase of cpi_imu_chains_solve on a zero right-hand side and Sigma_root = D_root^-1, then one warp
+ *       per pair walks up the levels: O(log2 n_states) 15x15 steps per pair (2 log2(n_states) + 3 launches in all; none when n_pairs
+ *       is 0).  Every coupling between two chains is structurally absent: a chain that is not SPD gets NaN blocks, and only that chain.
+ *       CPI_EINVAL for a negative n_pairs, n_pairs > 0 without a state, a NULL pair_i, pair_j or out with n_pairs > 0, and an out
+ *       equal to D, E, pair_i, pair_j or the workspace.  workspace: cpi_imu_chains_pair_covariance_workspace(n_chains, n_states) bytes.
+ *   GTSAM's 30x30 joint of keyframes {i, j} is the pairs (i, i), (j, j), (i, j) of one call.  As cpi_imu_chains_marginals, the call
+ *   inverts whatever system it is given (factor.chains_pair_marginals assembles the undamped one), and long IMU-only chains without
+ *   priors on later states are numerically singular in fp64: their covariances are meaningless (finite or not).
+ */
+int64_t cpi_imu_chains_pair_covariance_workspace(int64_t n_chains, int64_t n_states);
+int cpi_imu_chains_pair_covariance(int64_t n_chains, const int64_t* chain_offsets, int64_t chain_uniform, int64_t n_states,
+                                   const double* D, const double* E, int64_t n_pairs, const int64_t* pair_i, const int64_t* pair_j,
+                                   double* out, void* workspace, void* stream);
+
+/*
  * Re-preintegration of the windows whose bias estimate left the records' linearisation point (DESIGN.md section 3i): the
  * re-integration VINS-Mono and OKVIS run between solves, on the device.  A factor corrects its record to the bias of its state i
  * only to first order (J_q, J_a, J_b, H_a, H_b; model 2 also O_a, O_b in the orientation), which limits accuracy once the
